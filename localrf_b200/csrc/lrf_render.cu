@@ -9,7 +9,7 @@
 // One persistent CTA per SM, 16 warps (512 threads; LRF_THREADS) in two roles that only meet through
 // mbarriers and a few shared-memory counters:
 //
-//   producers (warps 0 .. W_CONS-1: 12)  each takes one ray at a time from a global counter (dynamic
+//   producers (warps 0 .. W_CONS-1: 8)  each takes one ray at a time from a global counter (dynamic
 //       scheduling: no wave quantisation of a 4096-ray batch).  March: lane = sample, 32 samples
 //       per step, transmittance by a warp-shuffle product scan with a carried prefix.  Samples
 //       with w > threshold go to a small per-warp queue whose entries carry their ray slot (so samples of
@@ -18,7 +18,7 @@
 //       A tile in shared memory (K-major 8x8 core matrices).  Rows are handed out by an atomic cursor, so
 //       rays of all producers interleave in a tile; each row carries (ray slot, weight).  Every row arrives
 //       once on the tile's "full" mbarrier (128 arrivals = tile ready).
-//   consumers (the last warpgroup, or two with LRF_CONS_WARPS=8)  per tile, one 64-row half at a time:
+//   consumers (the last two warpgroups, or one with LRF_CONS_WARPS=4)  per tile, one 64-row half each:
 //       layer 1 (A from shared memory, basis folded into W1, K = 80) and layer 2 (A = the bias + ReLU'd
 //       layer-1 accumulator re-split in registers, K = 128) as wgmma m64 bf16 MMAs, three products
 //       hi*hi + hi*lo + lo*hi per K-step, fp32 accumulators in registers; layer 3 (131 -> 3) + sigmoid on
@@ -31,7 +31,10 @@
 // render_kernel_t<true> (fields with positional encodings) inserts a layer 0 (basis_mat as its own product),
 // builds the encoded layer-1 input in registers 64 columns at a time and streams layer 1's weight chunks by TMA.
 // Compile-time experiments kept as switches: LRF_THREADS, LRF_CONS_WARPS, LRF_SPIN_NS,
-// LRF_STEAL.  The weight operands are staged once per CTA by TMA bulk copies (cp.async.bulk -> UBLKCP).
+// LRF_STEAL.  The weight operands are staged once per CTA by TMA bulk copies (cp.async.bulk -> UBLKCP); the
+// sample table is read from global memory through the L1.  The launcher sets the shared-memory carveout to the
+// smallest step that holds the CTA: the default build's folded-MLP layout fits the 196 KB step, which leaves
+// the L1 60 KB for the texel gathers.
 #include <cstdlib>
 
 #include "lrf_device.cuh"
@@ -42,13 +45,14 @@ namespace lrf {
 #define LRF_THREADS 512             // 16 warps (128 registers each); 640 = 20 warps at 96 registers
 #endif
 #ifndef LRF_CONS_WARPS
-#define LRF_CONS_WARPS 4            // 4: one consumer warpgroup takes both halves of a tile; 8: two, one half each
+#define LRF_CONS_WARPS 8            // 8: two consumer warpgroups, one half of a tile each (8 producers); 4: one consumer
+                                    // warpgroup takes both halves (12 producers)
 #endif
 constexpr int THREADS = LRF_THREADS;
 constexpr int N_CONS = LRF_CONS_WARPS;
 constexpr int N_CWG = N_CONS / 4;               // consumer warpgroups
 constexpr int W_CONS = THREADS / 32 - N_CONS;   // the last warps: consumers (whole warpgroups)
-constexpr int MAX_PROD = W_CONS;                // producer warps 0 .. W_CONS-1 (12 at 512 threads / 4 consumers)
+constexpr int MAX_PROD = W_CONS;                // producer warps 0 .. W_CONS-1 (8 at 512 threads / 8 consumers)
 constexpr int XA_LD = 33;                       // (positional encodings) floats per row of the basis-feature buffer
 static_assert(THREADS % 128 == 0 && W_CONS >= 1 && (N_CONS == 4 || N_CONS == 8), "warp roles");
 constexpr int NSLOT = 3;            // ray slots per producer warp
@@ -108,13 +112,13 @@ struct Ctrl {                       // CTA control block in shared memory
 };
 
 struct SmemV3 {
-  int prep, a1, mslot, mw, part, slots, recs, q, alpha, z, ctrl, total;
+  int prep, a1, mslot, mw, part, slots, recs, q, alpha, ctrl, total;
   int per_prod;                     // bytes of one producer's queue (+ alpha table)
 };
 
 constexpr int PE_WBUF = (PE_RESIDENT + 1023) & ~1023;     // offset of the streamed layer-1 chunk inside the prep region
-__host__ __device__ inline SmemV3 smem_v3(int S, bool floater, int nprod, bool pe = false) {
-  SmemV3 L;
+__host__ __device__ constexpr SmemV3 smem_v3(int S, bool floater, int nprod, bool pe = false) {
+  SmemV3 L{};
   int off = 0;
   const int Sp = (S + 3) & ~3;
   L.prep = off;   off += pe ? PE_WBUF + 2 * PE_WC_BYTES : PREP_BYTES;
@@ -132,12 +136,21 @@ __host__ __device__ inline SmemV3 smem_v3(int S, bool floater, int nprod, bool p
   L.per_prod = (L.per_prod + 15) & ~15;
   off += nprod * L.per_prod;
   L.alpha = QCAP * 7 + (16 - (QCAP * 7) % 16) % 16;     // offset of the alpha table inside a producer block
-  L.z = off;      off += (Sp + 4) * 4;
   off = (off + 15) & ~15;
   L.ctrl = off;   off += (int)sizeof(Ctrl);
   L.total = (off + 15) & ~15;
   return L;
 }
+// Hopper's two largest shared-memory carveout steps are 196 and 228 KB, and the SM reserves 1 KB of each CTA's
+// share.  Without the floater filter the layout does not depend on S (the sample table is read from global
+// memory through the L1), so the default build's CTA fits the 196 KB step for every sample table and the L1
+// keeps 60 KB for the texel gathers (28 KB at the 228 KB step).  The LRF_STEAL / LRF_THREADS / LRF_CONS_WARPS
+// experiments may need more.
+constexpr int SMEM_196K_STEP = 196 * 1024 - 1024;
+static_assert(LRF_STEAL || THREADS != 512 || N_CONS != 8 ||
+              (smem_v3(344, false, MAX_PROD).total <= SMEM_196K_STEP &&
+               smem_v3(65535, false, MAX_PROD).total <= SMEM_196K_STEP),
+              "the folded-MLP layout must fit the 196 KB carveout step");
 
 // ---- outputs (local_tensorfs.py:467-497) --------------------------------------------------------
 __device__ __forceinline__ void write_rgb(const BatchDev& B, long long r,
@@ -325,8 +338,8 @@ struct WarpQ {
 // gathers the first n (<= 32) queued samples (each with its own ray, read from its slot) and submits
 // them as tile rows.  Their slots' `pending` counts were raised when the samples were selected.
 template <bool H16>
-__device__ __forceinline__ void flush_rows(const ProdCtx& P, const FieldDev& F, const float* z_s,
-                                           const Slot* slots, const WarpQ& Q, int n) {
+__device__ __forceinline__ void flush_rows(const ProdCtx& P, const FieldDev& F, const Slot* slots,
+                                           const WarpQ& Q, int n) {
   unsigned int start = 0;
   if (P.lane == 0) start = atomicAdd(&P.ctrl->cursor, (unsigned int)n);
   start = __shfl_sync(0xffffffffu, start, 0);
@@ -339,7 +352,7 @@ __device__ __forceinline__ void flush_rows(const ProdCtx& P, const FieldDev& F, 
     R.o[0] = sl->o[0]; R.o[1] = sl->o[1]; R.o[2] = sl->o[2];
     R.vd[0] = sl->vd[0]; R.vd[1] = sl->vd[1]; R.vd[2] = sl->vd[2];
     float p[3], q[3];
-    sample_pos(F, R, z_s[k], p, q);
+    sample_pos(F, R, __ldg(F.z + k), p, q);
     wait_tile_free(P.ctrl, T);
     unsigned char* a_hi = P.smem + P.L->a1 + b * (2 * OPER1_BYTES);
     if constexpr (H16) app_row_bf16(F, q, a_hi, a_hi + OPER1_BYTES, row);
@@ -355,8 +368,8 @@ __device__ __forceinline__ void flush_rows(const ProdCtx& P, const FieldDev& F, 
 // appends the lanes with on == true (mask m = their ballot) to the warp's queue; flushes 32 rows when it
 // holds >= 32.  The caller has already added popc(m) to the slot's pending count.
 template <bool H16>
-__device__ __forceinline__ void queue_push(const ProdCtx& P, const FieldDev& F, const float* z_s,
-                                           const Slot* slots, WarpQ& Q, unsigned m, bool on, int k,
+__device__ __forceinline__ void queue_push(const ProdCtx& P, const FieldDev& F, const Slot* slots,
+                                           WarpQ& Q, unsigned m, bool on, int k,
                                            float wgt, int slot_id) {
   const int lane = P.lane;
   if (on) {
@@ -367,7 +380,7 @@ __device__ __forceinline__ void queue_push(const ProdCtx& P, const FieldDev& F, 
   Q.n_app += __popc(m);
   __syncwarp();
   if (Q.qn >= 32) {
-    flush_rows<H16>(P, F, z_s, slots, Q, 32);
+    flush_rows<H16>(P, F, slots, Q, 32);
     unsigned short tk = 0; float tw = 0.0f; unsigned char ts = 0;
     if (lane < Q.qn - 32) { tk = Q.qk[32 + lane]; tw = Q.qw[32 + lane]; ts = Q.qs[32 + lane]; }
     __syncwarp();
@@ -379,9 +392,8 @@ __device__ __forceinline__ void queue_push(const ProdCtx& P, const FieldDev& F, 
 
 // alpha of sample k of the ray in slot-resident form (tensorBase.py:581-610); counts valid samples
 template <bool H16>
-__device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R, const float* z_s, int k,
-                                              int S, int& marched) {
-  const float z = z_s[k];
+__device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R, int k, int S, int& marched) {
+  const float z = __ldg(F.z + k);
   float p[3], q[3];
   sample_pos(F, R, z, p, q);
   bool valid = (k != S - 1);                                  // ray_valid[:, -1] = 0
@@ -391,7 +403,7 @@ __device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R,
     sigma = feature2density(density_feature_t<H16>(F, q), F.density_shift, F.act);
     ++marched;
   }
-  const float dist = z_s[k + 1] - z;
+  const float dist = (k + 1 < S ? __ldg(F.z + k + 1) : z) - z;    // the last sample's dist is 0 (tensorBase.py:584-587)
   float alpha = 1.0f - expf(-sigma * dist * F.distance_scale);   // tensorBase.py:610, same form
   if (k == S - 1) alpha = 1.0f;                                  // alpha[:, -1] = 1
   return alpha;
@@ -400,7 +412,7 @@ __device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R,
 // One claimed step (32 samples) of the ray described by `rec`: see RayRec.
 template <bool H16>
 __device__ __forceinline__ void process_step(const ProdCtx& P, const FieldDev& F, const BatchDev& B,
-                                             const float* z_s, Slot* slots, RayRec* rec, int s, WarpQ& Q) {
+                                             Slot* slots, RayRec* rec, int s, WarpQ& Q) {
   const int lane = P.lane, S = F.S, k = s * 32 + lane;
   const int slot_id = *reinterpret_cast<volatile int*>(&rec->slot_id);
   const long long ray = *reinterpret_cast<volatile long long*>(&rec->ray);
@@ -411,7 +423,7 @@ __device__ __forceinline__ void process_step(const ProdCtx& P, const FieldDev& F
   const bool skip = (unsigned)s >= *reinterpret_cast<volatile unsigned int*>(&rec->stop_at);
   float alpha = 0.0f;
   int marched = 0;
-  if (!skip && k < S) alpha = sample_alpha<H16>(F, R, z_s, k, S, marched);
+  if (!skip && k < S) alpha = sample_alpha<H16>(F, R, k, S, marched);
   const float f = (k < S) ? (1.0f - alpha) + 1e-10f : 1.0f;
   const float inc = warp_scan_mul(f, lane);
   float exc = __shfl_up_sync(0xffffffffu, inc, 1);
@@ -432,7 +444,7 @@ __device__ __forceinline__ void process_step(const ProdCtx& P, const FieldDev& F
   }
   const bool live = !skip && !(carry < T_EPS);                  // a terminated ray's later steps contribute nothing
   const float wgt = live ? alpha * (carry * exc) : 0.0f;
-  const float zk = (k < S) ? z_s[k] : 0.0f;
+  const float zk = (k < S) ? __ldg(F.z + k) : 0.0f;
   const float acc_s = warp_sum((live && k < S) ? wgt : 0.0f);
   const float dep_s = warp_sum((live && k < S) ? wgt * zk : 0.0f);
   const int marched_s = (int)warp_sum(live ? (float)marched : 0.0f);
@@ -446,7 +458,7 @@ __device__ __forceinline__ void process_step(const ProdCtx& P, const FieldDev& F
     __threadfence_block();
     atomicOr(&rec->done, 1u << s);
   }
-  queue_push<H16>(P, F, z_s, slots, Q, m, on, k, wgt, slot_id);
+  queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
 }
 
 // =================================================================================================
@@ -463,7 +475,6 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
   const SmemV3 L = smem_v3(F.S, floater, nprod, PE);
   Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem + L.ctrl);
   Slot* slots = reinterpret_cast<Slot*>(smem + L.slots);
-  float* z_s = reinterpret_cast<float*>(smem + L.z);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int S = F.S;
 
@@ -482,8 +493,6 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
       tma_bulk_g2s(smem_u32(smem + L.prep) + o, reinterpret_cast<const char*>(F.prep) + o,
                    min(CH, bytes - o), smem_u32(&ctrl->bar_w));
   }
-  for (int k = tid; k < S; k += THREADS) z_s[k] = F.z[k];
-  if (tid == 0) z_s[S] = F.z[S - 1];       // dist of the last sample = 0 (tensorBase.py:584-587)
   for (int e = tid; e < MAX_PROD * NSLOT * (int)sizeof(Slot) / 4; e += THREADS)
     reinterpret_cast<int*>(slots)[e] = 0;
   if (LRF_STEAL && tid < nprod)                                      // no ray open: nothing to claim
@@ -542,7 +551,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
         st = __shfl_sync(0xffffffffu, st, 0);
         if (st == 0) break;
         if (spins == SPIN_PAD) {
-          if (Q.qn > 0) { flush_rows<H16>(P, F, z_s, slots, Q, Q.qn); Q.qn = 0; }
+          if (Q.qn > 0) { flush_rows<H16>(P, F, slots, Q, Q.qn); Q.qn = 0; }
           pad_open_tile(P);
           spins = 0;
         }
@@ -613,7 +622,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
             if (lane == 0) { __threadfence_block(); atomicOr(&rec->ready, mask); atomicOr(&rec->done, mask); }
             break;
           }
-          process_step<H16>(P, F, B, z_s, slots, rec, (int)st, Q);
+          process_step<H16>(P, F, B, slots, rec, (int)st, Q);
         }
         while (*reinterpret_cast<volatile unsigned int*>(&rec->done) != full_mask) { }   // helpers' steps
         __threadfence_block();
@@ -628,7 +637,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
         for (; k0 < S; k0 += 32) {
           const int k = k0 + lane;
           float alpha = 0.0f;
-          if (k < S) alpha = sample_alpha<H16>(F, R, z_s, k, S, marched);
+          if (k < S) alpha = sample_alpha<H16>(F, R, k, S, marched);
           const float f = (k < S) ? (1.0f - alpha) + 1e-10f : 1.0f;
           const float inc = warp_scan_mul(f, lane);
           float exc = __shfl_up_sync(0xffffffffu, inc, 1);
@@ -636,7 +645,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
           const float wgt = alpha * (carry * exc);
           if (k < S) {
             acc_p += wgt;
-            dep_p += wgt * z_s[k];
+            dep_p += wgt * __ldg(F.z + k);
             idx_p += wgt * (float)k;
             if (floater) alpha_s[k] = alpha;
             else if (wo) wo[k] = wgt;
@@ -646,7 +655,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
             const bool on = (k < S) && (wgt > F.weight_thres);          // tensorBase.py:622
             const unsigned m = __ballot_sync(0xffffffffu, on);
             if (lane == 0 && m) atomicAdd(&slot->pending, __popc(m));
-            queue_push<H16>(P, F, z_s, slots, Q, m, on, k, wgt, slot_id);
+            queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
             if (carry < T_EPS) { k0 += 32; break; }                      // early ray termination
           }
         }
@@ -672,7 +681,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
             const bool on = (k < S) && (wgt > F.weight_thres);
             const unsigned m = __ballot_sync(0xffffffffu, on);
             if (lane == 0 && m) atomicAdd(&slot->pending, __popc(m));
-            queue_push<H16>(P, F, z_s, slots, Q, m, on, k, wgt, slot_id);
+            queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
           }
         }
         n_march += (unsigned long long)warp_sum((float)marched);
@@ -704,7 +713,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
             st = __shfl_sync(0xffffffffu, st, 0);
             if (st >= (unsigned)n_steps) break;
             __threadfence_block();
-            process_step<H16>(P, F, B, z_s, slots, other, (int)st, Q);
+            process_step<H16>(P, F, B, slots, other, (int)st, Q);
             any = true;
           }
         }
@@ -714,7 +723,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
         }
       }
     }
-    if (Q.qn > 0) { flush_rows<H16>(P, F, z_s, slots, Q, Q.qn); Q.qn = 0; }
+    if (Q.qn > 0) { flush_rows<H16>(P, F, slots, Q, Q.qn); Q.qn = 0; }
     // -- the last producer completes the open tile and publishes the tile count ----------------------
     if (lane == 0 && B.stats) { atomicAdd(B.stats, n_march); atomicAdd(B.stats + 1, Q.n_app); }
     unsigned int d = 0;
@@ -918,12 +927,28 @@ cudaError_t launch_render(const FieldDev& F, const BatchDev& B, int n_sms, int m
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
+  const void* kern = variant == 1 ? (const void*)render_kernel_t<true, false>
+                   : variant == 2 ? (const void*)render_kernel_t<false, true> : (const void*)render_kernel_t<false, false>;
   if (dev >= 0 && dev < 64 && smem > configured[variant][dev]) {
-    e = variant == 1 ? cudaFuncSetAttribute(render_kernel_t<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-      : variant == 2 ? cudaFuncSetAttribute(render_kernel_t<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                     : cudaFuncSetAttribute(render_kernel_t<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     configured[variant][dev] = smem;
+  }
+  // The shared-memory carveout is the smallest step that holds this launch's CTA, so the L1 gets the rest;
+  // it is the code's choice, not the driver's.  A percentage that is not a step rounds up to the next step.
+  static size_t carved[3][64] = {{0}, {0}, {0}};       // per kernel, per device: the CTA size the carveout was set for
+  if (dev >= 0 && dev < 64 && smem != carved[variant][dev]) {
+    int per_sm = 0, reserved = 0;
+    e = cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
+    if (e != cudaSuccess) return e;
+    static const int steps_kb[] = {0, 8, 16, 32, 64, 100, 132, 164, 196, 228};   // sm_90
+    int pct = 100;
+    for (int kb : steps_kb)
+      if (kb * 1024 >= (int)smem + reserved && kb * 1024 <= per_sm) { pct = (int)(kb * 1024LL * 100 / per_sm); break; }
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+    if (e != cudaSuccess) return e;
+    carved[variant][dev] = smem;
   }
   e = cudaMemsetAsync(B.sched, 0, 2 * sizeof(unsigned long long), stream);   // ray counter + finished-CTA counter
   if (e != cudaSuccess) return e;
