@@ -97,7 +97,7 @@ def build(force=False, verbose=False):
     if not force and not _stale():
         return LIB_PATH
     nvcc = os.environ.get("NVCC", "nvcc")
-    extra = os.environ.get("LRF_NVCC_EXTRA", "").split()          # tuning experiments (e.g. -DLRF_THREADS=640)
+    extra = os.environ.get("LRF_NVCC_EXTRA", "").split()          # extra nvcc flags (e.g. -Xptxas -warn-spills)
     cmd = [nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB_PATH] + SOURCES
     env = dict(os.environ)
     env.pop("CC", None); env.pop("CXX", None)  # the image's CC points at a gcc without libgomp

@@ -94,17 +94,6 @@ __host__ inline size_t bwd_scratch_layout(long long n, int S, BwdScratch* out, u
 
 // ---- small device helpers --------------------------------------------------------------------------
 
-// grid_sample border coordinate with derivative (zero when clipped)
-__device__ __forceinline__ void coord_g(float c, int size, int& i0, int& i1, float& t, float& dc) {
-  float x = ((c + 1.0f) * 0.5f) * (float)(size - 1);
-  dc = (x <= 0.0f || x >= (float)(size - 1)) ? 0.0f : 0.5f * (float)(size - 1);
-  x = fminf((float)(size - 1), fmaxf(x, 0.0f));
-  const float f = floorf(x);
-  i0 = (int)f;
-  i1 = min(i0 + 1, size - 1);
-  t = x - f;
-}
-
 // d contract(p)/dp applied to dpc (ray_utils.py:9-12; amax routes the norm's gradient to the
 // component of largest magnitude)
 __device__ __forceinline__ void contract_bwd(float p0, float p1, float p2, float g0, float g1,
@@ -123,10 +112,6 @@ __device__ __forceinline__ void contract_bwd(float p0, float p1, float p2, float
   const float pj = j == 0 ? p0 : (j == 1 ? p1 : p2);
   const float extra = (pj >= 0.0f ? 1.0f : -1.0f) * ds * dot;
   if (j == 0) o0 += extra; else if (j == 1) o1 += extra; else o2 += extra;
-}
-
-__device__ __forceinline__ void red4g(float* p, float x, float y, float z, float w) {
-  atomicAdd(reinterpret_cast<float4*>(p), make_float4(x, y, z, w));
 }
 
 __device__ __forceinline__ void load_ray(const float* rays, long long ray, RaySm& R) {
@@ -167,7 +152,7 @@ bwd_march_kernel(const FieldDev F, const BwdArgs A) {
         valid = (k != S - 1);                                          // ray_valid[:, -1] = 0
         if (valid && F.alpha_vol) valid = alpha_mask(F, p) > 0.0f;     // tensorBase.py:593-598
         float sigma = 0.0f;
-        if (valid) { fe = density_feature(F, q); sigma = feature2density(fe, F.density_shift, F.act); }
+        if (valid) { fe = density_feature_t<false>(F, q); sigma = feature2density(fe, F.density_shift, F.act); }
         const float znext = (k + 1 < S) ? __ldg(F.z + k + 1) : z;
         alpha = 1.0f - expf(-sigma * (znext - z) * F.distance_scale);   // tensorBase.py:610
         if (k == S - 1) alpha = 1.0f;                                  // alpha[:, -1] = 1
@@ -365,25 +350,14 @@ bwd_shade_kernel(const FieldDev F, const BwdArgs A) {
       const float qq[3] = {q_s[ls * 3], q_s[ls * 3 + 1], q_s[ls * 3 + 2]};
 #pragma unroll
       for (int i = 0; i < 3; ++i) {
-        const int W = F.g[mat0(i)], H = F.g[mat1(i)], Ln = F.g[vecm(i)];
-        int x0, x1, y0, y1, l0, l1; float tx, ty, tl;
-        grid_coord(qq[mat0(i)], W, x0, x1, tx);
-        grid_coord(qq[mat1(i)], H, y0, y1, ty);
-        grid_coord(qq[vecm(i)], Ln, l0, l1, tl);
-        const float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-        const float w10 = (1.0f - tx) * ty, w11 = tx * ty, u0 = 1.0f - tl;
+        const VmTap t = vm_tap<CA>(F.g, i, qq);
         for (int grp = cq; grp < CA / 4; grp += 4) {                    // 4 components per 16-byte group
-          const float* P = F.aplane[i] + grp * 4;
-          const float* Lp = F.aline[i] + grp * 4;
-          const float4 a = ldg4(P + ((size_t)y0 * W + x0) * CA), b = ldg4(P + ((size_t)y0 * W + x1) * CA);
-          const float4 c = ldg4(P + ((size_t)y1 * W + x0) * CA), d = ldg4(P + ((size_t)y1 * W + x1) * CA);
-          const float4 u = ldg4(Lp + (size_t)l0 * CA), v = ldg4(Lp + (size_t)l1 * CA);
+          float v[4];
+          vm_products<4>(t, F.aplane[i], F.aline[i], grp * 4, v);
           float* xo = X_s + ls * LDX + i * CA + grp * 4;
           const bool ok = ls < n_valid;
-          xo[0] = ok ? (a.x * w00 + b.x * w01 + c.x * w10 + d.x * w11) * (u.x * u0 + v.x * tl) : 0.0f;
-          xo[1] = ok ? (a.y * w00 + b.y * w01 + c.y * w10 + d.y * w11) * (u.y * u0 + v.y * tl) : 0.0f;
-          xo[2] = ok ? (a.z * w00 + b.z * w01 + c.z * w10 + d.z * w11) * (u.z * u0 + v.z * tl) : 0.0f;
-          xo[3] = ok ? (a.w * w00 + b.w * w01 + c.w * w10 + d.w * w11) * (u.w * u0 + v.w * tl) : 0.0f;
+#pragma unroll
+          for (int e = 0; e < 4; ++e) xo[e] = ok ? v[e] : 0.0f;
         }
       }
     }
@@ -658,44 +632,9 @@ bwd_shade_kernel(const FieldDev F, const BwdArgs A) {
         const float qq[3] = {q_s[ls * 3], q_s[ls * 3 + 1], q_s[ls * 3 + 2]};
         float dq[3] = {0.0f, 0.0f, 0.0f};
 #pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          const int W = F.g[mat0(i)], H = F.g[mat1(i)], Ln = F.g[vecm(i)];
-          int x0, x1, y0, y1, l0, l1; float tx, ty, tl, dx, dy, dl;
-          coord_g(qq[mat0(i)], W, x0, x1, tx, dx);
-          coord_g(qq[mat1(i)], H, y0, y1, ty, dy);
-          coord_g(qq[vecm(i)], Ln, l0, l1, tl, dl);
-          const float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-          const float w10 = (1.0f - tx) * ty, w11 = tx * ty, u0 = 1.0f - tl;
-          float gx = 0.0f, gy = 0.0f, gl = 0.0f;
-          for (int grp = cq; grp < CA / 4; grp += 4) {                  // 4 components per 16-byte group
-            const size_t o00 = ((size_t)y0 * W + x0) * CA + grp * 4, o01 = ((size_t)y0 * W + x1) * CA + grp * 4;
-            const size_t o10 = ((size_t)y1 * W + x0) * CA + grp * 4, o11 = ((size_t)y1 * W + x1) * CA + grp * 4;
-            const size_t ol0 = (size_t)l0 * CA + grp * 4, ol1 = (size_t)l1 * CA + grp * 4;
-            const float4 a4 = ldg4(F.aplane[i] + o00), b4 = ldg4(F.aplane[i] + o01);
-            const float4 c4 = ldg4(F.aplane[i] + o10), d4 = ldg4(F.aplane[i] + o11);
-            const float4 u4 = ldg4(F.aline[i] + ol0), v4 = ldg4(F.aline[i] + ol1);
-            const float av[4] = {a4.x, a4.y, a4.z, a4.w}, bv[4] = {b4.x, b4.y, b4.z, b4.w};
-            const float cv[4] = {c4.x, c4.y, c4.z, c4.w}, dv[4] = {d4.x, d4.y, d4.z, d4.w};
-            const float uv[4] = {u4.x, u4.y, u4.z, u4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
-            float dP[4], dL[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float gc = X_s[ls * LDX + i * CA + grp * 4 + e];
-              dP[e] = gc * (uv[e] * u0 + vv[e] * tl);
-              dL[e] = gc * (av[e] * w00 + bv[e] * w01 + cv[e] * w10 + dv[e] * w11);
-              gx += dP[e] * ((bv[e] - av[e]) * (1.0f - ty) + (dv[e] - cv[e]) * ty);
-              gy += dP[e] * ((cv[e] - av[e]) * (1.0f - tx) + (dv[e] - bv[e]) * tx);
-              gl += dL[e] * (vv[e] - uv[e]);
-            }
-            red4g(A.d_aplane[i] + o00, dP[0] * w00, dP[1] * w00, dP[2] * w00, dP[3] * w00);
-            red4g(A.d_aplane[i] + o01, dP[0] * w01, dP[1] * w01, dP[2] * w01, dP[3] * w01);
-            red4g(A.d_aplane[i] + o10, dP[0] * w10, dP[1] * w10, dP[2] * w10, dP[3] * w10);
-            red4g(A.d_aplane[i] + o11, dP[0] * w11, dP[1] * w11, dP[2] * w11, dP[3] * w11);
-            red4g(A.d_aline[i] + ol0, dL[0] * u0, dL[1] * u0, dL[2] * u0, dL[3] * u0);
-            red4g(A.d_aline[i] + ol1, dL[0] * tl, dL[1] * tl, dL[2] * tl, dL[3] * tl);
-          }
-          dq[mat0(i)] += gx * dx; dq[mat1(i)] += gy * dy; dq[vecm(i)] += gl * dl;
-        }
+        for (int i = 0; i < 3; ++i)                                       // this thread's 4-component groups cq, cq + 4
+          vm_pair_backward<CA, 1>(F.g, i, F.aplane[i], F.aline[i], A.d_aplane[i], A.d_aline[i], qq,
+                                  [&](int c) { return X_s[ls * LDX + i * CA + c]; }, dq, 4 * cq, 16);
         dq0 = dq[0]; dq1 = dq[1]; dq2 = dq[2];
       }
       dq0 += __shfl_xor_sync(0xffffffffu, dq0, 1); dq0 += __shfl_xor_sync(0xffffffffu, dq0, 2);
@@ -790,46 +729,9 @@ bwd_density_kernel(const FieldDev F, const BwdArgs A) {
           float p[3], q[3], dq[3] = {0.0f, 0.0f, 0.0f};
           sample_pos(F, R, zk, p, q);
 #pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            const int W = F.g[mat0(i)], H = F.g[mat1(i)], Ln = F.g[vecm(i)];
-            int x0, x1, y0, y1, l0, l1; float tx, ty, tl, dx, dy, dl;
-            coord_g(q[mat0(i)], W, x0, x1, tx, dx);
-            coord_g(q[mat1(i)], H, y0, y1, ty, dy);
-            coord_g(q[vecm(i)], Ln, l0, l1, tl, dl);
-            const size_t o00 = ((size_t)y0 * W + x0) * CD, o01 = ((size_t)y0 * W + x1) * CD;
-            const size_t o10 = ((size_t)y1 * W + x0) * CD, o11 = ((size_t)y1 * W + x1) * CD;
-            const size_t ol0 = (size_t)l0 * CD, ol1 = (size_t)l1 * CD;
-            const float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-            const float w10 = (1.0f - tx) * ty, w11 = tx * ty, u0 = 1.0f - tl;
-            float gx = 0.0f, gy = 0.0f, gl = 0.0f;
-#pragma unroll
-            for (int c = 0; c < CD; c += 4) {
-              const float4 a = ldg4(F.dplane[i] + o00 + c), b = ldg4(F.dplane[i] + o01 + c);
-              const float4 cc = ldg4(F.dplane[i] + o10 + c), d = ldg4(F.dplane[i] + o11 + c);
-              const float4 u = ldg4(F.dline[i] + ol0 + c), v = ldg4(F.dline[i] + ol1 + c);
-              const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-              const float cv[4] = {cc.x, cc.y, cc.z, cc.w}, dv[4] = {d.x, d.y, d.z, d.w};
-              const float uv[4] = {u.x, u.y, u.z, u.w}, vv[4] = {v.x, v.y, v.z, v.w};
-              float dP[4], dL[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float P = av[e] * w00 + bv[e] * w01 + cv[e] * w10 + dv[e] * w11;
-                const float Lv = uv[e] * u0 + vv[e] * tl;
-                dP[e] = df * Lv;
-                dL[e] = df * P;
-                gx += dP[e] * ((bv[e] - av[e]) * (1.0f - ty) + (dv[e] - cv[e]) * ty);
-                gy += dP[e] * ((cv[e] - av[e]) * (1.0f - tx) + (dv[e] - bv[e]) * tx);
-                gl += dL[e] * (vv[e] - uv[e]);
-              }
-              red4g(A.d_dplane[i] + o00 + c, dP[0] * w00, dP[1] * w00, dP[2] * w00, dP[3] * w00);
-              red4g(A.d_dplane[i] + o01 + c, dP[0] * w01, dP[1] * w01, dP[2] * w01, dP[3] * w01);
-              red4g(A.d_dplane[i] + o10 + c, dP[0] * w10, dP[1] * w10, dP[2] * w10, dP[3] * w10);
-              red4g(A.d_dplane[i] + o11 + c, dP[0] * w11, dP[1] * w11, dP[2] * w11, dP[3] * w11);
-              red4g(A.d_dline[i] + ol0 + c, dL[0] * u0, dL[1] * u0, dL[2] * u0, dL[3] * u0);
-              red4g(A.d_dline[i] + ol1 + c, dL[0] * tl, dL[1] * tl, dL[2] * tl, dL[3] * tl);
-            }
-            dq[mat0(i)] += gx * dx; dq[mat1(i)] += gy * dy; dq[vecm(i)] += gl * dl;
-          }
+          for (int i = 0; i < 3; ++i)
+            vm_pair_backward<CD>(F.g, i, F.dplane[i], F.dline[i], A.d_dplane[i], A.d_dline[i], q,
+                                 [&](int) { return df; }, dq);
           float dp0, dp1, dp2;
           contract_bwd(R.o[0] + R.vd[0] * zk, R.o[1] + R.vd[1] * zk, R.o[2] + R.vd[2] * zk,
                        dq[0] * F.ainv[0], dq[1] * F.ainv[1], dq[2] * F.ainv[2], dp0, dp1, dp2);

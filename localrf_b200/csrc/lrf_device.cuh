@@ -3,20 +3,11 @@
 #pragma once
 #include <cuda_bf16.h>
 
+#include <type_traits>
+
 #include "lrf_common.cuh"
 
 namespace lrf {
-
-// Experiment switch (code size): LRF_ROLL_PLANES=1 keeps the loop over the three planes of the
-// VM gathers ROLLED (a third of the gather code, plane geometry indexed at run time); 0 = fully unrolled (default).
-#ifndef LRF_ROLL_PLANES
-#define LRF_ROLL_PLANES 0
-#endif
-#if LRF_ROLL_PLANES
-#define LRF_PLANE_LOOP _Pragma("unroll 1")
-#else
-#define LRF_PLANE_LOOP _Pragma("unroll")
-#endif
 
 constexpr int TM = 128;      // appearance samples per MLP tile (two wgmma M = 64 halves)
 constexpr float T_EPS = 1e-10f;  // early-termination transmittance
@@ -332,165 +323,171 @@ __device__ __forceinline__ float alpha_mask(const FieldDev& F, const float* p) {
   return v;
 }
 
-// compute_densityfeature for one point (tensoRF.py:112-151), channel-last planes/lines
-__device__ __forceinline__ float density_feature(const FieldDev& F, const float* q) {
+// ---- the VM (plane x line) lookup (tensoRF.py:112-194) -------------------------------------------
+// Grids are channel-last: plane i is [H][W][C] texels, line i is [L][C].  Component c of pair i at a point is
+// (a w00 + b w01 + c w10 + d w11) * (u (1 - tl) + v tl), a..d the plane's four taps, u, v the line's two.
+// Texels are fp32, or bf16 with 16-bit grid storage (LrfField.grid_dtype = LRF_GRID_BF16): half the sectors
+// and half the load instructions.  bf16 -> fp32 is exact (a 16-bit shift) and the arithmetic is the same
+// expressions, so a field whose parameters are bf16-representable gives the same values from either storage.
+template <bool H16>
+using Texel = std::conditional_t<H16, __nv_bfloat16, float>;
+template <bool H16>
+__device__ __forceinline__ const Texel<H16>* texels(const float* grid) {
+  return reinterpret_cast<const Texel<H16>*>(grid);
+}
+
+struct VmTap {                     // one plane / line pair at one point
+  size_t p00, p01, p10, p11;       // element offsets of the plane's four taps ([y][x])
+  size_t l0, l1;                   // and of the line's two
+  float w00, w01, w10, w11;        // bilinear weights
+  float u0, tl;                    // linear weights of l0 and l1 (u0 = 1 - tl)
+};
+
+template <int C>
+__device__ __forceinline__ VmTap vm_tap(const int* g3, int i, const float* q) {
+  const int W = g3[mat0(i)], H = g3[mat1(i)], L = g3[vecm(i)];
+  int x0, x1, y0, y1, l0, l1;
+  float tx, ty, tl;
+  grid_coord(q[mat0(i)], W, x0, x1, tx);
+  grid_coord(q[mat1(i)], H, y0, y1, ty);
+  grid_coord(q[vecm(i)], L, l0, l1, tl);
+  VmTap t;
+  t.p00 = ((size_t)y0 * W + x0) * C; t.p01 = ((size_t)y0 * W + x1) * C;
+  t.p10 = ((size_t)y1 * W + x0) * C; t.p11 = ((size_t)y1 * W + x1) * C;
+  t.l0 = (size_t)l0 * C; t.l1 = (size_t)l1 * C;
+  t.w00 = (1.0f - tx) * (1.0f - ty); t.w01 = tx * (1.0f - ty);
+  t.w10 = (1.0f - tx) * ty; t.w11 = tx * ty;
+  t.u0 = 1.0f - tl; t.tl = tl;
+  return t;
+}
+
+// one 16-byte piece of a texel as floats: 4 fp32 components, or 8 bf16 ones
+__device__ __forceinline__ void ldg_texel(const float* p, float (&v)[4]) {
+  const float4 r = ldg4(p);
+  v[0] = r.x; v[1] = r.y; v[2] = r.z; v[3] = r.w;
+}
+__device__ __forceinline__ void ldg_texel(const __nv_bfloat16* p, float (&v)[8]) {
+  const uint4 r = __ldg(reinterpret_cast<const uint4*>(p));
+  v[0] = __uint_as_float(r.x << 16); v[1] = __uint_as_float(r.x & 0xffff0000u);
+  v[2] = __uint_as_float(r.y << 16); v[3] = __uint_as_float(r.y & 0xffff0000u);
+  v[4] = __uint_as_float(r.z << 16); v[5] = __uint_as_float(r.z & 0xffff0000u);
+  v[6] = __uint_as_float(r.w << 16); v[7] = __uint_as_float(r.w & 0xffff0000u);
+}
+
+// components c .. c + N - 1 of one pair at tap t: out[e] = bilinear(plane) * linear(line), one 16-byte piece
+// of each of the six texels at a time
+template <int N, class T>
+__device__ __forceinline__ void vm_products(const VmTap& t, const T* plane, const T* line, int c, float* out) {
+  constexpr int U = 16 / sizeof(T);
+  static_assert(N % U == 0, "whole 16-byte pieces");
+#pragma unroll
+  for (int h = c; h < c + N; h += U) {
+    float a[U], b[U], cc[U], d[U], u[U], v[U];
+    ldg_texel(plane + t.p00 + h, a); ldg_texel(plane + t.p01 + h, b);
+    ldg_texel(plane + t.p10 + h, cc); ldg_texel(plane + t.p11 + h, d);
+    ldg_texel(line + t.l0 + h, u); ldg_texel(line + t.l1 + h, v);
+#pragma unroll
+    for (int e = 0; e < U; ++e)
+      out[h - c + e] = (a[e] * t.w00 + b[e] * t.w01 + cc[e] * t.w10 + d[e] * t.w11) * (u[e] * t.u0 + v[e] * t.tl);
+  }
+}
+
+// compute_densityfeature for one point (tensoRF.py:112-151): components 0..7 of each plane, then planes 0, 1, 2
+template <bool H16>
+__device__ __forceinline__ float density_feature_t(const FieldDev& F, const float* q) {
   float sigma = 0.0f;
-LRF_PLANE_LOOP
+#pragma unroll
   for (int i = 0; i < 3; ++i) {
-    const int W = F.g[mat0(i)], H = F.g[mat1(i)], L = F.g[vecm(i)];
-    int x0, x1, y0, y1, l0, l1;
-    float tx, ty, tl;
-    grid_coord(q[mat0(i)], W, x0, x1, tx);
-    grid_coord(q[mat1(i)], H, y0, y1, ty);
-    grid_coord(q[vecm(i)], L, l0, l1, tl);
-    const float* P = F.dplane[i];
-    const float* p00 = P + ((size_t)y0 * W + x0) * CD;
-    const float* p01 = P + ((size_t)y0 * W + x1) * CD;
-    const float* p10 = P + ((size_t)y1 * W + x0) * CD;
-    const float* p11 = P + ((size_t)y1 * W + x1) * CD;
-    const float* q0 = F.dline[i] + (size_t)l0 * CD;
-    const float* q1 = F.dline[i] + (size_t)l1 * CD;
-    float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-    float w10 = (1.0f - tx) * ty, w11 = tx * ty;
+    float v[CD];
+    vm_products<CD>(vm_tap<CD>(F.g, i, q), texels<H16>(F.dplane[i]), texels<H16>(F.dline[i]), 0, v);
     float s = 0.0f;
 #pragma unroll
-    for (int h = 0; h < CD / 4; ++h) {
-      float4 a = ldg4(p00 + 4 * h), b = ldg4(p01 + 4 * h), c = ldg4(p10 + 4 * h),
-             d = ldg4(p11 + 4 * h);
-      float4 u = ldg4(q0 + 4 * h), v = ldg4(q1 + 4 * h);
-      float px = a.x * w00 + b.x * w01 + c.x * w10 + d.x * w11;
-      float py = a.y * w00 + b.y * w01 + c.y * w10 + d.y * w11;
-      float pz = a.z * w00 + b.z * w01 + c.z * w10 + d.z * w11;
-      float pw = a.w * w00 + b.w * w01 + c.w * w10 + d.w * w11;
-      s += px * (u.x * (1.0f - tl) + v.x * tl);
-      s += py * (u.y * (1.0f - tl) + v.y * tl);
-      s += pz * (u.z * (1.0f - tl) + v.z * tl);
-      s += pw * (u.w * (1.0f - tl) + v.w * tl);
-    }
+    for (int e = 0; e < CD; ++e) s += v[e];
     sigma += s;
   }
   return sigma;
 }
 
 // one plane's 24 appearance features of one point (tensoRF.py:153-194): out[c] = plane_c * line_c
-__device__ __forceinline__ void app_plane_features(const FieldDev& F, int i, const float* q,
-                                                   float* out /*[CA]*/) {
-  const int W = F.g[mat0(i)], H = F.g[mat1(i)], L = F.g[vecm(i)];
+template <bool H16>
+__device__ __forceinline__ void app_plane_features_t(const FieldDev& F, int i, const float* q, float* out /*[CA]*/) {
+  const VmTap t = vm_tap<CA>(F.g, i, q);
+#pragma unroll
+  for (int c = 0; c < CA; c += 8) vm_products<8>(t, texels<H16>(F.aplane[i]), texels<H16>(F.aline[i]), c, out + c);
+}
+
+// ---- backward of the VM lookup (F.grid_sample align_corners=True, padding_mode="border") ----------------
+// pixel coordinate, its two taps and d(pixel)/d(normalised coordinate) (0 when clipped: ATen clip_coordinates_set_grad)
+__device__ __forceinline__ void grid_coord_grad(float c, int size, int& i0, int& i1, float& t,
+                                                float& dcoord) {
+  float x = ((c + 1.0f) * 0.5f) * (float)(size - 1);
+  dcoord = (x <= 0.0f || x >= (float)(size - 1)) ? 0.0f : 0.5f * (float)(size - 1);
+  x = fminf((float)(size - 1), fmaxf(x, 0.0f));
+  const float f = floorf(x);
+  i0 = (int)f;
+  i1 = min(i0 + 1, size - 1);
+  t = x - f;
+}
+
+// Device only: the gradient scatter needs global atomics, which the host build of this header
+// (tests/host_emul, for the forward building blocks) does not provide.
+#ifdef __CUDACC__
+// 16-byte vector reduction (red.global.add.v4.f32, sm_90+): one atomic per 4 components
+__device__ __forceinline__ void red4(float* p, float x, float y, float z, float w) {
+  atomicAdd(reinterpret_cast<float4*>(p), make_float4(x, y, z, w));
+}
+
+// backward of one plane/line pair with C components, over the 4-component groups c_first, c_first + c_step, ...
+// (UNROLL of them per loop step).  g(c) = dL/d(plane_c * line_c).  Parameter gradients are accumulated by atomic
+// adds, four components at a time; the gradient of the normalised point is added to dq.
+template <int C, int UNROLL = 2, class G>
+__device__ __forceinline__ void vm_pair_backward(const int* g3, int i, const float* plane,
+                                                 const float* line, float* d_plane, float* d_line,
+                                                 const float* q, G g, float* dq, int c_first = 0, int c_step = 4) {
+  const int W = g3[mat0(i)], H = g3[mat1(i)], L = g3[vecm(i)];
   int x0, x1, y0, y1, l0, l1;
-  float tx, ty, tl;
-  grid_coord(q[mat0(i)], W, x0, x1, tx);
-  grid_coord(q[mat1(i)], H, y0, y1, ty);
-  grid_coord(q[vecm(i)], L, l0, l1, tl);
-  const float* P = F.aplane[i];
-  const float* p00 = P + ((size_t)y0 * W + x0) * CA;
-  const float* p01 = P + ((size_t)y0 * W + x1) * CA;
-  const float* p10 = P + ((size_t)y1 * W + x0) * CA;
-  const float* p11 = P + ((size_t)y1 * W + x1) * CA;
-  const float* q0 = F.aline[i] + (size_t)l0 * CA;
-  const float* q1 = F.aline[i] + (size_t)l1 * CA;
-  float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-  float w10 = (1.0f - tx) * ty, w11 = tx * ty;
+  float tx, ty, tl, dx, dy, dl;
+  grid_coord_grad(q[mat0(i)], W, x0, x1, tx, dx);
+  grid_coord_grad(q[mat1(i)], H, y0, y1, ty, dy);
+  grid_coord_grad(q[vecm(i)], L, l0, l1, tl, dl);
+  const size_t o00 = ((size_t)y0 * W + x0) * C, o01 = ((size_t)y0 * W + x1) * C;
+  const size_t o10 = ((size_t)y1 * W + x0) * C, o11 = ((size_t)y1 * W + x1) * C;
+  const size_t ol0 = (size_t)l0 * C, ol1 = (size_t)l1 * C;
+  const float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
+  const float w10 = (1.0f - tx) * ty, w11 = tx * ty, u0 = 1.0f - tl;
+  float gx = 0.0f, gy = 0.0f, gl = 0.0f;
+#pragma unroll UNROLL
+  for (int c = c_first; c < C; c += c_step) {
+    const float4 a = ldg4(plane + o00 + c), b = ldg4(plane + o01 + c);
+    const float4 cc = ldg4(plane + o10 + c), d = ldg4(plane + o11 + c);
+    const float4 u = ldg4(line + ol0 + c), v = ldg4(line + ol1 + c);
+    const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+    const float cv[4] = {cc.x, cc.y, cc.z, cc.w}, dv[4] = {d.x, d.y, d.z, d.w};
+    const float uv[4] = {u.x, u.y, u.z, u.w}, vv[4] = {v.x, v.y, v.z, v.w};
+    float dP[4], dLc[4];
 #pragma unroll
-  for (int h = 0; h < CA / 4; ++h) {
-    float4 a = ldg4(p00 + 4 * h), b = ldg4(p01 + 4 * h), c = ldg4(p10 + 4 * h),
-           d = ldg4(p11 + 4 * h);
-    float4 u = ldg4(q0 + 4 * h), v = ldg4(q1 + 4 * h);
-    out[4 * h + 0] = (a.x * w00 + b.x * w01 + c.x * w10 + d.x * w11) * (u.x * (1.0f - tl) + v.x * tl);
-    out[4 * h + 1] = (a.y * w00 + b.y * w01 + c.y * w10 + d.y * w11) * (u.y * (1.0f - tl) + v.y * tl);
-    out[4 * h + 2] = (a.z * w00 + b.z * w01 + c.z * w10 + d.z * w11) * (u.z * (1.0f - tl) + v.z * tl);
-    out[4 * h + 3] = (a.w * w00 + b.w * w01 + c.w * w10 + d.w * w11) * (u.w * (1.0f - tl) + v.w * tl);
-  }
-}
-
-// ---- 16-bit grid storage (LrfField.grid_dtype = LRF_GRID_BF16) ----------------------------------
-// The same gathers reading bfloat16 texels in the same [H][W][C] / [L][C] layout: a density texel is ONE
-// 16-byte load (8 components), an appearance texel three (24 components) -- half the sectors and half the
-// load instructions of the fp32 grids.  bf16 -> fp32 is exact (a 16-bit shift) and the arithmetic is the fp32
-// code's, expression for expression, so a field whose parameters are bf16-representable renders the same
-// values from either storage.
-struct Tex8 { float v[8]; };
-__device__ __forceinline__ Tex8 ldg8_bf16(const __nv_bfloat16* p) {
-  const uint4 r = __ldg(reinterpret_cast<const uint4*>(p));
-  Tex8 t;
-  t.v[0] = __uint_as_float(r.x << 16); t.v[1] = __uint_as_float(r.x & 0xffff0000u);
-  t.v[2] = __uint_as_float(r.y << 16); t.v[3] = __uint_as_float(r.y & 0xffff0000u);
-  t.v[4] = __uint_as_float(r.z << 16); t.v[5] = __uint_as_float(r.z & 0xffff0000u);
-  t.v[6] = __uint_as_float(r.w << 16); t.v[7] = __uint_as_float(r.w & 0xffff0000u);
-  return t;
-}
-
-// compute_densityfeature for one point, bf16 texels (cf. density_feature)
-__device__ __forceinline__ float density_feature_bf16(const FieldDev& F, const float* q) {
-  static_assert(CD == 8, "one 16-byte load per density texel");
-  float sigma = 0.0f;
-LRF_PLANE_LOOP
-  for (int i = 0; i < 3; ++i) {
-    const int W = F.g[mat0(i)], H = F.g[mat1(i)], L = F.g[vecm(i)];
-    int x0, x1, y0, y1, l0, l1;
-    float tx, ty, tl;
-    grid_coord(q[mat0(i)], W, x0, x1, tx);
-    grid_coord(q[mat1(i)], H, y0, y1, ty);
-    grid_coord(q[vecm(i)], L, l0, l1, tl);
-    const __nv_bfloat16* P = reinterpret_cast<const __nv_bfloat16*>(F.dplane[i]);
-    const __nv_bfloat16* Ln = reinterpret_cast<const __nv_bfloat16*>(F.dline[i]);
-    const Tex8 a = ldg8_bf16(P + ((size_t)y0 * W + x0) * CD), b = ldg8_bf16(P + ((size_t)y0 * W + x1) * CD);
-    const Tex8 c = ldg8_bf16(P + ((size_t)y1 * W + x0) * CD), d = ldg8_bf16(P + ((size_t)y1 * W + x1) * CD);
-    const Tex8 u = ldg8_bf16(Ln + (size_t)l0 * CD), v = ldg8_bf16(Ln + (size_t)l1 * CD);
-    float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-    float w10 = (1.0f - tx) * ty, w11 = tx * ty;
-    float s = 0.0f;
-#pragma unroll
-    for (int e = 0; e < CD; ++e) {
-      float px = a.v[e] * w00 + b.v[e] * w01 + c.v[e] * w10 + d.v[e] * w11;
-      s += px * (u.v[e] * (1.0f - tl) + v.v[e] * tl);
+    for (int e = 0; e < 4; ++e) {
+      const float P = av[e] * w00 + bv[e] * w01 + cv[e] * w10 + dv[e] * w11;
+      const float Lc = uv[e] * u0 + vv[e] * tl;
+      const float gc = g(c + e);
+      dP[e] = gc * Lc;
+      dLc[e] = gc * P;
+      gx += dP[e] * ((bv[e] - av[e]) * (1.0f - ty) + (dv[e] - cv[e]) * ty);
+      gy += dP[e] * ((cv[e] - av[e]) * (1.0f - tx) + (dv[e] - bv[e]) * tx);
+      gl += dLc[e] * (vv[e] - uv[e]);
     }
-    sigma += s;
+    red4(d_plane + o00 + c, dP[0] * w00, dP[1] * w00, dP[2] * w00, dP[3] * w00);
+    red4(d_plane + o01 + c, dP[0] * w01, dP[1] * w01, dP[2] * w01, dP[3] * w01);
+    red4(d_plane + o10 + c, dP[0] * w10, dP[1] * w10, dP[2] * w10, dP[3] * w10);
+    red4(d_plane + o11 + c, dP[0] * w11, dP[1] * w11, dP[2] * w11, dP[3] * w11);
+    red4(d_line + ol0 + c, dLc[0] * u0, dLc[1] * u0, dLc[2] * u0, dLc[3] * u0);
+    red4(d_line + ol1 + c, dLc[0] * tl, dLc[1] * tl, dLc[2] * tl, dLc[3] * tl);
   }
-  return sigma;
+  dq[mat0(i)] += gx * dx;
+  dq[mat1(i)] += gy * dy;
+  dq[vecm(i)] += gl * dl;
 }
-
-// one plane's 24 appearance features of one point, bf16 texels (cf. app_plane_features)
-__device__ __forceinline__ void app_plane_features_bf16(const FieldDev& F, int i, const float* q,
-                                                        float* out /*[CA]*/) {
-  static_assert(CA % 8 == 0, "16-byte loads of 8 components");
-  const int W = F.g[mat0(i)], H = F.g[mat1(i)], L = F.g[vecm(i)];
-  int x0, x1, y0, y1, l0, l1;
-  float tx, ty, tl;
-  grid_coord(q[mat0(i)], W, x0, x1, tx);
-  grid_coord(q[mat1(i)], H, y0, y1, ty);
-  grid_coord(q[vecm(i)], L, l0, l1, tl);
-  const __nv_bfloat16* P = reinterpret_cast<const __nv_bfloat16*>(F.aplane[i]);
-  const __nv_bfloat16* p00 = P + ((size_t)y0 * W + x0) * CA;
-  const __nv_bfloat16* p01 = P + ((size_t)y0 * W + x1) * CA;
-  const __nv_bfloat16* p10 = P + ((size_t)y1 * W + x0) * CA;
-  const __nv_bfloat16* p11 = P + ((size_t)y1 * W + x1) * CA;
-  const __nv_bfloat16* q0 = reinterpret_cast<const __nv_bfloat16*>(F.aline[i]) + (size_t)l0 * CA;
-  const __nv_bfloat16* q1 = reinterpret_cast<const __nv_bfloat16*>(F.aline[i]) + (size_t)l1 * CA;
-  float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-  float w10 = (1.0f - tx) * ty, w11 = tx * ty;
-#pragma unroll
-  for (int c8 = 0; c8 < CA / 8; ++c8) {
-    const Tex8 a = ldg8_bf16(p00 + 8 * c8), b = ldg8_bf16(p01 + 8 * c8), c = ldg8_bf16(p10 + 8 * c8),
-               d = ldg8_bf16(p11 + 8 * c8);
-    const Tex8 u = ldg8_bf16(q0 + 8 * c8), v = ldg8_bf16(q1 + 8 * c8);
-#pragma unroll
-    for (int e = 0; e < 8; ++e)
-      out[8 * c8 + e] = (a.v[e] * w00 + b.v[e] * w01 + c.v[e] * w10 + d.v[e] * w11) *
-                        (u.v[e] * (1.0f - tl) + v.v[e] * tl);
-  }
-}
-
-// storage-type dispatch (compile time): H16 = bf16 texels
-template <bool H16>
-__device__ __forceinline__ float density_feature_t(const FieldDev& F, const float* q) {
-  if constexpr (H16) return density_feature_bf16(F, q);
-  else return density_feature(F, q);
-}
-template <bool H16>
-__device__ __forceinline__ void app_plane_features_t(const FieldDev& F, int i, const float* q, float* out) {
-  if constexpr (H16) app_plane_features_bf16(F, i, q, out);
-  else app_plane_features(F, i, q, out);
-}
+#endif  // __CUDACC__
 
 // ---- warp primitives ----------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -9,18 +9,6 @@
 
 namespace lrf {
 
-// pixel coordinate, its two taps and d(pixel)/d(normalised coordinate) (0 when clipped)
-__device__ __forceinline__ void grid_coord_grad(float c, int size, int& i0, int& i1, float& t,
-                                                float& dcoord) {
-  float x = ((c + 1.0f) * 0.5f) * (float)(size - 1);
-  dcoord = (x <= 0.0f || x >= (float)(size - 1)) ? 0.0f : 0.5f * (float)(size - 1);
-  x = fminf((float)(size - 1), fmaxf(x, 0.0f));
-  const float f = floorf(x);
-  i0 = (int)f;
-  i1 = min(i0 + 1, size - 1);
-  t = x - f;
-}
-
 // forward: prod[m][i*C + c] = bilinear(plane_i[c]) * linear(line_i[c])      (tensoRF.py:174-194)
 __global__ void app_products_kernel(const FieldDev F, const float* __restrict__ xyz, long long M,
                                     float* __restrict__ out) {
@@ -28,72 +16,14 @@ __global__ void app_products_kernel(const FieldDev F, const float* __restrict__ 
   if (m >= M) return;
   const float q[3] = {xyz[3 * m], xyz[3 * m + 1], xyz[3 * m + 2]};
   float feat[CA];
-#pragma unroll 1
+#pragma unroll
   for (int i = 0; i < 3; ++i) {
-    if (i == 0) app_plane_features(F, 0, q, feat);
-    else if (i == 1) app_plane_features(F, 1, q, feat);
-    else app_plane_features(F, 2, q, feat);
+    app_plane_features_t<false>(F, i, q, feat);
 #pragma unroll
     for (int c = 0; c < CA; c += 4)
       *reinterpret_cast<float4*>(out + m * NF + i * CA + c) =
           make_float4(feat[c], feat[c + 1], feat[c + 2], feat[c + 3]);
   }
-}
-
-// 16-byte vector reduction (red.global.add.v4.f32, sm_90+): one atomic per 4 components
-__device__ __forceinline__ void red4(float* p, float x, float y, float z, float w) {
-  atomicAdd(reinterpret_cast<float4*>(p), make_float4(x, y, z, w));
-}
-
-// backward of one plane/line pair with C components.  g(c) = dL/d(plane_c * line_c).
-// Components are contiguous in memory (channel-last), so parameters are read and their gradients
-// accumulated four at a time.
-template <int C, class G>
-__device__ __forceinline__ void vm_pair_backward(const int* g3, int i, const float* plane,
-                                                 const float* line, float* d_plane, float* d_line,
-                                                 const float* q, G g, float* dq) {
-  const int W = g3[mat0(i)], H = g3[mat1(i)], L = g3[vecm(i)];
-  int x0, x1, y0, y1, l0, l1;
-  float tx, ty, tl, dx, dy, dl;
-  grid_coord_grad(q[mat0(i)], W, x0, x1, tx, dx);
-  grid_coord_grad(q[mat1(i)], H, y0, y1, ty, dy);
-  grid_coord_grad(q[vecm(i)], L, l0, l1, tl, dl);
-  const size_t o00 = ((size_t)y0 * W + x0) * C, o01 = ((size_t)y0 * W + x1) * C;
-  const size_t o10 = ((size_t)y1 * W + x0) * C, o11 = ((size_t)y1 * W + x1) * C;
-  const size_t ol0 = (size_t)l0 * C, ol1 = (size_t)l1 * C;
-  const float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-  const float w10 = (1.0f - tx) * ty, w11 = tx * ty, u0 = 1.0f - tl;
-  float gx = 0.0f, gy = 0.0f, gl = 0.0f;
-#pragma unroll 2
-  for (int c = 0; c < C; c += 4) {
-    const float4 a = ldg4(plane + o00 + c), b = ldg4(plane + o01 + c);
-    const float4 cc = ldg4(plane + o10 + c), d = ldg4(plane + o11 + c);
-    const float4 u = ldg4(line + ol0 + c), v = ldg4(line + ol1 + c);
-    const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-    const float cv[4] = {cc.x, cc.y, cc.z, cc.w}, dv[4] = {d.x, d.y, d.z, d.w};
-    const float uv[4] = {u.x, u.y, u.z, u.w}, vv[4] = {v.x, v.y, v.z, v.w};
-    float dP[4], dLc[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float P = av[e] * w00 + bv[e] * w01 + cv[e] * w10 + dv[e] * w11;
-      const float Lc = uv[e] * u0 + vv[e] * tl;
-      const float gc = g(c + e);
-      dP[e] = gc * Lc;
-      dLc[e] = gc * P;
-      gx += dP[e] * ((bv[e] - av[e]) * (1.0f - ty) + (dv[e] - cv[e]) * ty);
-      gy += dP[e] * ((cv[e] - av[e]) * (1.0f - tx) + (dv[e] - bv[e]) * tx);
-      gl += dLc[e] * (vv[e] - uv[e]);
-    }
-    red4(d_plane + o00 + c, dP[0] * w00, dP[1] * w00, dP[2] * w00, dP[3] * w00);
-    red4(d_plane + o01 + c, dP[0] * w01, dP[1] * w01, dP[2] * w01, dP[3] * w01);
-    red4(d_plane + o10 + c, dP[0] * w10, dP[1] * w10, dP[2] * w10, dP[3] * w10);
-    red4(d_plane + o11 + c, dP[0] * w11, dP[1] * w11, dP[2] * w11, dP[3] * w11);
-    red4(d_line + ol0 + c, dLc[0] * u0, dLc[1] * u0, dLc[2] * u0, dLc[3] * u0);
-    red4(d_line + ol1 + c, dLc[0] * tl, dLc[1] * tl, dLc[2] * tl, dLc[3] * tl);
-  }
-  dq[mat0(i)] += gx * dx;
-  dq[mat1(i)] += gy * dy;
-  dq[vecm(i)] += gl * dl;
 }
 
 struct GradPtrs {

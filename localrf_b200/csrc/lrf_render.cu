@@ -6,7 +6,7 @@
 // clamp.  Replaces TensorBase.forward (models/tensorBase.py:567-636) and the per-field body of
 // LocalTensorfs.forward (local_tensorfs.py:397-497).
 //
-// One persistent CTA per SM, 16 warps (512 threads; LRF_THREADS) in two roles that only meet through
+// One persistent CTA per SM, 16 warps (512 threads) in two roles that only meet through
 // mbarriers and a few shared-memory counters:
 //
 //   producers (warps 0 .. W_CONS-1: 8)  each takes one ray at a time from a global counter (dynamic
@@ -18,7 +18,7 @@
 //       A tile in shared memory (K-major 8x8 core matrices).  Rows are handed out by an atomic cursor, so
 //       rays of all producers interleave in a tile; each row carries (ray slot, weight).  Every row arrives
 //       once on the tile's "full" mbarrier (128 arrivals = tile ready).
-//   consumers (the last two warpgroups, or one with LRF_CONS_WARPS=4)  per tile, one 64-row half each:
+//   consumers (the last two warpgroups)  per tile, one 64-row half each:
 //       layer 1 (A from shared memory, basis folded into W1, K = 80) and layer 2 (A = the bias + ReLU'd
 //       layer-1 accumulator re-split in registers, K = 128) as wgmma m64 bf16 MMAs, three products
 //       hi*hi + hi*lo + lo*hi per K-step, fp32 accumulators in registers; layer 3 (131 -> 3) + sigmoid on
@@ -30,34 +30,23 @@
 //
 // render_kernel_t<true> (fields with positional encodings) inserts a layer 0 (basis_mat as its own product),
 // builds the encoded layer-1 input in registers 64 columns at a time and streams layer 1's weight chunks by TMA.
-// Compile-time experiments kept as switches: LRF_THREADS, LRF_CONS_WARPS, LRF_SPIN_NS,
-// LRF_STEAL.  The weight operands are staged once per CTA by TMA bulk copies (cp.async.bulk -> UBLKCP); the
-// sample table is read from global memory through the L1.  The launcher sets the shared-memory carveout to the
+// The weight operands are staged once per CTA by TMA bulk copies (cp.async.bulk -> UBLKCP); the sample table is read from global memory through the L1.  The launcher sets the shared-memory carveout to the
 // smallest step that holds the CTA: the default build's folded-MLP layout fits the 196 KB step, which leaves
 // the L1 60 KB for the texel gathers.
-#include <cstdlib>
-
 #include "lrf_device.cuh"
 
 namespace lrf {
 
-#ifndef LRF_THREADS
-#define LRF_THREADS 512             // 16 warps (128 registers each); 640 = 20 warps at 96 registers
-#endif
-#ifndef LRF_CONS_WARPS
-#define LRF_CONS_WARPS 8            // 8: two consumer warpgroups, one half of a tile each (8 producers); 4: one consumer
-                                    // warpgroup takes both halves (12 producers)
-#endif
-constexpr int THREADS = LRF_THREADS;
-constexpr int N_CONS = LRF_CONS_WARPS;
-constexpr int N_CWG = N_CONS / 4;               // consumer warpgroups
-constexpr int W_CONS = THREADS / 32 - N_CONS;   // the last warps: consumers (whole warpgroups)
-constexpr int MAX_PROD = W_CONS;                // producer warps 0 .. W_CONS-1 (8 at 512 threads / 8 consumers)
+constexpr int THREADS = 512;                    // 16 warps (128 registers each)
+constexpr int N_CWG = 2;                        // consumer warpgroups, one 64-row half of a tile each
+constexpr int N_CONS = 4 * N_CWG;               // the last warps: consumers
+constexpr int W_CONS = THREADS / 32 - N_CONS;
+constexpr int MAX_PROD = W_CONS;                // producer warps 0 .. W_CONS-1 (8)
 constexpr int XA_LD = 33;                       // (positional encodings) floats per row of the basis-feature buffer
-static_assert(THREADS % 128 == 0 && W_CONS >= 1 && (N_CONS == 4 || N_CONS == 8), "warp roles");
 constexpr int NSLOT = 3;            // ray slots per producer warp
 constexpr int QCAP = 64;            // per-warp queue of selected samples
 constexpr int SPIN_PAD = 2048;      // polls before a blocked producer pads the open tile
+constexpr unsigned SPIN_NS = 200;   // back-off of a producer waiting for a free tile: spinning takes issue slots from the gathers
 
 // colour accumulators are 32-bit fixed point (2^-30 units, 9.3e-10: finer than an fp32 ulp of the
 // sums, which are <= 1): integer adds are associative, so the rows of a ray can be composited in any
@@ -80,39 +69,18 @@ struct Slot {                       // one ray in flight between a producer and 
   int state;                        // 0 free, 1 active
 };
 
-#ifndef LRF_STEAL
-#define LRF_STEAL 0                 // (correct; measured slower on the previous GPU target) idle producers help the in-flight rays of their CTA, one 32-sample step at a time
-#endif
-constexpr int MAXST = 32;           // steps a ray may have for step stealing (S <= 1024); longer rays march sequentially
-
-// One ray being marched by its owner producer and, once the global ray queue is empty, by the idle
-// producers of the CTA: steps are claimed from `next_step`; step s publishes the product P[s] of its
-// 32 transmittance factors right after its density gathers, then waits for P[0..s-1] and multiplies
-// them IN ORDER (bit-identical to the sequential carry), so every weight is independent of who
-// computed which step; per-step partial sums are added in step order by the owner.
-struct RayRec {
-  unsigned int next_step;           // claim counter (>= n_steps between rays: nothing to claim)
-  unsigned int stop_at;             // steps >= stop_at contribute nothing (early ray termination, T < 1e-10)
-  unsigned int ready, done;         // bit s: P[s] published / step s finished (sums stored, selected samples counted)
-  int slot_id;
-  long long ray;
-  float P[MAXST], accs[MAXST], deps[MAXST];
-  int marched[MAXST];
-};
-
 struct Ctrl {                       // CTA control block in shared memory
   unsigned long long bar_w, full[2];
   unsigned long long wrdy;          // fields with positional encodings: the streamed layer-1 weight chunk has landed
   unsigned int released;            // tiles whose A1 buffer + row metadata may be overwritten
   unsigned int cursor;              // rows handed out so far (tile = cursor >> 7)
   unsigned int prod_done;
-  unsigned int draw_done;           // producers whose draw from the global ray queue has failed (they help from then on)
   unsigned int n_tiles_final;
   unsigned int done;
 };
 
 struct SmemV3 {
-  int prep, a1, mslot, mw, part, slots, recs, q, alpha, ctrl, total;
+  int prep, a1, mslot, mw, part, slots, q, alpha, ctrl, total;
   int per_prod;                     // bytes of one producer's queue (+ alpha table)
 };
 
@@ -130,7 +98,6 @@ __host__ __device__ constexpr SmemV3 smem_v3(int S, bool floater, int nprod, boo
   off = (off + 15) & ~15;
   L.slots = off;  off += MAX_PROD * NSLOT * (int)sizeof(Slot);
   off = (off + 15) & ~15;
-  L.recs = off;   off += (LRF_STEAL ? nprod * (int)sizeof(RayRec) : 0);
   L.q = off;
   L.per_prod = QCAP * 2 + QCAP * 4 + QCAP + (floater ? Sp * 4 : 0);   // sample index, weight, slot id per entry
   L.per_prod = (L.per_prod + 15) & ~15;
@@ -144,12 +111,10 @@ __host__ __device__ constexpr SmemV3 smem_v3(int S, bool floater, int nprod, boo
 // Hopper's two largest shared-memory carveout steps are 196 and 228 KB, and the SM reserves 1 KB of each CTA's
 // share.  Without the floater filter the layout does not depend on S (the sample table is read from global
 // memory through the L1), so the default build's CTA fits the 196 KB step for every sample table and the L1
-// keeps 60 KB for the texel gathers (28 KB at the 228 KB step).  The LRF_STEAL / LRF_THREADS / LRF_CONS_WARPS
-// experiments may need more.
+// keeps 60 KB for the texel gathers (28 KB at the 228 KB step).
 constexpr int SMEM_196K_STEP = 196 * 1024 - 1024;
-static_assert(LRF_STEAL || THREADS != 512 || N_CONS != 8 ||
-              (smem_v3(344, false, MAX_PROD).total <= SMEM_196K_STEP &&
-               smem_v3(65535, false, MAX_PROD).total <= SMEM_196K_STEP),
+static_assert(smem_v3(344, false, MAX_PROD).total <= SMEM_196K_STEP &&
+              smem_v3(65535, false, MAX_PROD).total <= SMEM_196K_STEP,
               "the folded-MLP layout must fit the 196 KB carveout step");
 
 // ---- outputs (local_tensorfs.py:467-497) --------------------------------------------------------
@@ -201,74 +166,16 @@ __device__ __forceinline__ void finalize_slot(const BatchDev& B, Slot* s) {
 }
 
 // 72 appearance products of one sample -> one row of the A1 tile (bf16 hi/lo, 9 chunks of 8)
+template <bool H16>
 __device__ __forceinline__ void app_row(const FieldDev& F, const float* q, unsigned char* a_hi,
                                         unsigned char* a_lo, int row) {
-LRF_PLANE_LOOP
+#pragma unroll
   for (int i = 0; i < 3; ++i) {
-    const int W = F.g[mat0(i)], H = F.g[mat1(i)], L = F.g[vecm(i)];
-    int x0, x1, y0, y1, l0, l1;
-    float tx, ty, tl;
-    grid_coord(q[mat0(i)], W, x0, x1, tx);
-    grid_coord(q[mat1(i)], H, y0, y1, ty);
-    grid_coord(q[vecm(i)], L, l0, l1, tl);
-    const float* P = F.aplane[i];
-    const float* p00 = P + ((size_t)y0 * W + x0) * CA;
-    const float* p01 = P + ((size_t)y0 * W + x1) * CA;
-    const float* p10 = P + ((size_t)y1 * W + x0) * CA;
-    const float* p11 = P + ((size_t)y1 * W + x1) * CA;
-    const float* q0 = F.aline[i] + (size_t)l0 * CA;
-    const float* q1 = F.aline[i] + (size_t)l1 * CA;
-    const float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-    const float w10 = (1.0f - tx) * ty, w11 = tx * ty;
-    const float u0 = 1.0f - tl;
+    const VmTap t = vm_tap<CA>(F.g, i, q);
 #pragma unroll
     for (int c8 = 0; c8 < CA / 8; ++c8) {
       float v[8];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int o = c8 * 8 + h * 4;
-        const float4 a = ldg4(p00 + o), b = ldg4(p01 + o), c = ldg4(p10 + o), d = ldg4(p11 + o);
-        const float4 u = ldg4(q0 + o), w = ldg4(q1 + o);
-        v[4 * h + 0] = (a.x * w00 + b.x * w01 + c.x * w10 + d.x * w11) * (u.x * u0 + w.x * tl);
-        v[4 * h + 1] = (a.y * w00 + b.y * w01 + c.y * w10 + d.y * w11) * (u.y * u0 + w.y * tl);
-        v[4 * h + 2] = (a.z * w00 + b.z * w01 + c.z * w10 + d.z * w11) * (u.z * u0 + w.z * tl);
-        v[4 * h + 3] = (a.w * w00 + b.w * w01 + c.w * w10 + d.w * w11) * (u.w * u0 + w.w * tl);
-      }
-      store_chunk(a_hi, a_lo, row, i * (CA / 8) + c8, K1_CHUNKS, v);
-    }
-  }
-}
-
-// the same row from bf16 texels (LrfField.grid_dtype = LRF_GRID_BF16): three 16-byte loads per texel
-__device__ __forceinline__ void app_row_bf16(const FieldDev& F, const float* q, unsigned char* a_hi,
-                                             unsigned char* a_lo, int row) {
-LRF_PLANE_LOOP
-  for (int i = 0; i < 3; ++i) {
-    const int W = F.g[mat0(i)], H = F.g[mat1(i)], L = F.g[vecm(i)];
-    int x0, x1, y0, y1, l0, l1;
-    float tx, ty, tl;
-    grid_coord(q[mat0(i)], W, x0, x1, tx);
-    grid_coord(q[mat1(i)], H, y0, y1, ty);
-    grid_coord(q[vecm(i)], L, l0, l1, tl);
-    const __nv_bfloat16* P = reinterpret_cast<const __nv_bfloat16*>(F.aplane[i]);
-    const __nv_bfloat16* p00 = P + ((size_t)y0 * W + x0) * CA;
-    const __nv_bfloat16* p01 = P + ((size_t)y0 * W + x1) * CA;
-    const __nv_bfloat16* p10 = P + ((size_t)y1 * W + x0) * CA;
-    const __nv_bfloat16* p11 = P + ((size_t)y1 * W + x1) * CA;
-    const __nv_bfloat16* q0 = reinterpret_cast<const __nv_bfloat16*>(F.aline[i]) + (size_t)l0 * CA;
-    const __nv_bfloat16* q1 = reinterpret_cast<const __nv_bfloat16*>(F.aline[i]) + (size_t)l1 * CA;
-    const float w00 = (1.0f - tx) * (1.0f - ty), w01 = tx * (1.0f - ty);
-    const float w10 = (1.0f - tx) * ty, w11 = tx * ty;
-    const float u0 = 1.0f - tl;
-#pragma unroll
-    for (int c8 = 0; c8 < CA / 8; ++c8) {
-      const Tex8 a = ldg8_bf16(p00 + 8 * c8), b = ldg8_bf16(p01 + 8 * c8), c = ldg8_bf16(p10 + 8 * c8),
-                 d = ldg8_bf16(p11 + 8 * c8);
-      const Tex8 u = ldg8_bf16(q0 + 8 * c8), w = ldg8_bf16(q1 + 8 * c8);
-      float v[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e)
-        v[e] = (a.v[e] * w00 + b.v[e] * w01 + c.v[e] * w10 + d.v[e] * w11) * (u.v[e] * u0 + w.v[e] * tl);
+      vm_products<8>(t, texels<H16>(F.aplane[i]), texels<H16>(F.aline[i]), 8 * c8, v);
       store_chunk(a_hi, a_lo, row, i * (CA / 8) + c8, K1_CHUNKS, v);
     }
   }
@@ -286,12 +193,7 @@ struct ProdCtx {
 // can be more than two tiles ahead of the consumers, which a 1-bit phase cannot express.
 __device__ __forceinline__ void wait_tile_free(Ctrl* ctrl, unsigned int T) {
   if (T >= 2) {
-#ifndef LRF_SPIN_NS
-#define LRF_SPIN_NS 200
-#endif
-    while (*reinterpret_cast<volatile unsigned int*>(&ctrl->released) + 1u < T) {
-      if (LRF_SPIN_NS) __nanosleep(LRF_SPIN_NS);   // back off: a spinning producer takes issue slots from the gathers
-    }
+    while (*reinterpret_cast<volatile unsigned int*>(&ctrl->released) + 1u < T) __nanosleep(SPIN_NS);
     __threadfence_block();
   }
 }
@@ -355,8 +257,7 @@ __device__ __forceinline__ void flush_rows(const ProdCtx& P, const FieldDev& F, 
     sample_pos(F, R, __ldg(F.z + k), p, q);
     wait_tile_free(P.ctrl, T);
     unsigned char* a_hi = P.smem + P.L->a1 + b * (2 * OPER1_BYTES);
-    if constexpr (H16) app_row_bf16(F, q, a_hi, a_hi + OPER1_BYTES, row);
-    else app_row(F, q, a_hi, a_hi + OPER1_BYTES, row);
+    app_row<H16>(F, q, a_hi, a_hi + OPER1_BYTES, row);
     P.smem[P.L->mslot + b * TM + row] = (unsigned char)sid;
     reinterpret_cast<float*>(P.smem + P.L->mw)[b * TM + row] = Q.qw[P.lane];
     fence_async_smem();                  // generic-proxy writes -> visible to the tensor core
@@ -409,58 +310,6 @@ __device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R,
   return alpha;
 }
 
-// One claimed step (32 samples) of the ray described by `rec`: see RayRec.
-template <bool H16>
-__device__ __forceinline__ void process_step(const ProdCtx& P, const FieldDev& F, const BatchDev& B,
-                                             Slot* slots, RayRec* rec, int s, WarpQ& Q) {
-  const int lane = P.lane, S = F.S, k = s * 32 + lane;
-  const int slot_id = *reinterpret_cast<volatile int*>(&rec->slot_id);
-  const long long ray = *reinterpret_cast<volatile long long*>(&rec->ray);
-  Slot* slot = slots + slot_id;
-  RaySm R;
-  R.o[0] = slot->o[0]; R.o[1] = slot->o[1]; R.o[2] = slot->o[2];
-  R.vd[0] = slot->vd[0]; R.vd[1] = slot->vd[1]; R.vd[2] = slot->vd[2];
-  const bool skip = (unsigned)s >= *reinterpret_cast<volatile unsigned int*>(&rec->stop_at);
-  float alpha = 0.0f;
-  int marched = 0;
-  if (!skip && k < S) alpha = sample_alpha<H16>(F, R, k, S, marched);
-  const float f = (k < S) ? (1.0f - alpha) + 1e-10f : 1.0f;
-  const float inc = warp_scan_mul(f, lane);
-  float exc = __shfl_up_sync(0xffffffffu, inc, 1);
-  if (lane == 0) exc = 1.0f;
-  const float Ploc = __shfl_sync(0xffffffffu, inc, 31);
-  if (lane == 0) {
-    *reinterpret_cast<volatile float*>(&rec->P[s]) = skip ? 0.0f : Ploc;
-    __threadfence_block();
-    atomicOr(&rec->ready, 1u << s);
-  }
-  // carry = ((1 * P[0]) * P[1]) ... * P[s-1], the sequential order
-  float carry = 1.0f;
-  if (!skip) {
-    const unsigned need = s ? (0xffffffffu >> (32 - s)) : 0u;
-    while ((*reinterpret_cast<volatile unsigned int*>(&rec->ready) & need) != need) { }
-    __threadfence_block();
-    for (int j = 0; j < s; ++j) carry *= *reinterpret_cast<volatile float*>(&rec->P[j]);
-  }
-  const bool live = !skip && !(carry < T_EPS);                  // a terminated ray's later steps contribute nothing
-  const float wgt = live ? alpha * (carry * exc) : 0.0f;
-  const float zk = (k < S) ? __ldg(F.z + k) : 0.0f;
-  const float acc_s = warp_sum((live && k < S) ? wgt : 0.0f);
-  const float dep_s = warp_sum((live && k < S) ? wgt * zk : 0.0f);
-  const int marched_s = (int)warp_sum(live ? (float)marched : 0.0f);
-  if (B.weights && k < S) B.weights[(size_t)ray * S + k] = wgt;
-  if (live && carry * Ploc < T_EPS && lane == 0) atomicMin(&rec->stop_at, (unsigned)(s + 1));
-  const bool on = live && (k < S) && (wgt > F.weight_thres);    // tensorBase.py:622
-  const unsigned m = __ballot_sync(0xffffffffu, on);
-  if (lane == 0) {
-    rec->accs[s] = acc_s; rec->deps[s] = dep_s; rec->marched[s] = marched_s;
-    if (m) atomicAdd(&slot->pending, __popc(m));                // before `done`: the owner drops its token after it
-    __threadfence_block();
-    atomicOr(&rec->done, 1u << s);
-  }
-  queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
-}
-
 // =================================================================================================
 // PE = the field has positional encodings (fea_pe > 0 or view_pe > 0): basis_mat is its own tensor-core
 // product (layer 0), the consumers build the encoded layer-1 input chunk by chunk in registers, layer 1's weight
@@ -484,7 +333,7 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
     mbar_init(smem_u32(&ctrl->full[0]), TM);
     mbar_init(smem_u32(&ctrl->full[1]), TM);
     if (PE) mbar_init(smem_u32(&ctrl->wrdy), 1);
-    ctrl->cursor = 0; ctrl->prod_done = 0; ctrl->draw_done = 0; ctrl->n_tiles_final = 0; ctrl->done = 0;
+    ctrl->cursor = 0; ctrl->prod_done = 0; ctrl->n_tiles_final = 0; ctrl->done = 0;
     ctrl->released = 0;
     constexpr uint32_t bytes = PE ? PE_RESIDENT : PREP_BYTES;
     mbar_expect_tx(smem_u32(&ctrl->bar_w), bytes);
@@ -495,8 +344,6 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
   }
   for (int e = tid; e < MAX_PROD * NSLOT * (int)sizeof(Slot) / 4; e += THREADS)
     reinterpret_cast<int*>(slots)[e] = 0;
-  if (LRF_STEAL && tid < nprod)                                      // no ray open: nothing to claim
-    reinterpret_cast<RayRec*>(smem + L.recs)[tid].next_step = 0x40000000u;
   {  // K padding 72..79 of both A1 tiles (hi and lo) is zero for the whole launch
     const float zero[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     for (int e = tid; e < 2 * TM; e += THREADS) {
@@ -527,11 +374,6 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
     Q.qs = mine + QCAP * 6;
     Q.qn = 0; Q.n_app = 0;
     float* alpha_s = reinterpret_cast<float*>(mine + L.alpha);
-    RayRec* recs = reinterpret_cast<RayRec*>(smem + L.recs);
-    RayRec* rec = recs + prod_id;
-    const int n_steps = (S + 31) >> 5;
-    const bool stepwise = LRF_STEAL && !floater && n_steps <= MAXST;   // else: the owner marches its ray alone
-    const unsigned full_mask = n_steps >= 32 ? 0xffffffffu : ((1u << n_steps) - 1u);
     unsigned long long n_march = 0;
     int next_slot = 0;
     for (;;) {
@@ -589,103 +431,61 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
       }
       __syncwarp();
       float acc = 0.0f, dep = 0.0f;
-      if (stepwise) {
-        // -- march by claimed steps (tensorBase.py:581-615); idle producers of this CTA may take steps --
-        if (lane == 0) {
-          rec->slot_id = slot_id; rec->ray = ray;
-          rec->stop_at = (unsigned)n_steps; rec->ready = 0u; rec->done = 0u;
-          __threadfence_block();
-          *reinterpret_cast<volatile unsigned int*>(&rec->next_step) = 0u;     // opens the ray for claims
+      // -- march (tensorBase.py:581-615) ------------------------------------------------------------
+      float carry = 1.0f, acc_p = 0.0f, dep_p = 0.0f, idx_p = 0.0f;
+      int k0 = 0, marched = 0;
+      float* wo = B.weights ? B.weights + (size_t)ray * S : nullptr;
+      for (; k0 < S; k0 += 32) {
+        const int k = k0 + lane;
+        float alpha = 0.0f;
+        if (k < S) alpha = sample_alpha<H16>(F, R, k, S, marched);
+        const float f = (k < S) ? (1.0f - alpha) + 1e-10f : 1.0f;
+        const float inc = warp_scan_mul(f, lane);
+        float exc = __shfl_up_sync(0xffffffffu, inc, 1);
+        if (lane == 0) exc = 1.0f;
+        const float wgt = alpha * (carry * exc);
+        if (k < S) {
+          acc_p += wgt;
+          dep_p += wgt * __ldg(F.z + k);
+          idx_p += wgt * (float)k;
+          if (floater) alpha_s[k] = alpha;
+          else if (wo) wo[k] = wgt;
         }
+        carry *= __shfl_sync(0xffffffffu, inc, 31);
+        if (!floater) {
+          const bool on = (k < S) && (wgt > F.weight_thres);          // tensorBase.py:622
+          const unsigned m = __ballot_sync(0xffffffffu, on);
+          if (lane == 0 && m) atomicAdd(&slot->pending, __popc(m));
+          queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
+          if (carry < T_EPS) { k0 += 32; break; }                      // early ray termination
+        }
+      }
+      if (!floater && wo)
+        for (int k = k0 + lane; k < S; k += 32) wo[k] = 0.0f;          // terminated tail
+      acc = warp_sum(acc_p); dep = warp_sum(dep_p);
+      if (floater) {                                                   // tensorBase.py:617-620
+        const float lim = warp_sum(idx_p) * B.floater_thresh;
         __syncwarp();
-        for (;;) {
-          unsigned int st = 0;
-          if (lane == 0) st = atomicAdd(&rec->next_step, 1u);
-          st = __shfl_sync(0xffffffffu, st, 0);
-          if (st >= (unsigned)n_steps) break;
-          if (st >= *reinterpret_cast<volatile unsigned int*>(&rec->stop_at)) {
-            // the ray has terminated (T < 1e-10): close it -- this step and every unclaimed one contribute
-            // nothing (steps a helper has already claimed past this point skip themselves)
-            unsigned int rem = 0;
-            if (lane == 0) rem = atomicExch(&rec->next_step, 0x40000000u);
-            rem = min(__shfl_sync(0xffffffffu, rem, 0), (unsigned)n_steps);
-            unsigned int mask = 1u << st;
-            for (unsigned int j = rem; j < (unsigned)n_steps; ++j) mask |= 1u << j;
-            if (lane < n_steps && ((mask >> lane) & 1u)) {
-              rec->accs[lane] = 0.0f; rec->deps[lane] = 0.0f; rec->marched[lane] = 0;
-              *reinterpret_cast<volatile float*>(&rec->P[lane]) = 0.0f;
-            }
-            if (B.weights)
-              for (int k = (int)st * 32 + lane; k < S; k += 32)
-                if ((mask >> (k >> 5)) & 1u) B.weights[(size_t)ray * S + k] = 0.0f;
-            __syncwarp();
-            if (lane == 0) { __threadfence_block(); atomicOr(&rec->ready, mask); atomicOr(&rec->done, mask); }
-            break;
-          }
-          process_step<H16>(P, F, B, slots, rec, (int)st, Q);
-        }
-        while (*reinterpret_cast<volatile unsigned int*>(&rec->done) != full_mask) { }   // helpers' steps
-        __threadfence_block();
-        int marched = 0;
-        for (int j = 0; j < n_steps; ++j) { acc += rec->accs[j]; dep += rec->deps[j]; marched += rec->marched[j]; }
-        n_march += (unsigned long long)marched;
-      } else {
-        // -- sequential march of the whole ray by its owner (floater filter, very long sample tables) ----
-        float carry = 1.0f, acc_p = 0.0f, dep_p = 0.0f, idx_p = 0.0f;
-        int k0 = 0, marched = 0;
-        float* wo = B.weights ? B.weights + (size_t)ray * S : nullptr;
-        for (; k0 < S; k0 += 32) {
-          const int k = k0 + lane;
-          float alpha = 0.0f;
-          if (k < S) alpha = sample_alpha<H16>(F, R, k, S, marched);
-          const float f = (k < S) ? (1.0f - alpha) + 1e-10f : 1.0f;
+        float c2 = 1.0f;
+        for (int kb = 0; kb < S; kb += 32) {
+          const int k = kb + lane;
+          float a = (k < S) ? alpha_s[k] : 0.0f;
+          if ((float)k < lim) a = 0.0f;
+          if (k == S - 1) a = 1.0f;
+          const float f = (k < S) ? (1.0f - a) + 1e-10f : 1.0f;
           const float inc = warp_scan_mul(f, lane);
           float exc = __shfl_up_sync(0xffffffffu, inc, 1);
           if (lane == 0) exc = 1.0f;
-          const float wgt = alpha * (carry * exc);
-          if (k < S) {
-            acc_p += wgt;
-            dep_p += wgt * __ldg(F.z + k);
-            idx_p += wgt * (float)k;
-            if (floater) alpha_s[k] = alpha;
-            else if (wo) wo[k] = wgt;
-          }
-          carry *= __shfl_sync(0xffffffffu, inc, 31);
-          if (!floater) {
-            const bool on = (k < S) && (wgt > F.weight_thres);          // tensorBase.py:622
-            const unsigned m = __ballot_sync(0xffffffffu, on);
-            if (lane == 0 && m) atomicAdd(&slot->pending, __popc(m));
-            queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
-            if (carry < T_EPS) { k0 += 32; break; }                      // early ray termination
-          }
+          const float wgt = a * (c2 * exc);
+          c2 *= __shfl_sync(0xffffffffu, inc, 31);
+          if (k < S && wo) wo[k] = wgt;
+          const bool on = (k < S) && (wgt > F.weight_thres);
+          const unsigned m = __ballot_sync(0xffffffffu, on);
+          if (lane == 0 && m) atomicAdd(&slot->pending, __popc(m));
+          queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
         }
-        if (!floater && wo)
-          for (int k = k0 + lane; k < S; k += 32) wo[k] = 0.0f;          // terminated tail
-        acc = warp_sum(acc_p); dep = warp_sum(dep_p);
-        if (floater) {                                                   // tensorBase.py:617-620
-          const float lim = warp_sum(idx_p) * B.floater_thresh;
-          __syncwarp();
-          float c2 = 1.0f;
-          for (int kb = 0; kb < S; kb += 32) {
-            const int k = kb + lane;
-            float a = (k < S) ? alpha_s[k] : 0.0f;
-            if ((float)k < lim) a = 0.0f;
-            if (k == S - 1) a = 1.0f;
-            const float f = (k < S) ? (1.0f - a) + 1e-10f : 1.0f;
-            const float inc = warp_scan_mul(f, lane);
-            float exc = __shfl_up_sync(0xffffffffu, inc, 1);
-            if (lane == 0) exc = 1.0f;
-            const float wgt = a * (c2 * exc);
-            c2 *= __shfl_sync(0xffffffffu, inc, 31);
-            if (k < S && wo) wo[k] = wgt;
-            const bool on = (k < S) && (wgt > F.weight_thres);
-            const unsigned m = __ballot_sync(0xffffffffu, on);
-            if (lane == 0 && m) atomicAdd(&slot->pending, __popc(m));
-            queue_push<H16>(P, F, slots, Q, m, on, k, wgt, slot_id);
-          }
-        }
-        n_march += (unsigned long long)warp_sum((float)marched);
       }
+      n_march += (unsigned long long)warp_sum((float)marched);
       // -- depth now, colour when the last row of this ray has been composited ---------------------
       if (lane == 0) {
         float dpt = __fdiv_rn(dep, R.nrm) * R.blend;                   // tensorBase.py:615
@@ -698,30 +498,6 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
         if (old == 1) { __threadfence_block(); finalize_slot(B, slot); }
       }
       __syncwarp();
-    }
-    // -- the global ray queue is empty: help the rays still in flight in this CTA, step by step ------
-    if (lane == 0) { __threadfence_block(); atomicAdd(&ctrl->draw_done, 1u); }
-    if (stepwise) {
-      for (;;) {
-        bool any = false;
-        for (int r = 1; r < nprod; ++r) {
-          RayRec* other = recs + ((prod_id + r) % nprod);
-          for (;;) {
-            if (*reinterpret_cast<volatile unsigned int*>(&other->next_step) >= (unsigned)n_steps) break;
-            unsigned int st = 0;
-            if (lane == 0) st = atomicAdd(&other->next_step, 1u);
-            st = __shfl_sync(0xffffffffu, st, 0);
-            if (st >= (unsigned)n_steps) break;
-            __threadfence_block();
-            process_step<H16>(P, F, B, slots, other, (int)st, Q);
-            any = true;
-          }
-        }
-        if (!any) {
-          if (*reinterpret_cast<volatile unsigned int*>(&ctrl->draw_done) >= (unsigned)nprod) break;
-          __nanosleep(200);
-        }
-      }
     }
     if (Q.qn > 0) { flush_rows<H16>(P, F, slots, Q, Q.qn); Q.qn = 0; }
     // -- the last producer completes the open tile and publishes the tile count ----------------------
@@ -764,112 +540,109 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
       }
       if (stop) break;
       const uint32_t a1 = smem_u32(smem + L.a1 + b * (2 * OPER1_BYTES));
-#pragma unroll 1
-      for (int hp = 0; hp < 2 / N_CWG; ++hp) {
-        const int h = hp * N_CWG + wg;                  // tile rows 64 h .. 64 h + 63
-        const uint32_t a_hi = a1 + (uint32_t)h * 8u * K1_CHUNKS * 128u, a_lo = a_hi + OPER1_BYTES;
-        float acc[64];
-        if (PE) {
-          // -- layer 0: the 27 basis features; then the encoded layer-1 input, 64 columns at a time ---------
-          // x = [a, sin(a_d 2^f) (d-major, f-minor), cos(...)]   (tensorBase.py:14-21,115-125); zeros when !refine
-          {
-            float a0[16];
+      const int h = wg;                                 // tile rows 64 h .. 64 h + 63
+      const uint32_t a_hi = a1 + (uint32_t)h * 8u * K1_CHUNKS * 128u, a_lo = a_hi + OPER1_BYTES;
+      float acc[64];
+      if (PE) {
+        // -- layer 0: the 27 basis features; then the encoded layer-1 input, 64 columns at a time ---------
+        // x = [a, sin(a_d 2^f) (d-major, f-minor), cos(...)]   (tensorBase.py:14-21,115-125); zeros when !refine
+        {
+          float a0[16];
 #pragma unroll
-            for (int i = 0; i < 16; ++i) a0[i] = 0.0f;
-            const uint32_t sbo = (uint32_t)K1_CHUNKS * 128u;
-            wgmma_fence();
-            for (int ks = 0; ks < K1 / 16; ++ks) {
-              const uint32_t ko = (uint32_t)ks * 256u;
-              const uint64_t ah = gmma_desc(a_hi + ko, 128u, sbo), al = gmma_desc(a_lo + ko, 128u, sbo);
-              const uint64_t bh = gmma_desc(prep_a + PE_B0HI + ko, 128u, sbo), bl = gmma_desc(prep_a + PE_B0LO + ko, 128u, sbo);
-              wgmma_n32_ss(a0, ah, bh, ks > 0 ? 1u : 0u);
-              wgmma_n32_ss(a0, ah, bl, 1u);
-              wgmma_n32_ss(a0, al, bh, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait_all();
-            fence_regs(a0);
-            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");   // the previous half's reads of xa are done
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-              for (int j = 0; j < 2; ++j) {
-                xa[wg_row(j) * XA_LD + 8 * i + 2 * q] = a0[4 * i + 2 * j];
-                xa[wg_row(j) * XA_LD + 8 * i + 2 * q + 1] = a0[4 * i + 2 * j + 1];
-              }
-            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+          for (int i = 0; i < 16; ++i) a0[i] = 0.0f;
+          const uint32_t sbo = (uint32_t)K1_CHUNKS * 128u;
+          wgmma_fence();
+          for (int ks = 0; ks < K1 / 16; ++ks) {
+            const uint32_t ko = (uint32_t)ks * 256u;
+            const uint64_t ah = gmma_desc(a_hi + ko, 128u, sbo), al = gmma_desc(a_lo + ko, 128u, sbo);
+            const uint64_t bh = gmma_desc(prep_a + PE_B0HI + ko, 128u, sbo), bl = gmma_desc(prep_a + PE_B0LO + ko, 128u, sbo);
+            wgmma_n32_ss(a0, ah, bh, ks > 0 ? 1u : 0u);
+            wgmma_n32_ss(a0, ah, bl, 1u);
+            wgmma_n32_ss(a0, al, bh, 1u);
           }
-          const int Fp = F.fea_pe, nsin = APP_DIM * Fp;
-          auto enc = [&](int j, int k) -> float {        // encoded input k of fragment row j
-            const float* a = xa + wg_row(j) * XA_LD;
-            if (k < APP_DIM) return a[k];
-            if (B.refine && k < APP_DIM + 2 * nsin) {
-              const int e = (k - APP_DIM) % nsin, d = e / Fp, f = e - d * Fp;
-              const float ang = a[d] * (float)(1 << f);
-              return (k - APP_DIM) < nsin ? sinf(ang) : cosf(ang);
+          wgmma_commit();
+          wgmma_wait_all();
+          fence_regs(a0);
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");   // the previous half's reads of xa are done
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              xa[wg_row(j) * XA_LD + 8 * i + 2 * q] = a0[4 * i + 2 * j];
+              xa[wg_row(j) * XA_LD + 8 * i + 2 * q + 1] = a0[4 * i + 2 * j + 1];
             }
-            return 0.0f;
-          };
-#pragma unroll
-          for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
-#pragma unroll 1
-          for (int c = 0; c < nch; ++c) {
-            uint32_t xh[PE_KC / 16][4], xl[PE_KC / 16][4];
-#pragma unroll
-            for (int ks = 0; ks < PE_KC / 16; ++ks)
-#pragma unroll
-              for (int r = 0; r < 4; ++r) {               // A fragment register r: row j = r & 1, K 16 ks + 8 (r >> 1) + 2q
-                const int k = c * PE_KC + 16 * ks + 8 * (r >> 1) + 2 * q;
-                split2(enc(r & 1, k), enc(r & 1, k + 1), xh[ks][r], xl[ks][r]);
-              }
-            mbar_wait(wrdy, wuse & 1u);                   // weight chunk c is in shared memory
-            const uint32_t sbo = (uint32_t)(PE_KC / 8) * 128u;
-            wgmma_fence();
-#pragma unroll
-            for (int ks = 0; ks < PE_KC / 16; ++ks) {
-              const uint32_t ko = (uint32_t)ks * 256u;
-              const uint64_t bh = gmma_desc(wbuf + ko, 128u, sbo), bl = gmma_desc(wbuf + PE_WC_BYTES + ko, 128u, sbo);
-              wgmma_n128_rs(acc, xh[ks], bh, 1u);
-              wgmma_n128_rs(acc, xh[ks], bl, 1u);
-              wgmma_n128_rs(acc, xl[ks], bh, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait_all();
-            fence_regs(acc);
-            ++wuse;
-            asm volatile("bar.sync 1, %0;" ::"n"(N_CONS * 32) : "memory");   // every consumer is done with the chunk
-            if (ctid == 0) {                              // the next chunk (of this tile, or chunk 0 of the next)
-              mbar_expect_tx(wrdy, 2 * PE_WC_BYTES);
-              tma_bulk_g2s(wbuf, w1_g + (size_t)((c + 1) % nch) * 2 * PE_WC_BYTES, 2 * PE_WC_BYTES, wrdy);
-            }
-          }
-        } else {
-          mlp_gemm_n128(acc, a_hi, a_lo, prep_a + PREP_B1HI, prep_a + PREP_B1LO, K1 / 16, K1_CHUNKS);
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
         }
-        float sc[2][3];
-        mlp_layers23(acc, tail, prep_a + (PE ? PE_B2HI : PREP_B2HI), prep_a + (PE ? PE_B2LO : PREP_B2LO), sc);
-        // -- composite (tensorBase.py:632): w * rgb into the ray's fixed-point accumulators -------------
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int row = 64 * h + wg_row(j);
-          const int my_slot = smem[L.mslot + b * TM + row];
-          if (q != 0 || my_slot == 0xFF) continue;
-          const float my_w = reinterpret_cast<const float*>(smem + L.mw)[b * TM + row];
-          Slot* sl = slots + my_slot;
-#pragma unroll
-          for (int c = 0; c < 3; ++c) {
-            float v = sc[j][c];
-            if (PE) v += sl->vterm[c];
-            else v += W3_s[c * W3_LD + FC] * sl->vd[0] + W3_s[c * W3_LD + FC + 1] * sl->vd[1] +
-                      W3_s[c * W3_LD + FC + 2] * sl->vd[2];
-            v += b3_s[c];
-            v = __fdiv_rn(1.0f, 1.0f + expf(-v));
-            atomicAdd(&sl->rgb[c], __float2uint_rn(my_w * v * FIX_SCALE));
+        const int Fp = F.fea_pe, nsin = APP_DIM * Fp;
+        auto enc = [&](int j, int k) -> float {        // encoded input k of fragment row j
+          const float* a = xa + wg_row(j) * XA_LD;
+          if (k < APP_DIM) return a[k];
+          if (B.refine && k < APP_DIM + 2 * nsin) {
+            const int e = (k - APP_DIM) % nsin, d = e / Fp, f = e - d * Fp;
+            const float ang = a[d] * (float)(1 << f);
+            return (k - APP_DIM) < nsin ? sinf(ang) : cosf(ang);
           }
-          __threadfence_block();
-          const int old = atomicSub(&sl->pending, 1);
-          if (old == 1) { __threadfence_block(); finalize_slot(B, sl); }
+          return 0.0f;
+        };
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+#pragma unroll 1
+        for (int c = 0; c < nch; ++c) {
+          uint32_t xh[PE_KC / 16][4], xl[PE_KC / 16][4];
+#pragma unroll
+          for (int ks = 0; ks < PE_KC / 16; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {               // A fragment register r: row j = r & 1, K 16 ks + 8 (r >> 1) + 2q
+              const int k = c * PE_KC + 16 * ks + 8 * (r >> 1) + 2 * q;
+              split2(enc(r & 1, k), enc(r & 1, k + 1), xh[ks][r], xl[ks][r]);
+            }
+          mbar_wait(wrdy, wuse & 1u);                   // weight chunk c is in shared memory
+          const uint32_t sbo = (uint32_t)(PE_KC / 8) * 128u;
+          wgmma_fence();
+#pragma unroll
+          for (int ks = 0; ks < PE_KC / 16; ++ks) {
+            const uint32_t ko = (uint32_t)ks * 256u;
+            const uint64_t bh = gmma_desc(wbuf + ko, 128u, sbo), bl = gmma_desc(wbuf + PE_WC_BYTES + ko, 128u, sbo);
+            wgmma_n128_rs(acc, xh[ks], bh, 1u);
+            wgmma_n128_rs(acc, xh[ks], bl, 1u);
+            wgmma_n128_rs(acc, xl[ks], bh, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait_all();
+          fence_regs(acc);
+          ++wuse;
+          asm volatile("bar.sync 1, %0;" ::"n"(N_CONS * 32) : "memory");   // every consumer is done with the chunk
+          if (ctid == 0) {                              // the next chunk (of this tile, or chunk 0 of the next)
+            mbar_expect_tx(wrdy, 2 * PE_WC_BYTES);
+            tma_bulk_g2s(wbuf, w1_g + (size_t)((c + 1) % nch) * 2 * PE_WC_BYTES, 2 * PE_WC_BYTES, wrdy);
+          }
         }
+      } else {
+        mlp_gemm_n128(acc, a_hi, a_lo, prep_a + PREP_B1HI, prep_a + PREP_B1LO, K1 / 16, K1_CHUNKS);
+      }
+      float sc[2][3];
+      mlp_layers23(acc, tail, prep_a + (PE ? PE_B2HI : PREP_B2HI), prep_a + (PE ? PE_B2LO : PREP_B2LO), sc);
+      // -- composite (tensorBase.py:632): w * rgb into the ray's fixed-point accumulators -------------
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int row = 64 * h + wg_row(j);
+        const int my_slot = smem[L.mslot + b * TM + row];
+        if (q != 0 || my_slot == 0xFF) continue;
+        const float my_w = reinterpret_cast<const float*>(smem + L.mw)[b * TM + row];
+        Slot* sl = slots + my_slot;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          float v = sc[j][c];
+          if (PE) v += sl->vterm[c];
+          else v += W3_s[c * W3_LD + FC] * sl->vd[0] + W3_s[c * W3_LD + FC + 1] * sl->vd[1] +
+                    W3_s[c * W3_LD + FC + 2] * sl->vd[2];
+          v += b3_s[c];
+          v = __fdiv_rn(1.0f, 1.0f + expf(-v));
+          atomicAdd(&sl->rgb[c], __float2uint_rn(my_w * v * FIX_SCALE));
+        }
+        __threadfence_block();
+        const int old = atomicSub(&sl->pending, 1);
+        if (old == 1) { __threadfence_block(); finalize_slot(B, sl); }
       }
       // the A tile and its row metadata have been read: the producers may rewrite buffer b
       asm volatile("bar.sync 1, %0;" ::"n"(N_CONS * 32) : "memory");
@@ -899,13 +672,9 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
 // ---- host-side launcher --------------------------------------------------------------------------
 int render_threads() { return THREADS; }
 
+// the most producer warps whose queues fit max_smem (the floater filter's alpha tables grow with S)
 static int pick_nprod(int S, bool floater, int max_smem, bool pe = false) {
-  int cap = MAX_PROD;
-  if (const char* e = getenv("LRF_NPROD")) {      // tuning / debugging knob
-    const int v = atoi(e);
-    if (v >= 1 && v < cap) cap = v;
-  }
-  for (int n = cap; n >= 1; --n)
+  for (int n = MAX_PROD; n >= 1; --n)
     if (smem_v3(S, floater, n, pe).total <= max_smem) return n;
   return 0;
 }

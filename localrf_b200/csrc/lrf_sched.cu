@@ -36,7 +36,7 @@ __global__ void dense_alpha_kernel(const FieldDev F, const float3 amax, int gx, 
     }
     float sigma = 0.0f;
     if (!F.alpha_vol || alpha_mask(F, p) > 0.0f)
-      sigma = feature2density(density_feature(F, q), F.density_shift, F.act);
+      sigma = feature2density(density_feature_t<false>(F, q), F.density_shift, F.act);
     alpha[e] = 1.0f - expf(-sigma * length);
   }
 }
