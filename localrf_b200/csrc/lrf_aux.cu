@@ -101,6 +101,26 @@ mlp_kernel(const float* __restrict__ prep_g, const float* __restrict__ feats,
 }
 
 // ---- small kernels ------------------------------------------------------------------------------
+// element `off` (bytes) of a bf16 hi / lo operand image pair: v = hi + lo
+__device__ __forceinline__ void put_hi_lo(unsigned char* hi_img, unsigned char* lo_img, int off, float v) {
+  const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+  const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
+  *reinterpret_cast<__nv_bfloat16*>(hi_img + off) = hi;
+  *reinterpret_cast<__nv_bfloat16*>(lo_img + off) = lo;
+}
+
+// the fp32 tail of a prepared block: b1, b2, the first n_w3 columns of each row of W3 [3][w3_ld] (zero
+// beyond), b3; thread t of `stride`
+__device__ __forceinline__ void fill_tail(float* tail, const float* b1, const float* b2, const float* w3, int w3_ld,
+                                          int n_w3, const float* b3, int t, int stride) {
+  for (int e = t; e < FC; e += stride) { tail[TAIL_B1 + e] = b1[e]; tail[TAIL_B2 + e] = b2[e]; }
+  for (int e = t; e < 3 * W3_LD; e += stride) {
+    const int c = e / W3_LD, n = e - c * W3_LD;
+    tail[TAIL_W3 + e] = n < n_w3 ? w3[c * w3_ld + n] : 0.0f;
+  }
+  for (int e = t; e < 4; e += stride) tail[TAIL_B3 + e] = e < 3 ? b3[e] : 0.0f;
+}
+
 // prepared block: bf16 hi/lo operand images of W1B = W1 @ basis and W2, fp32 biases and W3
 __global__ void prepare_kernel(const float* __restrict__ basis, const float* __restrict__ w1,
                                const float* __restrict__ b1, const float* __restrict__ w2,
@@ -113,28 +133,13 @@ __global__ void prepare_kernel(const float* __restrict__ basis, const float* __r
     float s = 0.0f;
     if (k < NF)
       for (int j = 0; j < APP_DIM; ++j) s = fmaf(w1[n * APP_DIM + j], basis[j * NF + k], s);
-    const __nv_bfloat16 hi = __float2bfloat16_rn(s);
-    const __nv_bfloat16 lo = __float2bfloat16_rn(s - __bfloat162float(hi));
-    const int off = oper_offset(n, k, K1_CHUNKS);
-    *reinterpret_cast<__nv_bfloat16*>(prep + PREP_B1HI + off) = hi;
-    *reinterpret_cast<__nv_bfloat16*>(prep + PREP_B1LO + off) = lo;
+    put_hi_lo(prep + PREP_B1HI, prep + PREP_B1LO, oper_offset(n, k, K1_CHUNKS), s);
   }
   for (int e = t; e < FC * FC; e += stride) {
     const int n = e / FC, k = e - n * FC;
-    const float s = w2[n * FC + k];
-    const __nv_bfloat16 hi = __float2bfloat16_rn(s);
-    const __nv_bfloat16 lo = __float2bfloat16_rn(s - __bfloat162float(hi));
-    const int off = oper_offset(n, k, K2_CHUNKS);
-    *reinterpret_cast<__nv_bfloat16*>(prep + PREP_B2HI + off) = hi;
-    *reinterpret_cast<__nv_bfloat16*>(prep + PREP_B2LO + off) = lo;
+    put_hi_lo(prep + PREP_B2HI, prep + PREP_B2LO, oper_offset(n, k, K2_CHUNKS), w2[n * FC + k]);
   }
-  float* tail = reinterpret_cast<float*>(prep + PREP_TAIL);
-  for (int e = t; e < FC; e += stride) { tail[TAIL_B1 + e] = b1[e]; tail[TAIL_B2 + e] = b2[e]; }
-  for (int e = t; e < 3 * W3_LD; e += stride) {
-    const int c = e / W3_LD, n = e - c * W3_LD;
-    tail[TAIL_W3 + e] = n < FC + 3 ? w3[c * (FC + 3) + n] : 0.0f;
-  }
-  for (int e = t; e < 4; e += stride) tail[TAIL_B3 + e] = e < 3 ? b3[e] : 0.0f;
+  fill_tail(reinterpret_cast<float*>(prep + PREP_TAIL), b1, b2, w3, FC + 3, FC + 3, b3, t, stride);
 }
 
 // prepared block of a field with positional encodings (layout: lrf_common.cuh)
@@ -145,35 +150,24 @@ __global__ void prepare_pe_kernel(const float* __restrict__ basis, const float* 
                                   unsigned char* __restrict__ prep) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int stride = gridDim.x * blockDim.x;
-  auto put = [&](unsigned char* hi_img, unsigned char* lo_img, int off, float v) {
-    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-    const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-    *reinterpret_cast<__nv_bfloat16*>(hi_img + off) = hi;
-    *reinterpret_cast<__nv_bfloat16*>(lo_img + off) = lo;
-  };
   for (int e = t; e < PE_N0 * K1; e += stride) {
     const int n = e / K1, k = e - n * K1;
-    put(prep + PE_B0HI, prep + PE_B0LO, oper_offset(n, k, K1_CHUNKS), (n < APP_DIM && k < NF) ? basis[n * NF + k] : 0.0f);
+    put_hi_lo(prep + PE_B0HI, prep + PE_B0LO, oper_offset(n, k, K1_CHUNKS),
+              (n < APP_DIM && k < NF) ? basis[n * NF + k] : 0.0f);
   }
   for (int e = t; e < FC * FC; e += stride) {
     const int n = e / FC, k = e - n * FC;
-    put(prep + PE_B2HI, prep + PE_B2LO, oper_offset(n, k, K2_CHUNKS), w2[n * FC + k]);
+    put_hi_lo(prep + PE_B2HI, prep + PE_B2LO, oper_offset(n, k, K2_CHUNKS), w2[n * FC + k]);
   }
   const int in_dim = pe_in_dim(fea_pe), nch = pe_chunks(fea_pe);
   for (int e = t; e < nch * FC * PE_KC; e += stride) {
     const int c = e / (FC * PE_KC), r = e - c * FC * PE_KC, n = r / PE_KC, kk = r - n * PE_KC;
     const int k = c * PE_KC + kk;
     unsigned char* img = prep + PE_W1 + (size_t)c * 2 * PE_WC_BYTES;
-    put(img, img + PE_WC_BYTES, oper_offset(n, kk, PE_KC / 8), k < in_dim ? w1[n * in_dim + k] : 0.0f);
+    put_hi_lo(img, img + PE_WC_BYTES, oper_offset(n, kk, PE_KC / 8), k < in_dim ? w1[n * in_dim + k] : 0.0f);
   }
-  float* tail = reinterpret_cast<float*>(prep + PE_TAIL);
-  const int w3_ld = FC + 3 * (1 + 2 * view_pe);
-  for (int e = t; e < FC; e += stride) { tail[TAIL_B1 + e] = b1[e]; tail[TAIL_B2 + e] = b2[e]; }
-  for (int e = t; e < 3 * W3_LD; e += stride) {
-    const int c = e / W3_LD, n = e - c * W3_LD;
-    tail[TAIL_W3 + e] = n < FC ? w3[c * w3_ld + n] : 0.0f;
-  }
-  for (int e = t; e < 4; e += stride) tail[TAIL_B3 + e] = e < 3 ? b3[e] : 0.0f;
+  // the view part of W3 is read from the module's own weight
+  fill_tail(reinterpret_cast<float*>(prep + PE_TAIL), b1, b2, w3, FC + 3 * (1 + 2 * view_pe), FC, b3, t, stride);
 }
 
 template <bool H16>      // H16: bf16 grid storage (LrfField.grid_dtype)

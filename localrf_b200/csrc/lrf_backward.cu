@@ -29,15 +29,12 @@
 
 namespace lrf {
 
-// prepared block of the backward (floats): folded layer 1 and W2, both transposed (k-major)
-constexpr int BP_W1BT = 0;                      // [NF][FC]   (W1 @ basis)^T
+// prepared block of the backward (floats): the forward's prepared block (lrf_common.cuh), whose bf16 images the
+// tensor-core shade step reads and whose fp32 tail (b1, b2, W3, b3) both shade steps read, then folded layer 1
+// and W2, both transposed (k-major), for the CUDA-core shade step
+constexpr int BP_W1BT = PREP_BYTES / 4;         // [NF][FC]   (W1 @ basis)^T
 constexpr int BP_W2T = BP_W1BT + NF * FC;       // [FC(k)][FC(n)]
-constexpr int BP_B1 = BP_W2T + FC * FC;
-constexpr int BP_B2 = BP_B1 + FC;
-constexpr int BP_W3 = BP_B2 + FC;               // [3][W3_LD]
-constexpr int BP_B3 = BP_W3 + 3 * W3_LD;
-constexpr int BP_FLOATS = BP_B3 + 4;
-constexpr size_t BP_TC_OFFSET = ((size_t)BP_FLOATS * sizeof(float) + 1023) & ~(size_t)1023;   // then the forward's bf16 operand block
+constexpr int BP_FLOATS = BP_W2T + FC * FC;
 
 struct BwdScratch {           // views into the caller's scratch block
   unsigned long long* count;  // number of shaded samples (zeroed per call)
@@ -92,37 +89,6 @@ __host__ inline size_t bwd_scratch_layout(long long n, int S, BwdScratch* out, u
   return off;
 }
 
-// ---- small device helpers --------------------------------------------------------------------------
-
-// d contract(p)/dp applied to dpc (ray_utils.py:9-12; amax routes the norm's gradient to the
-// component of largest magnitude)
-__device__ __forceinline__ void contract_bwd(float p0, float p1, float p2, float g0, float g1,
-                                             float g2, float& o0, float& o1, float& o2) {
-  float n = fmaxf(fmaxf(fabsf(p0), fabsf(p1)), fabsf(p2));
-  n = fmaxf(n, 1e-6f);
-  if (n <= 1.0f) { o0 = g0; o1 = g1; o2 = g2; return; }
-  const float s = __fdiv_rn(2.0f * n - 1.0f, n * n);
-  const float ds = -2.0f / (n * n) + 2.0f / (n * n * n);
-  const float dot = g0 * p0 + g1 * p1 + g2 * p2;
-  int j = 0;
-  float best = fabsf(p0);
-  if (fabsf(p1) > best) { j = 1; best = fabsf(p1); }
-  if (fabsf(p2) > best) { j = 2; }
-  o0 = s * g0; o1 = s * g1; o2 = s * g2;
-  const float pj = j == 0 ? p0 : (j == 1 ? p1 : p2);
-  const float extra = (pj >= 0.0f ? 1.0f : -1.0f) * ds * dot;
-  if (j == 0) o0 += extra; else if (j == 1) o1 += extra; else o2 += extra;
-}
-
-__device__ __forceinline__ void load_ray(const float* rays, long long ray, RaySm& R) {
-  const float* rp = rays + 6 * ray;
-  const float d0 = rp[3], d1 = rp[4], d2 = rp[5];
-  R.o[0] = rp[0]; R.o[1] = rp[1]; R.o[2] = rp[2];
-  R.nrm = sqrtf(d0 * d0 + d1 * d1 + d2 * d2);
-  R.vd[0] = __fdiv_rn(d0, R.nrm); R.vd[1] = __fdiv_rn(d1, R.nrm); R.vd[2] = __fdiv_rn(d2, R.nrm);
-  R.blend = 1.0f;
-}
-
 // ====================================================================================================
 // 1. march
 // ====================================================================================================
@@ -136,39 +102,22 @@ bwd_march_kernel(const FieldDev F, const BwdArgs A) {
   const long long n_warps = ((long long)gridDim.x * MARCH_THREADS) >> 5;
   for (long long ray = warp0; ray < A.n_rays; ray += n_warps) {
     RaySm R;
-    load_ray(A.rays, ray, R);
+    normalize_ray(A.rays + 6 * ray, A.rays + 6 * ray + 3, R);
     const float gsum = A.white_bg ? -(A.g_rgb[3 * ray] + A.g_rgb[3 * ray + 1] + A.g_rgb[3 * ray + 2]) : 0.0f;
     const float gd = A.g_depth[ray];
     const size_t base = (size_t)ray * S;
     float carry = 1.0f;
     for (int k0 = 0; k0 < S; k0 += 32) {
       const int k = k0 + lane;
-      float alpha = 0.0f, fe = 0.0f, z = 0.0f;
-      bool valid = false;
-      if (k < S) {
-        z = __ldg(F.z + k);
-        float p[3], q[3];
-        sample_pos(F, R, z, p, q);
-        valid = (k != S - 1);                                          // ray_valid[:, -1] = 0
-        if (valid && F.alpha_vol) valid = alpha_mask(F, p) > 0.0f;     // tensorBase.py:593-598
-        float sigma = 0.0f;
-        if (valid) { fe = density_feature_t<false>(F, q); sigma = feature2density(fe, F.density_shift, F.act); }
-        const float znext = (k + 1 < S) ? __ldg(F.z + k + 1) : z;
-        alpha = 1.0f - expf(-sigma * (znext - z) * F.distance_scale);   // tensorBase.py:610
-        if (k == S - 1) alpha = 1.0f;                                  // alpha[:, -1] = 1
-      }
-      const float f = (k < S) ? (1.0f - alpha) + 1e-10f : 1.0f;
-      const float inc = warp_scan_mul(f, lane);
-      float exc = __shfl_up_sync(0xffffffffu, inc, 1);
-      if (lane == 0) exc = 1.0f;
-      const float Tk = carry * exc;
-      const float wk = alpha * Tk;
-      carry *= __shfl_sync(0xffffffffu, inc, 31);
+      float alpha = 0.0f, fe, Tk, wk;
+      bool valid;
+      if (k < S) alpha = sample_alpha<false>(F, R, k, S, fe, valid);
+      transmittance_step(alpha, k < S, lane, carry, Tk, wk);
       const bool on = (k < S) && (wk > F.weight_thres);                // tensorBase.py:622
       if (k < S) {
         A.s.alpha[base + k] = alpha; A.s.T[base + k] = Tk; A.s.w[base + k] = wk;
         A.s.fe[base + k] = fe; A.s.valid[base + k] = valid ? 1 : 0;
-        A.s.gw[base + k] = gsum + gd * __fdiv_rn(z, R.nrm);            // d rgb_map(white bg) + d depth
+        A.s.gw[base + k] = gsum + gd * __fdiv_rn(__ldg(F.z + k), R.nrm);   // d rgb_map(white bg) + d depth
       }
       const unsigned m = __ballot_sync(0xffffffffu, on);
       if (m) {
@@ -292,15 +241,16 @@ bwd_shade_kernel(const FieldDev F, const BwdArgs A) {
   const uint32_t w1b_a = smem_u32(img), w2_a = w1b_a + 2 * OPER1_BYTES, scr_a = smem_u32(scr);
   const int wg = tid >> 7, q4 = tid & 3;
   if constexpr (TC) {
-    const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(A.bp) + BP_TC_OFFSET);
+    const uint4* src = reinterpret_cast<const uint4*>(A.bp);
     for (int e = tid; e < TC_IMG_BYTES / 16; e += SH_THREADS) reinterpret_cast<uint4*>(img)[e] = __ldg(src + e);
   } else {
     for (int e = tid; e < NF * FC; e += SH_THREADS) W1BT_s[(e / FC) * LDW + (e % FC)] = __ldg(A.bp + BP_W1BT + e);
     for (int e = tid; e < FC * FC; e += SH_THREADS) W2T_s[(e / FC) * LDW + (e % FC)] = __ldg(A.bp + BP_W2T + e);
   }
-  for (int e = tid; e < 3 * W3_LD; e += SH_THREADS) W3_s[e] = __ldg(A.bp + BP_W3 + e);
-  for (int e = tid; e < FC; e += SH_THREADS) { b1_s[e] = __ldg(A.bp + BP_B1 + e); b2_s[e] = __ldg(A.bp + BP_B2 + e); }
-  const float b3r[3] = {__ldg(A.bp + BP_B3), __ldg(A.bp + BP_B3 + 1), __ldg(A.bp + BP_B3 + 2)};
+  const float* tail = A.bp + PREP_TAIL / 4;
+  for (int e = tid; e < 3 * W3_LD; e += SH_THREADS) W3_s[e] = __ldg(tail + TAIL_W3 + e);
+  for (int e = tid; e < FC; e += SH_THREADS) { b1_s[e] = __ldg(tail + TAIL_B1 + e); b2_s[e] = __ldg(tail + TAIL_B2 + e); }
+  const float b3r[3] = {__ldg(tail + TAIL_B3), __ldg(tail + TAIL_B3 + 1), __ldg(tail + TAIL_B3 + 2)};
 
   // per-thread gradient accumulators, kept for the whole launch
   float accW2[8][8];      // dW2[n = 8 ts + i][k = tn + 16 j]
@@ -330,7 +280,7 @@ bwd_shade_kernel(const FieldDev F, const BwdArgs A) {
       if (tid < n_valid) { ray = A.s.app_ray[e0 + tid]; k = A.s.app_k[e0 + tid]; wk = A.s.w[(size_t)ray * S + k]; }
       ray_s[tid] = ray; kk_s[tid] = k; wk_s[tid] = wk;
       RaySm R;
-      load_ray(A.rays, ray, R);
+      normalize_ray(A.rays + 6 * (size_t)ray, A.rays + 6 * (size_t)ray + 3, R);
       const float z = __ldg(F.z + k);
       zk_s[tid] = z;
       float p[3], q[3];
@@ -691,7 +641,7 @@ bwd_density_kernel(const FieldDev F, const BwdArgs A) {
   const int n_chunks = (S + 31) / 32;
   for (long long ray = warp0; ray < A.n_rays; ray += n_warps) {
     RaySm R;
-    load_ray(A.rays, ray, R);
+    normalize_ray(A.rays + 6 * ray, A.rays + 6 * ray + 3, R);
     const float gd = A.g_depth[ray];
     const size_t base = (size_t)ray * S;
     float d_o[3] = {0.0f, 0.0f, 0.0f}, d_vd[3] = {0.0f, 0.0f, 0.0f};   // lane-partial sums
@@ -717,14 +667,7 @@ bwd_density_kernel(const FieldDev F, const BwdArgs A) {
         const float al = A.s.alpha[base + k];
         const float dalpha = gwk * A.s.T[base + k] - __fdiv_rn(excl, (1.0f - al) + 1e-10f);
         const float dsigma = dalpha * (1.0f - al) * (__ldg(F.z + k + 1) - zk) * F.distance_scale;
-        const float fe = A.s.fe[base + k];
-        float df;
-        if (F.act == 0) {
-          const float x = fe + F.density_shift;
-          df = dsigma * (x > 20.0f ? 1.0f : __fdiv_rn(1.0f, 1.0f + expf(-x)));
-        } else {
-          df = fe > 0.0f ? dsigma : 0.0f;
-        }
+        const float df = feature2density_grad(A.s.fe[base + k], F.density_shift, F.act, dsigma);
         if (df != 0.0f) {
           float p[3], q[3], dq[3] = {0.0f, 0.0f, 0.0f};
           sample_pos(F, R, zk, p, q);
@@ -759,11 +702,9 @@ bwd_density_kernel(const FieldDev F, const BwdArgs A) {
   }
 }
 
-// prepared block of the backward: folded layer 1 and W2 (both transposed), biases, W3
+// the backward's part of its prepared block: folded layer 1 and W2, both transposed
 __global__ void prepare_backward_kernel(const float* __restrict__ basis, const float* __restrict__ w1,
-                                        const float* __restrict__ b1, const float* __restrict__ w2,
-                                        const float* __restrict__ b2, const float* __restrict__ w3,
-                                        const float* __restrict__ b3, float* __restrict__ bp) {
+                                        const float* __restrict__ w2, float* __restrict__ bp) {
   const int t0 = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
   for (int e = t0; e < FC * NF; e += stride) {
     const int n = e / NF, t = e - n * NF;
@@ -775,16 +716,10 @@ __global__ void prepare_backward_kernel(const float* __restrict__ basis, const f
     const int n = e / FC, k = e - n * FC;
     bp[BP_W2T + k * FC + n] = w2[e];
   }
-  for (int e = t0; e < FC; e += stride) { bp[BP_B1 + e] = b1[e]; bp[BP_B2 + e] = b2[e]; }
-  for (int e = t0; e < 3 * W3_LD; e += stride) {
-    const int c = e / W3_LD, n = e - c * W3_LD;
-    bp[BP_W3 + e] = n < FC + 3 ? w3[c * (FC + 3) + n] : 0.0f;
-  }
-  for (int e = t0; e < 4; e += stride) bp[BP_B3 + e] = e < 3 ? b3[e] : 0.0f;
 }
 
 // ---- host-side launchers --------------------------------------------------------------------------
-size_t backward_prepared_bytes() { return BP_TC_OFFSET + (size_t)PREP_BYTES; }
+size_t backward_prepared_bytes() { return (size_t)BP_FLOATS * sizeof(float); }
 cudaError_t launch_prepare(const float* basis, const float* w1, const float* b1, const float* w2,
                            const float* b2, const float* w3, const float* b3, unsigned char* prep,
                            cudaStream_t stream);
@@ -796,10 +731,10 @@ size_t backward_shade_smem_bytes(bool tc) { return (size_t)(tc ? ShadeSmemT<true
 cudaError_t launch_prepare_backward(const float* basis, const float* w1, const float* b1,
                                     const float* w2, const float* b2, const float* w3,
                                     const float* b3, float* bp, cudaStream_t stream) {
-  prepare_backward_kernel<<<64, 256, 0, stream>>>(basis, w1, b1, w2, b2, w3, b3, bp);
+  prepare_backward_kernel<<<64, 256, 0, stream>>>(basis, w1, w2, bp);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return launch_prepare(basis, w1, b1, w2, b2, w3, b3, reinterpret_cast<unsigned char*>(bp) + BP_TC_OFFSET, stream);
+  return launch_prepare(basis, w1, b1, w2, b2, w3, b3, reinterpret_cast<unsigned char*>(bp), stream);
 }
 
 cudaError_t launch_render_backward(const FieldDev& F, BwdArgs A, void* scratch, int n_sms,

@@ -142,6 +142,26 @@ __device__ __forceinline__ void contract(float& x, float& y, float& z) {
   }
 }
 
+// d contract(p)/dp applied to dpc (ray_utils.py:9-12; amax routes the norm's gradient to the
+// component of largest magnitude)
+__device__ __forceinline__ void contract_bwd(float p0, float p1, float p2, float g0, float g1,
+                                             float g2, float& o0, float& o1, float& o2) {
+  float n = fmaxf(fmaxf(fabsf(p0), fabsf(p1)), fabsf(p2));
+  n = fmaxf(n, 1e-6f);
+  if (n <= 1.0f) { o0 = g0; o1 = g1; o2 = g2; return; }
+  const float s = __fdiv_rn(2.0f * n - 1.0f, n * n);
+  const float ds = -2.0f / (n * n) + 2.0f / (n * n * n);
+  const float dot = g0 * p0 + g1 * p1 + g2 * p2;
+  int j = 0;
+  float best = fabsf(p0);
+  if (fabsf(p1) > best) { j = 1; best = fabsf(p1); }
+  if (fabsf(p2) > best) { j = 2; }
+  o0 = s * g0; o1 = s * g1; o2 = s * g2;
+  const float pj = j == 0 ? p0 : (j == 1 ? p1 : p2);
+  const float extra = (pj >= 0.0f ? 1.0f : -1.0f) * ds * dot;
+  if (j == 0) o0 += extra; else if (j == 1) o1 += extra; else o2 += extra;
+}
+
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
 }
@@ -153,6 +173,15 @@ __device__ __forceinline__ float feature2density(float f, float shift, int act) 
     return x > 20.0f ? x : log1pf(expf(x));  // F.softplus(beta=1, threshold=20)
   }
   return fmaxf(f, 0.0f);
+}
+
+// dL/df from g = dL/d(feature2density(f))
+__device__ __forceinline__ float feature2density_grad(float f, float shift, int act, float g) {
+  if (act == 0) {
+    const float x = f + shift;
+    return g * (x > 20.0f ? 1.0f : __fdiv_rn(1.0f, 1.0f + expf(-x)));
+  }
+  return f > 0.0f ? g : 0.0f;
 }
 
 }  // namespace lrf

@@ -249,6 +249,14 @@ __device__ __forceinline__ void mlp_layers23(float (&acc)[64], const float* tail
 }
 
 // ---- ray setup (local_tensorfs.py:397-456 / tensorBase.py:578-580) ------------------------------
+// origin o, |d| and the normalised direction d / |d| (R.blend is the caller's)
+__device__ __forceinline__ void normalize_ray(const float* o, const float* d, RaySm& R) {
+  float n = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+  R.nrm = n;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) { R.o[a] = o[a]; R.vd[a] = __fdiv_rn(d[a], n); }
+}
+
 __device__ __forceinline__ void setup_ray(const BatchDev& B, long long r, RaySm& R) {
   float o[3], d[3];
   long long view = 0;
@@ -287,10 +295,7 @@ __device__ __forceinline__ void setup_ray(const BatchDev& B, long long r, RaySm&
       d[a] = c[a * 4 + 0] * dc[0] + c[a * 4 + 1] * dc[1] + c[a * 4 + 2] * dc[2];
     }
   }
-  float n = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-  R.nrm = n;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) { R.o[a] = o[a]; R.vd[a] = __fdiv_rn(d[a], n); }
+  normalize_ray(o, d, R);
   R.blend = B.blend ? B.blend[view * B.blend_stride] : 1.0f;
 }
 
@@ -416,6 +421,29 @@ __device__ __forceinline__ void app_plane_features_t(const FieldDev& F, int i, c
   for (int c = 0; c < CA; c += 8) vm_products<8>(t, texels<H16>(F.aplane[i]), texels<H16>(F.aline[i]), c, out + c);
 }
 
+// ---- one sample of the march (tensorBase.py:581-610) ---------------------------------------------
+// alpha of sample k < S of ray R; fe = its density feature and valid = whether it was looked up (not the
+// last sample, inside the alpha mask), fe = 0 where not
+template <bool H16>
+__device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R, int k, int S, float& fe,
+                                              bool& valid) {
+  const float z = __ldg(F.z + k);
+  float p[3], q[3];
+  sample_pos(F, R, z, p, q);
+  valid = (k != S - 1);                                       // ray_valid[:, -1] = 0
+  if (valid && F.alpha_vol) valid = alpha_mask(F, p) > 0.0f;  // tensorBase.py:593-598
+  float sigma = 0.0f;
+  fe = 0.0f;
+  if (valid) {
+    fe = density_feature_t<H16>(F, q);
+    sigma = feature2density(fe, F.density_shift, F.act);
+  }
+  const float dist = (k + 1 < S ? __ldg(F.z + k + 1) : z) - z;    // the last sample's dist is 0 (tensorBase.py:584-587)
+  float alpha = 1.0f - expf(-sigma * dist * F.distance_scale);   // tensorBase.py:610, same form
+  if (k == S - 1) alpha = 1.0f;                                  // alpha[:, -1] = 1
+  return alpha;
+}
+
 // ---- backward of the VM lookup (F.grid_sample align_corners=True, padding_mode="border") ----------------
 // pixel coordinate, its two taps and d(pixel)/d(normalised coordinate) (0 when clipped: ATen clip_coordinates_set_grad)
 __device__ __forceinline__ void grid_coord_grad(float c, int size, int& i0, int& i1, float& t,
@@ -505,6 +533,24 @@ __device__ __forceinline__ float warp_scan_mul(float v, int lane) {
   return v;
 }
 
-
+// transmittance of one 32-sample chunk of a ray, lane = sample (tensorBase.py:23-31): T = carry times the
+// product of (1 - alpha) + 1e-10 over the chunk's earlier samples, w = alpha T; then carry moves past the chunk.
+// Lanes past the ray's end (in = false) take part with a factor of 1.  use() runs once T and w are set, before
+// the carry's shuffle: the render producer accumulates and stores there (placed after the shuffle, that code
+// made ptxas spill 60-100 B more per thread in the render kernels).
+struct NoUse {
+  __device__ __forceinline__ void operator()() const {}
+};
+template <class Use = NoUse>
+__device__ __forceinline__ void transmittance_step(float alpha, bool in, int lane, float& carry, float& T,
+                                                   float& w, Use use = {}) {
+  const float inc = warp_scan_mul(in ? (1.0f - alpha) + 1e-10f : 1.0f, lane);
+  float exc = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane == 0) exc = 1.0f;
+  T = carry * exc;
+  w = alpha * T;
+  use();
+  carry *= __shfl_sync(0xffffffffu, inc, 31);
+}
 
 }  // namespace lrf

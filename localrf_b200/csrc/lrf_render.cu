@@ -291,25 +291,6 @@ __device__ __forceinline__ void queue_push(const ProdCtx& P, const FieldDev& F, 
   }
 }
 
-// alpha of sample k of the ray in slot-resident form (tensorBase.py:581-610); counts valid samples
-template <bool H16>
-__device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R, int k, int S, int& marched) {
-  const float z = __ldg(F.z + k);
-  float p[3], q[3];
-  sample_pos(F, R, z, p, q);
-  bool valid = (k != S - 1);                                  // ray_valid[:, -1] = 0
-  if (valid && F.alpha_vol) valid = alpha_mask(F, p) > 0.0f;  // tensorBase.py:593-598
-  float sigma = 0.0f;
-  if (valid) {
-    sigma = feature2density(density_feature_t<H16>(F, q), F.density_shift, F.act);
-    ++marched;
-  }
-  const float dist = (k + 1 < S ? __ldg(F.z + k + 1) : z) - z;    // the last sample's dist is 0 (tensorBase.py:584-587)
-  float alpha = 1.0f - expf(-sigma * dist * F.distance_scale);   // tensorBase.py:610, same form
-  if (k == S - 1) alpha = 1.0f;                                  // alpha[:, -1] = 1
-  return alpha;
-}
-
 // =================================================================================================
 // PE = the field has positional encodings (fea_pe > 0 or view_pe > 0): basis_mat is its own tensor-core
 // product (layer 0), the consumers build the encoded layer-1 input chunk by chunk in registers, layer 1's weight
@@ -437,21 +418,21 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
       float* wo = B.weights ? B.weights + (size_t)ray * S : nullptr;
       for (; k0 < S; k0 += 32) {
         const int k = k0 + lane;
-        float alpha = 0.0f;
-        if (k < S) alpha = sample_alpha<H16>(F, R, k, S, marched);
-        const float f = (k < S) ? (1.0f - alpha) + 1e-10f : 1.0f;
-        const float inc = warp_scan_mul(f, lane);
-        float exc = __shfl_up_sync(0xffffffffu, inc, 1);
-        if (lane == 0) exc = 1.0f;
-        const float wgt = alpha * (carry * exc);
+        float alpha = 0.0f, fe, T, wgt;
+        bool valid;
         if (k < S) {
-          acc_p += wgt;
-          dep_p += wgt * __ldg(F.z + k);
-          idx_p += wgt * (float)k;
-          if (floater) alpha_s[k] = alpha;
-          else if (wo) wo[k] = wgt;
+          alpha = sample_alpha<H16>(F, R, k, S, fe, valid);
+          if (valid) ++marched;
         }
-        carry *= __shfl_sync(0xffffffffu, inc, 31);
+        transmittance_step(alpha, k < S, lane, carry, T, wgt, [&] {
+          if (k < S) {
+            acc_p += wgt;
+            dep_p += wgt * __ldg(F.z + k);
+            idx_p += wgt * (float)k;
+            if (floater) alpha_s[k] = alpha;
+            else if (wo) wo[k] = wgt;
+          }
+        });
         if (!floater) {
           const bool on = (k < S) && (wgt > F.weight_thres);          // tensorBase.py:622
           const unsigned m = __ballot_sync(0xffffffffu, on);
@@ -472,12 +453,8 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
           float a = (k < S) ? alpha_s[k] : 0.0f;
           if ((float)k < lim) a = 0.0f;
           if (k == S - 1) a = 1.0f;
-          const float f = (k < S) ? (1.0f - a) + 1e-10f : 1.0f;
-          const float inc = warp_scan_mul(f, lane);
-          float exc = __shfl_up_sync(0xffffffffu, inc, 1);
-          if (lane == 0) exc = 1.0f;
-          const float wgt = a * (c2 * exc);
-          c2 *= __shfl_sync(0xffffffffu, inc, 31);
+          float T, wgt;
+          transmittance_step(a, k < S, lane, c2, T, wgt);
           if (k < S && wo) wo[k] = wgt;
           const bool on = (k < S) && (wgt > F.weight_thres);
           const unsigned m = __ballot_sync(0xffffffffu, on);

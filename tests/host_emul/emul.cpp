@@ -77,6 +77,42 @@ void emul_feature2density(const float* f, long long M, float shift, int act, flo
   for (long long m = 0; m < M; ++m) out[m] = feature2density(f[m], shift, act);
 }
 
+// contract_bwd: d contract(p)/dp applied to g, p and g [M][3]
+void emul_contract_bwd(const float* p, const float* g, long long M, float* out) {
+  for (long long m = 0; m < M; ++m) {
+    const float* a = p + 3 * m;
+    const float* b = g + 3 * m;
+    contract_bwd(a[0], a[1], a[2], b[0], b[1], b[2], out[3 * m], out[3 * m + 1], out[3 * m + 2]);
+  }
+}
+
+// sample_alpha over all S samples of n rays (origins o, directions d [n][3], normalised here) of a field with
+// an alpha mask (fp32 grids): alpha, fe [n][S] and valid [n][S]
+void emul_sample_alpha(const int* grid, const float* aabb, const void* const* dplane, const void* const* dline,
+                       const void* const* aplane, const void* const* aline, const float* vol, const int* dims,
+                       const float* alpha_aabb, float density_shift, float distance_scale, int act, const float* z,
+                       int S, const float* o, const float* d, long long n, float* alpha, float* fe,
+                       unsigned char* valid) {
+  FieldDev F = make_field(grid, aabb, dplane, dline, aplane, aline, 0);
+  F.alpha_vol = vol;
+  for (int a = 0; a < 3; ++a) {
+    F.ad[a] = dims[a];
+    F.aamin[a] = alpha_aabb[a];
+    F.aainv[a] = 1.0f / (alpha_aabb[3 + a] - alpha_aabb[a]) * 2.0f;
+  }
+  F.density_shift = density_shift; F.distance_scale = distance_scale; F.act = act;
+  F.z = z; F.S = S;
+  for (long long r = 0; r < n; ++r) {
+    RaySm R;
+    normalize_ray(o + 3 * r, d + 3 * r, R);
+    for (int k = 0; k < S; ++k) {
+      bool v;
+      alpha[r * S + k] = sample_alpha<false>(F, R, k, S, fe[r * S + k], v);
+      valid[r * S + k] = v ? 1 : 0;
+    }
+  }
+}
+
 // ray generation of LocalTensorfs.forward (ids2pixel, get_ray_directions_*, cam2rf, get_rays_lean, normalisation):
 // out_o / out_vd [n][3], out_nrm [n], dirs [n][3] (camera space), ij [n][2]
 void emul_setup_rays(const long long* ray_ids, long long n, long long n_views, int W, int H, int fov360, float focal,

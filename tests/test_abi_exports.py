@@ -57,12 +57,11 @@ def test_validation_errors_without_gpu():
     assert rc == -1
 
 
-def test_backward_sizes_and_validation_without_gpu():
+def test_backward_sizes_with_embedded_forward_block_and_validation_without_gpu():
     L = _lib.lib()
-    # (W1 @ basis)^T [72][128], W2^T [128][128], b1, b2, W3 [3][132], b3 [4] in fp32, then (1 KiB aligned)
-    # the forward's bf16 operand block, which the tensor-core shade step reads (W1B, W2 and, MN-major, their transposes)
-    fp32_part = 4 * (72 * 128 + 128 * 128 + 128 + 128 + 3 * 132 + 4)
-    assert L.lrf_prepared_backward_bytes() == (fp32_part + 1023) // 1024 * 1024 + L.lrf_prepared_bytes()
+    # the forward's prepared block (bf16 operand images of W1B and W2, fp32 b1, b2, W3, b3), then
+    # (W1 @ basis)^T [72][128] and W2^T [128][128] in fp32
+    assert L.lrf_prepared_backward_bytes() == L.lrf_prepared_bytes() + 4 * (72 * 128 + 128 * 128)
     n, S = 4096, 344
     need = L.lrf_backward_scratch_bytes(n, S)
     # 5 fp32 tables + 2 int32 lists + 1 byte per sample, the per-ray accumulators and the counter

@@ -158,6 +158,66 @@ def test_feature2density(emul):
     assert np.array_equal(out, np.maximum(x, 0))
 
 
+def test_contract_backward_vs_autograd(emul):
+    """contract_bwd against torch autograd through ray_utils.contract, inside and outside the unit cube."""
+    from localrf_b200.ray_utils import contract
+    p = np.concatenate([points(3000, 7, span=3.0), points(1000, 8, span=1.0)])
+    gout = np.random.default_rng(9).standard_normal(p.shape).astype(np.float32)
+    out = np.empty_like(p)
+    emul.emul_contract_bwd(_vp(p.ctypes.data), _vp(gout.ctypes.data), C.c_longlong(len(p)), _vp(out.ctypes.data))
+    x = torch.from_numpy(p).double().requires_grad_(True)
+    contract(x).backward(torch.from_numpy(gout).double())
+    ref = x.grad.numpy()
+    inside = np.abs(p).max(-1) <= 1
+    assert 0.2 < inside.mean() < 0.5
+    np.testing.assert_array_equal(out[inside], gout[inside])
+    np.testing.assert_allclose(out, ref, rtol=1e-5, atol=1e-5 * np.abs(ref).max())
+
+
+def test_sample_alpha_vs_oracle(emul):
+    """sample_alpha (sample position, alpha-mask validity, density feature, feature2density and alpha with the
+    alpha[:, -1] = 1 rule) for every sample of the golden rays of a field with an alpha mask, against values built
+    from the oracle's contract, alpha_mask_sample and density_feature."""
+    gd = load_golden("alphamask_32")
+    fd = full_field_dict(gd)
+    f = orc.Field(fd)
+    G = Grids(fd)
+    vol = np.ascontiguousarray(np.asarray(fd["alphaMask.alpha_volume"], np.float32).reshape(fd["alphaMask.alpha_volume"].shape[-3:]))
+    dims = (C.c_int * 3)(*vol.shape)
+    ab = np.asarray(fd["alphaMask.aabb"], np.float32).reshape(6).copy()
+    z = np.ascontiguousarray(gd["eval.z"], np.float32)
+    S = len(z)
+    rays = np.asarray(gd["rays"], np.float32)
+    o, d = np.ascontiguousarray(rays[:, :3]), np.ascontiguousarray(rays[:, 3:])
+    n = len(rays)
+    shift, scale = float(fd["density_shift"]), float(fd["distance_scale"])
+    act = {"softplus": 0, "relu": 1}[fd["fea2denseAct"]]
+    alpha, fe, valid = np.empty((n, S), np.float32), np.empty((n, S), np.float32), np.empty((n, S), np.uint8)
+    emul.emul_sample_alpha(G.grid, _vp(G.aabb.ctypes.data), G.ptrs["dplane"], G.ptrs["dline"], G.ptrs["aplane"],
+                           G.ptrs["aline"], _vp(vol.ctypes.data), dims, _vp(ab.ctypes.data), C.c_float(shift),
+                           C.c_float(scale), act, _vp(z.ctypes.data), S, _vp(o.ctypes.data), _vp(d.ctypes.data),
+                           C.c_longlong(n), _vp(alpha.ctypes.data), _vp(fe.ctypes.data), _vp(valid.ctypes.data))
+
+    vd = d / np.sqrt((d * d).sum(-1, dtype=np.float32))[:, None]
+    p = orc.contract((o[:, None] + vd[:, None] * z[None, :, None]).reshape(-1, 3))
+    q = (p - G.aabb[:3]) * (np.float32(2) / (G.aabb[3:] - G.aabb[:3])) - np.float32(1)
+    ok = (orc.alpha_mask_sample(f, p) > 0).reshape(n, S)
+    ok[:, -1] = False                                                       # ray_valid[:, -1] = 0
+    fe_ref = np.where(ok, orc.density_feature(f, q).reshape(n, S), np.float32(0))
+    fe_t = torch.from_numpy(fe_ref)
+    sigma = torch.nn.functional.softplus(fe_t + shift) if act == 0 else fe_t.clamp(min=0)
+    sigma = np.where(ok, sigma.numpy(), np.float32(0))
+    dist = np.append(np.diff(z), np.float32(0))
+    alpha_ref = 1 - np.exp(-sigma * dist * scale)
+    alpha_ref[:, -1] = 1                                                    # alpha[:, -1] = 1
+
+    assert ok.any() and (~ok[:, :-1]).any()                                 # the mask excludes some samples
+    np.testing.assert_array_equal(valid.astype(bool), ok)
+    assert np.abs(fe - fe_ref).max() <= 2e-6 * max(np.abs(fe_ref).max(), 1e-3)
+    assert np.abs(alpha - alpha_ref).max() <= 5e-6
+    assert alpha[:, :-1].max() > 0.1
+
+
 @pytest.mark.parametrize("fov360", [0, 1])
 def test_ray_generation_vs_oracle(emul, fov360):
     """setup_ray (ids2pixel, get_ray_directions_lean / _360, per-view cam2rf, get_rays_lean, normalisation)."""
