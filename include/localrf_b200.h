@@ -283,6 +283,23 @@ int lrf_frame_to_u8(const float *rgb, int32_t rgb_stride, const float *depth, in
                     float d_lo, float d_hi, const unsigned char *lut, unsigned char *rgb8, unsigned char *depth8,
                     lrf_stream_t stream);
 
+/* Test-frame metrics on the device.  replaces: renderer.py:162-163, `mse = ((gt_rgb - rgb_map) ** 2).mean()` and
+ * `rgb_ssim(gt_rgb, rgb_map, 1)` with rgb_ssim of utils/utils.py:232-287 (numpy + scipy.signal.convolve2d).
+ * img and gt are H x W x 3 fp32 frames, pixel (row, col) channel c at ptr[(row * W + col) * stride + c] (stride 3
+ * for [N][3], 4 for the interleaved pix layout).  Inputs and `out` may be device or pinned host memory.
+ * out[0] = mean of (gt - img)^2 over all H * W * 3 values (fp32 terms summed in fp64); out[1] = SSIM: a "valid"
+ * separable Gaussian filter (filter_size taps, filter_sigma) of the five moments, the squares and the cross
+ * product formed in fp32 as the reference's float32 arrays do, everything else in fp64, and the mean of the map.
+ * ssim_map, when non-NULL, receives the fp64 map [H - filter_size + 1][W - filter_size + 1][3].
+ * scratch: at least lrf_image_metrics_scratch_bytes(H, W, filter_size) bytes of device memory, 8-byte aligned.
+ * Bitwise deterministic, no host synchronisation.  filter_size outside [1, 16] is LRF_ERR_UNSUPPORTED.
+ * Difference from the reference: H or W below filter_size is LRF_ERR_INVALID (the reference averages an empty
+ * map and returns NaN). */
+size_t lrf_image_metrics_scratch_bytes(int32_t H, int32_t W, int32_t filter_size); /* 0 if invalid */
+int lrf_image_metrics(const float *img, int32_t img_stride, const float *gt, int32_t gt_stride, int32_t H, int32_t W,
+                      double max_val, int32_t filter_size, double filter_sigma, double k1, double k2, double *out,
+                      double *ssim_map, void *scratch, size_t scratch_bytes, lrf_stream_t stream);
+
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */
 int lrf_pack_bf16(const float *src, void *dst, int64_t n, lrf_stream_t stream);

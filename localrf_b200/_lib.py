@@ -10,7 +10,8 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
-SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_abi.cu"]
+SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
+           "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -82,7 +83,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_launch_info", "lrf_prepared_backward_bytes", "lrf_backward_scratch_bytes",
            "lrf_field_prepare_backward", "lrf_render_backward", "lrf_peer_barrier", "lrf_peer_signal_wait",
            "lrf_alpha_mask_build", "lrf_upsample", "lrf_density_l1", "lrf_density_l1_backward", "lrf_tv_sums",
-           "lrf_tv_sums_backward", "lrf_sample_ray", "lrf_frame_to_u8", "lrf_pack_bf16"]
+           "lrf_tv_sums_backward", "lrf_sample_ray", "lrf_frame_to_u8", "lrf_pack_bf16",
+           "lrf_image_metrics_scratch_bytes", "lrf_image_metrics"]
 
 
 def _stale():
@@ -170,6 +172,10 @@ def lib():
     L.lrf_sample_ray.argtypes = [_vp, _vp, C.c_int64, C.c_int32, C.c_float * 6, C.c_float, C.c_float, C.c_float,
                                  _vp, _vp, _vp, _vp]
     L.lrf_frame_to_u8.argtypes = [_vp, C.c_int32, _vp, C.c_int32, C.c_int64, C.c_float, C.c_float, _vp, _vp, _vp, _vp]
+    L.lrf_image_metrics_scratch_bytes.restype = C.c_size_t
+    L.lrf_image_metrics_scratch_bytes.argtypes = [C.c_int32] * 3
+    L.lrf_image_metrics.argtypes = [_vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32,
+                                    C.c_double, C.c_double, C.c_double, _vp, _vp, _vp, C.c_size_t, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

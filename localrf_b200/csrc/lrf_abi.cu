@@ -46,6 +46,10 @@ cudaError_t launch_peer_barrier(unsigned long long* const* peer_flags, int rank,
 cudaError_t launch_frame_u8(const float* rgb, int rgb_stride, const float* depth, int depth_stride, long long N,
                             float d_lo, float d_hi, const unsigned char* lut, unsigned char* rgb8,
                             unsigned char* depth8, int n_sms, cudaStream_t stream);
+size_t metrics_scratch_bytes(int H, int W);
+cudaError_t launch_image_metrics(const float* img, int img_stride, const float* gt, int gt_stride, int H, int W,
+                                 int fs, double sigma, double c1, double c2, double* out, double* ssim_map,
+                                 void* scratch, cudaStream_t stream);
 cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
                                 cudaStream_t stream);
 cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
@@ -572,6 +576,32 @@ int lrf_frame_to_u8(const float* rgb, int32_t rgb_stride, const float* depth, in
   cudaError_t e = lrf::launch_frame_u8(rgb, rgb_stride, depth, depth_stride, N, d_lo, d_hi, lut, rgb8, depth8,
                                        d.n_sms, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e, "frame_u8_kernel");
+  return LRF_OK;
+}
+
+size_t lrf_image_metrics_scratch_bytes(int32_t H, int32_t W, int32_t filter_size) {
+  if (filter_size < 1 || filter_size > 16 || H < filter_size || W < filter_size) return 0;
+  return lrf::metrics_scratch_bytes(H, W);
+}
+
+int lrf_image_metrics(const float* img, int32_t img_stride, const float* gt, int32_t gt_stride, int32_t H, int32_t W,
+                      double max_val, int32_t filter_size, double filter_sigma, double k1, double k2, double* out,
+                      double* ssim_map, void* scratch, size_t scratch_bytes, lrf_stream_t stream) {
+  if (!img) return fail(LRF_ERR_INVALID, "img is NULL");
+  if (!gt) return fail(LRF_ERR_INVALID, "gt is NULL");
+  if (!out) return fail(LRF_ERR_INVALID, "out is NULL");
+  if (img_stride < 3) return fail(LRF_ERR_INVALID, "img_stride must be >= 3");
+  if (gt_stride < 3) return fail(LRF_ERR_INVALID, "gt_stride must be >= 3");
+  if (filter_size < 1 || filter_size > 16) return fail(LRF_ERR_UNSUPPORTED, "filter_size must be in [1, 16]");
+  if (H < filter_size || W < filter_size)
+    return fail(LRF_ERR_INVALID, "H and W must be >= filter_size (the reference's SSIM map would be empty)");
+  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
+  if (scratch_bytes < lrf::metrics_scratch_bytes(H, W))
+    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_image_metrics_scratch_bytes(H, W, filter_size)");
+  const double c1 = (k1 * max_val) * (k1 * max_val), c2 = (k2 * max_val) * (k2 * max_val);
+  cudaError_t e = lrf::launch_image_metrics(img, img_stride, gt, gt_stride, H, W, filter_size, filter_sigma, c1, c2,
+                                            out, ssim_map, scratch, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "metrics_tile_kernel");
   return LRF_OK;
 }
 

@@ -8,14 +8,16 @@ them with numpy / cv2 / matplotlib and only then starts the next frame.  Here a 
 
 whose outputs are written by the GPU straight into pinned host buffers (zero-copy, 6 bytes per pixel instead
 of 16), with a CUDA event per frame.  `submit()` never blocks; `fetch()` returns the OLDEST finished frame,
-so encoding / writing frame i on the host overlaps the rendering of frames i+1..i+depth-1.
+so encoding / writing frame i on the host overlaps the rendering of frames i+1..i+depth-1.  A frame submitted
+with its ground truth (`gt=`) is also scored on the device (MSE and SSIM, renderer.py:162-163; metrics.py) into a
+pinned double[2] of its slot.
 """
 import ctypes as C
 
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, metrics
 from .tensorf import _ptr, _stream
 
 
@@ -41,7 +43,8 @@ class FramePipeline:
         for _ in range(int(n_buffers)):
             s = {"rgb8": torch.empty(self.n, 3, dtype=torch.uint8).pin_memory(),
                  "depth8": torch.empty(self.n, 3, dtype=torch.uint8).pin_memory(),
-                 "event": torch.cuda.Event(), "busy": False, "tag": None}
+                 "metrics": torch.zeros(2, dtype=torch.float64).pin_memory(),
+                 "event": torch.cuda.Event(), "busy": False, "tag": None, "has_gt": False}
             if keep_float:
                 s["rgb"] = torch.empty(self.n, 3).pin_memory()
                 s["depth"] = torch.empty(self.n).pin_memory()
@@ -51,13 +54,26 @@ class FramePipeline:
     def in_flight(self):
         return sum(s["busy"] for s in self.slots)
 
+    def _stage_gt(self, s, gt):
+        """gt as a frame the metrics kernel can read: CUDA and pinned tensors as they are, anything else copied
+        into the slot's pinned staging buffer (free: the slot's previous frame has been fetched)."""
+        if isinstance(gt, torch.Tensor) and (gt.is_cuda or gt.is_pinned()):
+            return gt
+        if "gt" not in s:
+            s["gt"] = torch.empty(self.n, 3).pin_memory()
+        s["gt"].copy_(torch.as_tensor(gt, dtype=torch.float32).reshape(self.n, 3))
+        return s["gt"]
+
     @torch.no_grad()
-    def submit(self, view_ids, tag=None, **forward_kw):
+    def submit(self, view_ids, gt=None, tag=None, **forward_kw):
         """Enqueues one frame (all W*H rays of `view_ids`; kwargs as LocalTensorfs.forward: cam2world,
-        world2rf, blending_weights, test_id, floater_thresh ...).  Raises if every buffer is in flight."""
+        world2rf, blending_weights, test_id, floater_thresh ...).  With `gt` ([H,W,3] float32: a CUDA tensor, a
+        pinned tensor, or anything torch.as_tensor takes), the frame's MSE and SSIM against it are computed on
+        the device as well (metrics.image_metrics).  Raises if every buffer is in flight."""
         s = self.slots[self.head]
         if s["busy"]:
             raise RuntimeError("all frame buffers are in flight: fetch() before submitting more")
+        g = None if gt is None else self._stage_gt(s, gt)
         out = (s["rgb"], s["depth"]) if self.keep_float else None
         rgb, depth, _, _ = self.lt(self.ids, view_ids, self.W, self.H, is_train=False, out=out, **forward_kw)
         with torch.cuda.device(self.dev):
@@ -65,15 +81,18 @@ class FramePipeline:
             _lib.check(_lib.lib().lrf_frame_to_u8(_ptr(rgb), 3, _ptr(depth), 1, self.n, self.minmax[0],
                                                   self.minmax[1], _ptr(self.lut), _ptr(s["rgb8"]),
                                                   _ptr(s["depth8"]), st))
+            if g is not None:
+                metrics._enqueue(rgb, g, s["metrics"], W=self.W)
             s["event"].record(torch.cuda.current_stream(self.dev))
-        s["busy"], s["tag"] = True, tag
-        s["hold"] = (rgb, depth)                        # keep device outputs alive until the event has passed
+        s["busy"], s["tag"], s["has_gt"] = True, tag, g is not None
+        s["hold"] = (rgb, depth, g)                     # keep device outputs alive until the event has passed
         self.head = (self.head + 1) % len(self.slots)
 
     def fetch(self):
         """Blocks until the oldest submitted frame is complete -> dict(tag, rgb8 [H,W,3] uint8 BGR,
-        depth8 [H,W,3] uint8 BGR, and rgb [H,W,3] / depth [H,W] float32 when keep_float).  The arrays are
-        views of the pinned buffer: valid until `len(buffers)` more frames have been submitted."""
+        depth8 [H,W,3] uint8 BGR, rgb [H,W,3] / depth [H,W] float32 when keep_float, and mse / ssim floats
+        when the frame was submitted with gt).  The arrays are views of the pinned buffer: valid until
+        `len(buffers)` more frames have been submitted."""
         s = self.slots[self.tail]
         if not s["busy"]:
             return None
@@ -86,6 +105,8 @@ class FramePipeline:
         if self.keep_float:
             out["rgb"] = s["rgb"].numpy().reshape(self.H, self.W, 3)
             out["depth"] = s["depth"].numpy().reshape(self.H, self.W)
+        if s["has_gt"]:
+            out["mse"], out["ssim"] = (float(v) for v in s["metrics"].numpy())
         return out
 
     def render(self, frames, **forward_kw):
