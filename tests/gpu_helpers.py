@@ -47,18 +47,20 @@ def local_from_golden(g, device="cuda"):
     return lt.to(device)
 
 
+def oracle_field(rf):
+    """One (product) TensorVMSplit as an oracle Field (reference layout, numpy; its alpha mask included)."""
+    from oracle import oracle as orc
+    fd = {k: v.detach().cpu().numpy() for k, v in rf.state_dict().items()}
+    kw = rf.get_kwargs()
+    for k in ("density_shift", "distance_scale", "rayMarch_weight_thres", "fea_pe", "view_pe",
+              "featureC", "app_dim", "step_ratio", "fea2denseAct", "gridSize"):
+        fd[k] = kw[k]
+    return orc.Field(fd)
+
+
 def oracle_fields(lt):
     """Every field of a (product) LocalTensorfs as an oracle Field (reference layout, numpy)."""
-    from oracle import oracle as orc
-    out = []
-    for rf in lt.tensorfs:
-        fd = {k: v.detach().cpu().numpy() for k, v in rf.state_dict().items()}
-        kw = rf.get_kwargs()
-        for k in ("density_shift", "distance_scale", "rayMarch_weight_thres", "fea_pe", "view_pe",
-                  "featureC", "app_dim", "step_ratio", "fea2denseAct", "gridSize"):
-            fd[k] = kw[k]
-        out.append(orc.Field(fd))
-    return out
+    return [oracle_field(rf) for rf in lt.tensorfs]
 
 
 def oracle_local(lt, fields, ids, view, W, H, world2rf=None, blend=None, floater_thresh=0.0):

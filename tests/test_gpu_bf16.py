@@ -15,7 +15,7 @@ import torch
 
 import localrf_b200 as L
 from localrf_b200 import _lib
-from gpu_helpers import module_from_golden, oracle_fields
+from gpu_helpers import module_from_golden, oracle_field
 from helpers import check_with_ties, load_golden, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -95,7 +95,7 @@ def test_render_bf16_storage_equals_fp32_storage_and_oracle(golden, floater):
           f"(bit-equal rgb: {torch.equal(rgb16, rgb32)}, weights: {torch.equal(w16, w32)})")
     assert e_w < 1e-5 and n2 == 0
     # ... and against the CPU oracle (pinned to the reference) evaluated on the same rounded parameters
-    f = oracle_fields(type("S", (), {"tensorfs": [m]})())[0]
+    f = oracle_field(m)
     ref = orc.field_forward(f, rays.cpu().numpy(), orc.sample_table(f.n_samples()), floater_thresh=floater)
     margin_o = np.abs(ref["weights"] - float(m.rayMarch_weight_thres)).min(-1)
     n3, e3 = check_with_ties(rgb16.cpu().numpy(), ref["rgb"], margin_o, TOL, f"{golden} rgb bf16 vs oracle", max_tie_frac=0.02)
