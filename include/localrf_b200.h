@@ -153,7 +153,7 @@ typedef struct LrfOutputs {
 int lrf_version(void);
 const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
- * 3 LrfGradients (0 for any other index).  Bindings compare these with their own mirrors at load
+ * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads (0 for any other index).  Bindings compare these with their own mirrors at load
  * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
@@ -299,6 +299,66 @@ size_t lrf_image_metrics_scratch_bytes(int32_t H, int32_t W, int32_t filter_size
 int lrf_image_metrics(const float *img, int32_t img_stride, const float *gt, int32_t gt_stride, int32_t H, int32_t W,
                       double max_val, int32_t filter_size, double filter_sigma, double k1, double k2, double *out,
                       double *ssim_map, void *scratch, size_t scratch_bytes, lrf_stream_t stream);
+
+/* Supervision losses of one training step on the device.  replaces: train.py:369-423 -- the loss-weighted L1
+ * rgb term, the optical-flow reprojection term (get_fwd_bwd_cam2cams / get_pred_flow / pts2px, utils/utils.py:
+ * 15-48) cut per view above its 0.9 quantile, and the monocular-depth term (compute_depth_loss, utils/utils.py:
+ * 50-59) cut per view above its 0.8 quantile.  The batch is view-major: rays v*R .. v*R+R-1 belong to view v
+ * (R = n_rays / n_views).  Device pointers, fp32 unless stated. */
+typedef struct LrfLossBatch {
+  int64_t n_rays;              /* N = n_views * R, R <= 4096 */
+  int64_t n_views;             /* V */
+  int64_t n_cams;              /* rows of cam2world (>= 1) */
+  int64_t starting_id;         /* absolute frame id of cam2world[0]; view v uses camera view_ids[v] - starting_id */
+  int32_t use_flow, use_depth; /* which regularisers are on (the rgb term always is) */
+  float flow_weight;           /* L_flow = mean(cut e) * flow_weight (the caller folds train.py's factors) */
+  float depth_weight;          /* L_depth = mean(cut d) * depth_weight */
+  const float *rgb_map;        /* [N][3] */
+  const float *rgb_train;      /* [N][3] */
+  const float *loss_weights;   /* [N] */
+  const int64_t *view_ids;     /* [V] absolute frame ids (flow) */
+  const float *depth_map;      /* [N] (flow, depth) */
+  const float *directions;     /* [N][3] camera-space ray directions (flow) */
+  const int64_t *ij;           /* [N][2] pixel (column, row) (flow) */
+  const float *cam2world;      /* [n_cams][3][4] (flow) */
+  const float *focal;          /* [1] (flow) */
+  const float *center;         /* [2] cx, cy (flow) */
+  const float *fwd_flow, *bwd_flow;  /* [N][2] (flow) */
+  const float *fwd_mask, *bwd_mask;  /* [N] (flow) */
+  const float *invdepths;      /* [N] (depth) */
+} LrfLossBatch;
+
+/* Gradients of lrf_supervision_losses_backward; each may be NULL (not wanted).  All are OVERWRITTEN, also when a
+ * term is off (d_directions, d_cam2world, d_focal and d_center are then zero without the flow term). */
+typedef struct LrfLossGrads {
+  float *d_rgb;                /* [N][3] */
+  float *d_depth;              /* [N] */
+  float *d_directions;         /* [N][3] */
+  float *d_cam2world;          /* [n_cams][3][4]: the per-view cam2cam gradients chained in view order */
+  float *d_focal;              /* [1] */
+  float *d_center;             /* [2] */
+} LrfLossGrads;
+
+/* Device scratch bytes of one forward + its backward (8-byte aligned).  0 if the sizes are invalid. */
+size_t lrf_supervision_scratch_bytes(int64_t n_rays, int64_t n_views, int64_t n_cams);
+/* losses[3] = {L_rgb, L_flow, L_depth} (a term that is off gives 0).  Per view: e = the flow residual of each ray
+ * (backward flow first, then forward; the forward mask is zero for every ray of a view whose ABSOLUTE id equals
+ * n_cams - 1, as in the reference), x = 1 / max(depth, 1e-6) and g = invdepths normalised by their lower medians
+ * and mean absolute deviations, d = (xn - gn)^2; each of e and d is zeroed above its torch.quantile (linear, bit
+ * for bit).  A view whose camera id view_ids[v] - starting_id lies outside [0, n_cams) gets NaN flow residuals
+ * (the id cannot be checked on the host without a synchronisation).  A MAD of 0 gives NaN/inf, as in the
+ * reference.  The scratch keeps the forward's decisions for the backward; its leading part is, in bytes:
+ * e [N] fp32 at 0, d [N] fp32 at 4N (both before the cut), tau [2][V] fp32 at 8N (flow, then depth thresholds),
+ * median ray indices [V][2] int32 at 8N + 8V (x, then g).  Entries of a term that is off are not written.
+ * No atomics, no host synchronisation: bitwise repeatable.  R > 4096 is LRF_ERR_UNSUPPORTED. */
+int lrf_supervision_losses(const LrfLossBatch *batch, float *losses, void *scratch, size_t scratch_bytes,
+                           lrf_stream_t stream);
+/* Backward of the same batch, after lrf_supervision_losses on the same scratch: grad_losses [3] (device) are the
+ * upstream gradients of the three losses.  Cut entries and the thresholds carry no gradient; each median passes
+ * its gradient to the ray the forward selected.  A view with an out-of-range camera id gives NaN gradients
+ * through its flow term and adds nothing to d_cam2world. */
+int lrf_supervision_losses_backward(const LrfLossBatch *batch, const float *grad_losses, const LrfLossGrads *grads,
+                                    void *scratch, size_t scratch_bytes, lrf_stream_t stream);
 
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */

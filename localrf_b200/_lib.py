@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
-           "lrf_abi.cu"]
+           "lrf_losses.cu", "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -42,6 +42,22 @@ class LrfField(C.Structure):
 
 
 GRID_F32, GRID_BF16 = 0, 1
+
+
+class LrfLossBatch(C.Structure):
+    _fields_ = [
+        ("n_rays", C.c_int64), ("n_views", C.c_int64), ("n_cams", C.c_int64), ("starting_id", C.c_int64),
+        ("use_flow", C.c_int32), ("use_depth", C.c_int32),
+        ("flow_weight", C.c_float), ("depth_weight", C.c_float),
+        ("rgb_map", _vp), ("rgb_train", _vp), ("loss_weights", _vp), ("view_ids", _vp), ("depth_map", _vp),
+        ("directions", _vp), ("ij", _vp), ("cam2world", _vp), ("focal", _vp), ("center", _vp),
+        ("fwd_flow", _vp), ("bwd_flow", _vp), ("fwd_mask", _vp), ("bwd_mask", _vp), ("invdepths", _vp),
+    ]
+
+
+class LrfLossGrads(C.Structure):
+    _fields_ = [("d_rgb", _vp), ("d_depth", _vp), ("d_directions", _vp), ("d_cam2world", _vp), ("d_focal", _vp),
+                ("d_center", _vp)]
 
 
 class LrfBatch(C.Structure):
@@ -84,7 +100,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_field_prepare_backward", "lrf_render_backward", "lrf_peer_barrier", "lrf_peer_signal_wait",
            "lrf_alpha_mask_build", "lrf_upsample", "lrf_density_l1", "lrf_density_l1_backward", "lrf_tv_sums",
            "lrf_tv_sums_backward", "lrf_sample_ray", "lrf_frame_to_u8", "lrf_pack_bf16",
-           "lrf_image_metrics_scratch_bytes", "lrf_image_metrics"]
+           "lrf_image_metrics_scratch_bytes", "lrf_image_metrics", "lrf_supervision_scratch_bytes",
+           "lrf_supervision_losses", "lrf_supervision_losses_backward"]
 
 
 def _stale():
@@ -137,7 +154,7 @@ def lib():
                            "rebuild it (python -c 'import localrf_b200; localrf_b200.build(force=True)')")
     L.lrf_sizeof.restype = C.c_size_t
     L.lrf_sizeof.argtypes = [C.c_int32]
-    for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients)):
+    for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads)):
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -176,6 +193,11 @@ def lib():
     L.lrf_image_metrics_scratch_bytes.argtypes = [C.c_int32] * 3
     L.lrf_image_metrics.argtypes = [_vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32,
                                     C.c_double, C.c_double, C.c_double, _vp, _vp, _vp, C.c_size_t, _vp]
+    L.lrf_supervision_scratch_bytes.restype = C.c_size_t
+    L.lrf_supervision_scratch_bytes.argtypes = [C.c_int64] * 3
+    L.lrf_supervision_losses.argtypes = [C.POINTER(LrfLossBatch), _vp, _vp, C.c_size_t, _vp]
+    L.lrf_supervision_losses_backward.argtypes = [C.POINTER(LrfLossBatch), _vp, C.POINTER(LrfLossGrads), _vp,
+                                                  C.c_size_t, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

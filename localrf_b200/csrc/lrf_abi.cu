@@ -50,6 +50,10 @@ size_t metrics_scratch_bytes(int H, int W);
 cudaError_t launch_image_metrics(const float* img, int img_stride, const float* gt, int gt_stride, int H, int W,
                                  int fs, double sigma, double c1, double c2, double* out, double* ssim_map,
                                  void* scratch, cudaStream_t stream);
+size_t losses_scratch_bytes(long long N, long long V);
+cudaError_t launch_supervision_losses(const LrfLossBatch& b, float* losses, void* scratch, cudaStream_t stream);
+cudaError_t launch_supervision_losses_backward(const LrfLossBatch& b, const float* grad_losses, const LrfLossGrads& g,
+                                               void* scratch, cudaStream_t stream);
 cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
                                 cudaStream_t stream);
 cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
@@ -196,6 +200,8 @@ size_t lrf_sizeof(int32_t which) {
     case 1: return sizeof(LrfBatch);
     case 2: return sizeof(LrfOutputs);
     case 3: return sizeof(LrfGradients);
+    case 4: return sizeof(LrfLossBatch);
+    case 5: return sizeof(LrfLossGrads);
     default: return 0;
   }
 }
@@ -602,6 +608,50 @@ int lrf_image_metrics(const float* img, int32_t img_stride, const float* gt, int
   cudaError_t e = lrf::launch_image_metrics(img, img_stride, gt, gt_stride, H, W, filter_size, filter_sigma, c1, c2,
                                             out, ssim_map, scratch, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e, "metrics_tile_kernel");
+  return LRF_OK;
+}
+
+static int check_loss_batch(const LrfLossBatch* b, const void* scratch, size_t scratch_bytes) {
+  if (!b) return fail(LRF_ERR_INVALID, "batch is NULL");
+  if (b->n_rays < 1 || b->n_views < 1 || b->n_rays % b->n_views != 0)
+    return fail(LRF_ERR_INVALID, "n_rays must be a positive multiple of n_views");
+  if (b->n_cams < 1) return fail(LRF_ERR_INVALID, "n_cams must be >= 1");
+  if (!b->rgb_map || !b->rgb_train || !b->loss_weights)
+    return fail(LRF_ERR_INVALID, "rgb_map / rgb_train / loss_weights is NULL");
+  if (b->use_flow && (!b->view_ids || !b->depth_map || !b->directions || !b->ij || !b->cam2world || !b->focal ||
+                      !b->center || !b->fwd_flow || !b->bwd_flow || !b->fwd_mask || !b->bwd_mask))
+    return fail(LRF_ERR_INVALID, "a pointer of the flow term is NULL");
+  if (b->use_depth && (!b->depth_map || !b->invdepths))
+    return fail(LRF_ERR_INVALID, "a pointer of the depth term is NULL");
+  if (b->n_rays / b->n_views > 4096) return fail(LRF_ERR_UNSUPPORTED, "more than 4096 rays per view");
+  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
+  if (scratch_bytes < lrf::losses_scratch_bytes(b->n_rays, b->n_views))
+    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_supervision_scratch_bytes(n_rays, n_views, n_cams)");
+  return LRF_OK;
+}
+
+size_t lrf_supervision_scratch_bytes(int64_t n_rays, int64_t n_views, int64_t n_cams) {
+  if (n_rays < 1 || n_views < 1 || n_rays % n_views != 0 || n_cams < 1) return 0;
+  return lrf::losses_scratch_bytes(n_rays, n_views);
+}
+
+int lrf_supervision_losses(const LrfLossBatch* b, float* losses, void* scratch, size_t scratch_bytes,
+                           lrf_stream_t stream) {
+  const int rc = check_loss_batch(b, scratch, scratch_bytes);
+  if (rc != LRF_OK) return rc;
+  if (!losses) return fail(LRF_ERR_INVALID, "losses is NULL");
+  cudaError_t e = lrf::launch_supervision_losses(*b, losses, scratch, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "supervision_losses");
+  return LRF_OK;
+}
+
+int lrf_supervision_losses_backward(const LrfLossBatch* b, const float* grad_losses, const LrfLossGrads* g,
+                                    void* scratch, size_t scratch_bytes, lrf_stream_t stream) {
+  const int rc = check_loss_batch(b, scratch, scratch_bytes);
+  if (rc != LRF_OK) return rc;
+  if (!grad_losses || !g) return fail(LRF_ERR_INVALID, "grad_losses / grads is NULL");
+  cudaError_t e = lrf::launch_supervision_losses_backward(*b, grad_losses, *g, scratch, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "supervision_losses_backward");
   return LRF_OK;
 }
 
