@@ -153,7 +153,7 @@ typedef struct LrfOutputs {
 int lrf_version(void);
 const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
- * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads (0 for any other index).  Bindings compare these with their own mirrors at load
+ * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor (0 for any other index).  Bindings compare these with their own mirrors at load
  * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
@@ -359,6 +359,33 @@ int lrf_supervision_losses(const LrfLossBatch *batch, float *losses, void *scrat
  * through its flow term and adds nothing to d_cam2world. */
 int lrf_supervision_losses_backward(const LrfLossBatch *batch, const float *grad_losses, const LrfLossGrads *grads,
                                     void *scratch, size_t scratch_bytes, lrf_stream_t stream);
+
+/* One Adam step over many fp32 tensors in one launch.  replaces: torch.optim.Adam.step with its default options
+ * (torch 2.11's _multi_tensor_adam, non-capturable) for every optimiser of a training step, local_tensorfs.py:
+ * 245,272-284.  The caller increments the step counters and folds the per-tensor scalars in double precision, as
+ * torch does, rounding each to float where ATen's opmath cast does.  Per element, in fp32 with one rounding each:
+ *   exp_avg = lerp(exp_avg, grad, one_minus_beta1); exp_avg_sq = exp_avg_sq * beta2;
+ *   exp_avg_sq = fma(one_minus_beta2, grad * grad, exp_avg_sq); d = sqrt(exp_avg_sq) / bc2_sqrt + eps;
+ *   param = fma(step_size, exp_avg / d, param).
+ * The four arrays of one entry have numel elements each and one dense layout; entries must not overlap (a parameter
+ * listed twice is updated once, from the values before the launch).  16-byte aligned entries use vector accesses. */
+typedef struct LrfAdamTensor {
+  float *param;
+  const float *grad;
+  float *exp_avg;
+  float *exp_avg_sq;
+  int64_t numel;               /* 0 = skipped */
+  float one_minus_beta1;       /* float(1 - beta1) */
+  float beta2;                 /* float(beta2) */
+  float one_minus_beta2;       /* float(1 - beta2) */
+  float eps;                   /* float(eps) */
+  float step_size;             /* float((lr / (1 - beta1 ** step)) * -1) */
+  float bc2_sqrt;              /* float((1 - beta2 ** step) ** 0.5) */
+} LrfAdamTensor;
+
+/* t: HOST array of n entries, read before the call returns.  One launch per 448 tensors; no atomics, no host
+ * synchronisation, bitwise repeatable.  n == 0 does nothing. */
+int lrf_adam_step(const LrfAdamTensor *t, int64_t n, lrf_stream_t stream);
 
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */

@@ -54,6 +54,7 @@ size_t losses_scratch_bytes(long long N, long long V);
 cudaError_t launch_supervision_losses(const LrfLossBatch& b, float* losses, void* scratch, cudaStream_t stream);
 cudaError_t launch_supervision_losses_backward(const LrfLossBatch& b, const float* grad_losses, const LrfLossGrads& g,
                                                void* scratch, cudaStream_t stream);
+cudaError_t launch_adam_step(const LrfAdamTensor* t, long long n, cudaStream_t stream);
 cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
                                 cudaStream_t stream);
 cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
@@ -202,6 +203,7 @@ size_t lrf_sizeof(int32_t which) {
     case 3: return sizeof(LrfGradients);
     case 4: return sizeof(LrfLossBatch);
     case 5: return sizeof(LrfLossGrads);
+    case 6: return sizeof(LrfAdamTensor);
     default: return 0;
   }
 }
@@ -652,6 +654,18 @@ int lrf_supervision_losses_backward(const LrfLossBatch* b, const float* grad_los
   if (!grad_losses || !g) return fail(LRF_ERR_INVALID, "grad_losses / grads is NULL");
   cudaError_t e = lrf::launch_supervision_losses_backward(*b, grad_losses, *g, scratch, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e, "supervision_losses_backward");
+  return LRF_OK;
+}
+
+int lrf_adam_step(const LrfAdamTensor* t, int64_t n, lrf_stream_t stream) {
+  if (n < 0 || (n > 0 && !t)) return fail(LRF_ERR_INVALID, "bad tensor table / n");
+  for (int64_t i = 0; i < n; ++i) {                 // every entry is checked before anything is launched
+    if (t[i].numel < 0) return fail(LRF_ERR_INVALID, "a tensor has numel < 0");
+    if (t[i].numel > 0 && (!t[i].param || !t[i].grad || !t[i].exp_avg || !t[i].exp_avg_sq))
+      return fail(LRF_ERR_INVALID, "param / grad / exp_avg / exp_avg_sq of a tensor with elements is NULL");
+  }
+  cudaError_t e = lrf::launch_adam_step(t, n, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "adam_kernel");
   return LRF_OK;
 }
 

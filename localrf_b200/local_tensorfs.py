@@ -20,6 +20,7 @@ import re
 import torch
 
 from . import _lib
+from .optim import adam_step, zero_grad
 from .tensorf import AlphaGridMask, TensorVMSplit, _ptr, _require_cuda, _stream
 from .utils import N_to_reso, mtx_to_sixD, sixD_to_mtx
 
@@ -197,13 +198,10 @@ class LocalTensorfs(torch.nn.Module):
 
     def optimizer_step_poses_only(self, loss):
         live = self._live_pose_ids()
-        for i in live:
-            self.r_optimizers[i].zero_grad()
-            self.t_optimizers[i].zero_grad()
+        stepped = [o for i in live for o in (self.r_optimizers[i], self.t_optimizers[i])]
+        zero_grad(stepped)
         loss.backward()
-        for i in live:
-            self.r_optimizers[i].step()
-            self.t_optimizers[i].step()
+        adam_step(stepped)
 
     def optimizer_step(self, loss, optimize_poses):
         """One optimisation step + the schedule events it triggers (:193-290)."""
@@ -225,27 +223,28 @@ class LocalTensorfs(torch.nn.Module):
             for group in opt.param_groups:
                 group["lr"] *= self.lr_factor
 
-        live = self._live_pose_ids()
-        for i in live:
+        stepped = [self.rf_optimizer]                       # every optimiser this step updates
+        for i in self._live_pose_ids():
             if optimize_poses:
                 decay(self.r_optimizers[i]); decay(self.t_optimizers[i])
-                self.r_optimizers[i].zero_grad(); self.t_optimizers[i].zero_grad()
+                stepped += [self.r_optimizers[i], self.t_optimizers[i]]
             if self.lr_exposure_init > 0:
                 decay(self.exp_optimizers[i])
-                self.exp_optimizers[i].zero_grad()
-        tune_intrinsics = (self.lr_i_init > 0 and self.blending_weights.shape[1] == 1
-                           and self.is_refining)
-        if tune_intrinsics:
+                stepped.append(self.exp_optimizers[i])
+        if self.lr_i_init > 0 and self.blending_weights.shape[1] == 1 and self.is_refining:
             decay(self.intrinsic_optimizer)
-            self.intrinsic_optimizer.zero_grad()
-        self.rf_optimizer.zero_grad()
+            stepped.append(self.intrinsic_optimizer)
+        zero_grad(stepped)
 
         loss.backward()
         if getattr(self, "dp_group", None) is not None:     # data-parallel training: average the step's
             from .dist import allreduce_gradients            # gradients over the ranks before any update
             allreduce_gradients(self, None if self.dp_group is True else self.dp_group)
 
-        self.rf_optimizer.step()
+        # One launch updates the field, the live frames' poses and exposures and the intrinsics.  The reference
+        # steps the pose, exposure and intrinsics optimisers after the upsample / alpha-mask events below; doing
+        # it here gives the same result, because those events read only the field's tensors.
+        adam_step(stepped)
         if self.is_refining:
             decay(self.rf_optimizer)
 
@@ -259,13 +258,6 @@ class LocalTensorfs(torch.nn.Module):
         if self.rf_iter[-1] in self.update_AlphaMask_list:  # rebuild the occupancy mask
             self.tensorfs[-1].updateAlphaMask(tuple((self.tensorfs[-1].gridSize / 2).int()))
 
-        for i in live:
-            if optimize_poses:
-                self.r_optimizers[i].step(); self.t_optimizers[i].step()
-            if self.lr_exposure_init > 0:
-                self.exp_optimizers[i].step()
-        if tune_intrinsics:
-            self.intrinsic_optimizer.step()
         if self.is_refining:
             self.rf_iter[-1] += 1
         return self.rf_iter[-1] >= self.n_iters - 1       # can_add_rf
