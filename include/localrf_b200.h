@@ -153,7 +153,7 @@ typedef struct LrfOutputs {
 int lrf_version(void);
 const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
- * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor (0 for any other index).  Bindings compare these with their own mirrors at load
+ * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor, 7 LrfCameraGrads (0 for any other index).  Bindings compare these with their own mirrors at load
  * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
@@ -225,6 +225,54 @@ int lrf_render_backward(const LrfField *field, const void *prepared_bwd, const f
                         int64_t n_rays, int32_t white_bg, const float *grad_rgb,
                         const float *grad_depth, const LrfGradients *grads, void *scratch,
                         size_t scratch_bytes, lrf_stream_t stream);
+
+/* ---- the training call of LocalTensorfs.forward with camera gradients ------------------------------------
+ * replaces: local_tensorfs.py:397-499 with is_train, one field, under autograd -- ids2pixel,
+ * get_ray_directions_lean / _360, cam2rf, get_rays_lean, the render, exposure (bmm) and clamp -- forward and
+ * backward.  Forward: lrf_render in ray-generation mode with finalize = 0 and exposure = NULL writes rgb_linear,
+ * then lrf_exposure_clamp writes rgb = clamp(E_v rgb_linear, 0, 1) with the render kernel's own finalize
+ * arithmetic (bitwise the rgb of a finalize = 1 launch).  exposure [n_views][3][3] may be NULL (identity); ray r
+ * uses view r / (n_rays / n_views). */
+int lrf_exposure_clamp(const float *rgb_linear, const float *exposure, int64_t n_rays, int64_t n_views, float *rgb,
+                       lrf_stream_t stream);
+
+/* Camera-side gradients of lrf_render_backward_batch.  Each may be NULL (not wanted); each is OVERWRITTEN. */
+typedef struct LrfCameraGrads {
+  float *d_cam2world;         /* [n_views][3][4] */
+  float *d_intrinsics;        /* [3] focal, cx, cy (zero for fov360: its directions do not use them) */
+  float *d_exposure;          /* [n_views][3][3]: sum over the view's rays of g' x^T (also when batch->exposure
+                                 is NULL: the gradient at the identity) */
+  float *d_world2rf;          /* [3] */
+} LrfCameraGrads;
+
+/* Scratch bytes of lrf_render_backward_batch; 0 if n_rays < 1, n_samples < 2, n_views < 1 or n_rays % n_views.
+ * The block holds, in this order and each part starting 16-byte aligned: the generated rays [n_rays][6] fp32
+ * (o, d: exactly what lrf_render marched) at byte 0, the camera-space directions [n_rays][3], g_lin [n_rays][3],
+ * g' [n_rays][3], d_rays [n_rays][6] (used when grads->d_rays is NULL), per-view fp64 partials, one slot
+ * [n_rays][n_samples][3] per sample for the colour branch's position gradient, and the block of lrf_render_backward. */
+size_t lrf_backward_batch_scratch_bytes(int64_t n_rays, int32_t n_samples, int64_t n_views);
+
+/* Backward of the training call above.  `batch` is the forward's LrfBatch in ray-generation mode (rays, blend
+ * and accumulate unset; its white_bg is the one the forward used); rgb_linear [n][3] the forward's pre-exposure
+ * colour; grad_rgb [n][3] = dL/d(rgb) of the CLAMPED output, grad_depth [n], grad_directions [n][3] or NULL
+ * (dL/d of the camera-space directions, e.g. from the flow loss).  Three stages:
+ *   1. per ray: the generated rays go to scratch; g' = grad_rgb [0 <= E x <= 1] (both ends pass the gradient,
+ *      as torch's clamp backward does); g_lin = E_v^T g';
+ *   2. lrf_render_backward on the scratch rays with g_lin: the field gradients are ACCUMULATED into `grads` as
+ *      there (atomic adds), d_rays (may be NULL here) overwritten -- summed in a fixed order (each sample's colour
+ *      term in its own scratch slot), unlike lrf_render_backward's d_rays;
+ *   3. per view: d_cam2world = [d_rays_d dir^T | d_rays_o], d_exposure = sum g' x^T, d_world2rf = sum d_rays_o,
+ *      and with d_dir = R_v^T d_rays_d + grad_directions: d focal = sum -d_dir . dir / focal,
+ *      d cx = sum -d_dir_x / focal, d cy = sum d_dir_y / focal.
+ * No float atomics in d_rays or in stages 1 and 3, and a fixed summation order (fp64): the camera gradients
+ * are bitwise repeatable.  LRF_ERR_INVALID before any device work for explicit rays, accumulate, a blend pointer,
+ * n_rays % n_views != 0, a NULL field-gradient pointer or too little scratch; floater_thresh > 0 and fields
+ * with positional encodings are LRF_ERR_UNSUPPORTED. */
+int lrf_render_backward_batch(const LrfField *field, const void *prepared_bwd, const LrfBatch *batch,
+                              const float *rgb_linear, const float *grad_rgb, const float *grad_depth,
+                              const float *grad_directions, const LrfGradients *grads,
+                              const LrfCameraGrads *cam_grads, void *scratch, size_t scratch_bytes,
+                              lrf_stream_t stream);
 
 /* Closes a fused pixel exchange: enqueues on `stream` a one-CTA kernel that (1) makes this GPU's
  * earlier peer stores visible system-wide, (2) writes `seq` into slot `rank` of every peer's flag

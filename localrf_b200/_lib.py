@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
-           "lrf_losses.cu", "lrf_optim.cu", "lrf_abi.cu"]
+           "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -99,6 +99,10 @@ class LrfGradients(C.Structure):
                 ("d_w3", _vp), ("d_b3", _vp)]
 
 
+class LrfCameraGrads(C.Structure):
+    _fields_ = [("d_cam2world", _vp), ("d_intrinsics", _vp), ("d_exposure", _vp), ("d_world2rf", _vp)]
+
+
 EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", "lrf_prepared_bytes_for", "lrf_field_prepare",
            "lrf_render", "lrf_mlp_forward", "lrf_app_products", "lrf_density_feature_backward",
            "lrf_app_products_backward", "lrf_density_feature", "lrf_app_feature", "lrf_repack_nchw_to_nhwc",
@@ -107,7 +111,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_alpha_mask_build", "lrf_upsample", "lrf_density_l1", "lrf_density_l1_backward", "lrf_tv_sums",
            "lrf_tv_sums_backward", "lrf_sample_ray", "lrf_frame_to_u8", "lrf_pack_bf16",
            "lrf_image_metrics_scratch_bytes", "lrf_image_metrics", "lrf_supervision_scratch_bytes",
-           "lrf_supervision_losses", "lrf_supervision_losses_backward", "lrf_adam_step"]
+           "lrf_supervision_losses", "lrf_supervision_losses_backward", "lrf_adam_step",
+           "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch"]
 
 
 def _stale():
@@ -161,7 +166,7 @@ def lib():
     L.lrf_sizeof.restype = C.c_size_t
     L.lrf_sizeof.argtypes = [C.c_int32]
     for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
-                                     LrfAdamTensor)):
+                                     LrfAdamTensor, LrfCameraGrads)):
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -187,6 +192,11 @@ def lib():
     L.lrf_field_prepare_backward.argtypes = [C.POINTER(LrfField), _vp, _vp]
     L.lrf_render_backward.argtypes = [C.POINTER(LrfField), _vp, _vp, C.c_int64, C.c_int32, _vp, _vp,
                                       C.POINTER(LrfGradients), _vp, C.c_size_t, _vp]
+    L.lrf_exposure_clamp.argtypes = [_vp, _vp, C.c_int64, C.c_int64, _vp, _vp]
+    L.lrf_backward_batch_scratch_bytes.restype = C.c_size_t
+    L.lrf_backward_batch_scratch_bytes.argtypes = [C.c_int64, C.c_int32, C.c_int64]
+    L.lrf_render_backward_batch.argtypes = [C.POINTER(LrfField), _vp, C.POINTER(LrfBatch), _vp, _vp, _vp, _vp,
+                                            C.POINTER(LrfGradients), C.POINTER(LrfCameraGrads), _vp, C.c_size_t, _vp]
     L.lrf_alpha_mask_build.argtypes = [C.POINTER(LrfField), C.c_int32 * 3, C.c_float, C.c_float, _vp, _vp, _vp, _vp]
     L.lrf_upsample.argtypes = [_vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp]
     L.lrf_density_l1.argtypes = [C.POINTER(LrfField), _vp, _vp]

@@ -71,7 +71,14 @@ cudaError_t launch_prepare_backward(const float* basis, const float* w1, const f
 cudaError_t launch_render_backward_abi(const FieldDev& F, const float* rays, long long n_rays,
                                        int white_bg, const float* g_rgb, const float* g_depth,
                                        const float* bp, const LrfGradients& G, void* scratch,
-                                       int n_sms, cudaStream_t stream);
+                                       int n_sms, cudaStream_t stream, float* dpos = nullptr);
+size_t train_backward_scratch_bytes(long long n, int S, long long V);
+cudaError_t launch_exposure_clamp(const float* x, const float* E, long long n, long long V, float* rgb, int n_sms,
+                                  cudaStream_t stream);
+cudaError_t launch_render_backward_batch(const FieldDev& F, const BatchDev& B, const float* bp, const float* x,
+                                         const float* g_rgb, const float* g_depth, const float* g_dirs,
+                                         const LrfGradients& G, const LrfCameraGrads& CG, void* scratch,
+                                         long long n_views, int n_sms, cudaStream_t stream);
 }  // namespace lrf
 
 namespace {
@@ -204,6 +211,7 @@ size_t lrf_sizeof(int32_t which) {
     case 4: return sizeof(LrfLossBatch);
     case 5: return sizeof(LrfLossGrads);
     case 6: return sizeof(LrfAdamTensor);
+    case 7: return sizeof(LrfCameraGrads);
     default: return 0;
   }
 }
@@ -478,6 +486,77 @@ int lrf_render_backward(const LrfField* f, const void* prepared_bwd, const float
                                                   static_cast<const float*>(prepared_bwd), *g, scratch,
                                                   d.n_sms, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e, "render_backward");
+  return LRF_OK;
+}
+
+int lrf_exposure_clamp(const float* x, const float* exposure, int64_t n_rays, int64_t n_views, float* rgb,
+                       lrf_stream_t stream) {
+  if (n_rays < 0 || n_views < 1 || n_rays % n_views != 0)
+    return fail(LRF_ERR_INVALID, "n_rays must be a multiple of n_views >= 1");
+  if (n_rays > 0 && (!x || !rgb)) return fail(LRF_ERR_INVALID, "rgb_linear / rgb is NULL");
+  DevInfo d;
+  int rc = device_info(d);
+  if (rc != LRF_OK) return rc;
+  cudaError_t e = lrf::launch_exposure_clamp(x, exposure, n_rays, n_views, rgb, d.n_sms, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "exposure_clamp_kernel");
+  return LRF_OK;
+}
+
+size_t lrf_backward_batch_scratch_bytes(int64_t n_rays, int32_t n_samples, int64_t n_views) {
+  if (n_rays < 1 || n_samples < 2 || n_views < 1 || n_rays % n_views != 0) return 0;
+  return lrf::train_backward_scratch_bytes(n_rays, n_samples, n_views);
+}
+
+int lrf_render_backward_batch(const LrfField* f, const void* prepared_bwd, const LrfBatch* b, const float* x,
+                              const float* grad_rgb, const float* grad_depth, const float* grad_directions,
+                              const LrfGradients* g, const LrfCameraGrads* cg, void* scratch, size_t scratch_bytes,
+                              lrf_stream_t stream) {
+  if (!prepared_bwd) return fail(LRF_ERR_INVALID, "prepared_bwd is NULL (call lrf_field_prepare_backward first)");
+  lrf::FieldDev F;
+  int rc = make_field(f, true, true, nullptr, F);
+  if (rc != LRF_OK) return rc;
+  if (!b || !g || !cg) return fail(LRF_ERR_INVALID, "batch / grads / cam_grads is NULL");
+  if (b->rays) return fail(LRF_ERR_INVALID, "the batch backward generates its rays: batch->rays must be NULL");
+  if (b->accumulate) return fail(LRF_ERR_INVALID, "accumulate is not supported by the batch backward");
+  if (b->blend) return fail(LRF_ERR_INVALID, "a blend pointer is not supported by the batch backward");
+  if (b->n_rays < 1 || b->n_views < 1 || b->n_rays % b->n_views != 0)
+    return fail(LRF_ERR_INVALID, "n_rays must be a positive multiple of n_views");
+  if (b->n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  if (!b->ray_ids || !b->cam2world) return fail(LRF_ERR_INVALID, "ray_ids/cam2world is NULL");
+  if (b->W < 1 || b->H < 1) return fail(LRF_ERR_INVALID, "W/H must be positive");
+  if (!b->fov360 && !b->intrinsics && !(b->focal != 0.0f)) return fail(LRF_ERR_INVALID, "focal must be non-zero");
+  if (!x || !grad_rgb || !grad_depth) return fail(LRF_ERR_INVALID, "rgb_linear / grad_rgb / grad_depth is NULL");
+  if (!g->d_w1b || !g->d_b1 || !g->d_w2 || !g->d_b2 || !g->d_w3 || !g->d_b3)
+    return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
+  for (int i = 0; i < 3; ++i) {
+    if (!g->d_dplane[i] || !g->d_dline[i] || !g->d_aplane[i] || !g->d_aline[i])
+      return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
+    if (((uintptr_t)g->d_dplane[i] | (uintptr_t)g->d_dline[i] | (uintptr_t)g->d_aplane[i] |
+         (uintptr_t)g->d_aline[i]) & 15)
+      return fail(LRF_ERR_INVALID, "plane/line gradient buffers must be 16-byte aligned");
+  }
+  if (!scratch || ((uintptr_t)scratch & 15)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 16-byte aligned");
+  if (scratch_bytes < lrf::train_backward_scratch_bytes(b->n_rays, F.S, b->n_views))
+    return fail(LRF_ERR_INVALID, "scratch is smaller than lrf_backward_batch_scratch_bytes(n_rays, n_samples, n_views)");
+  if (b->floater_thresh > 0.0f) return fail(LRF_ERR_UNSUPPORTED, "the backward is built for floater_thresh = 0");
+  lrf::BatchDev B;
+  memset(&B, 0, sizeof(B));
+  B.n_rays = b->n_rays;
+  B.rays_per_view = b->n_rays / b->n_views;
+  B.ray_ids = reinterpret_cast<const long long*>(b->ray_ids);
+  B.W = b->W; B.H = b->H; B.fov360 = b->fov360;
+  B.focal = b->focal; B.cx = b->cx; B.cy = b->cy;
+  B.intrinsics = b->intrinsics;
+  B.c2w = b->cam2world;
+  B.w2rf = b->world2rf;
+  B.exposure = b->exposure;
+  B.white_bg = b->white_bg;
+  DevInfo d;
+  if ((rc = device_info(d)) != LRF_OK) return rc;
+  cudaError_t e = lrf::launch_render_backward_batch(F, B, static_cast<const float*>(prepared_bwd), x, grad_rgb,
+                                                    grad_depth, grad_directions, *g, *cg, scratch, b->n_views,
+                                                    d.n_sms, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "render_backward_batch");
   return LRF_OK;
 }
 

@@ -39,6 +39,8 @@ constexpr int BP_FLOATS = BP_W2T + FC * FC;
 struct BwdScratch {           // views into the caller's scratch block
   unsigned long long* count;  // number of shaded samples (zeroed per call)
   float* d_ovd;               // [n][6] position-gradient accumulators (zeroed per call)
+  float* dpos;                // NULL, or [n][S][3] zeroed by the caller: each shaded sample's colour-branch position
+                              // gradient in its own slot instead of d_ovd's atomics (a fixed summation order)
   float *alpha, *T, *w, *fe, *gw;   // [n][S]
   unsigned char* valid;       // [n][S]
   int *app_ray, *app_k;       // [n*S]
@@ -594,10 +596,15 @@ bwd_shade_kernel(const FieldDev F, const BwdArgs A) {
         float dp0, dp1, dp2;
         contract_bwd(praw_s[ls * 3], praw_s[ls * 3 + 1], praw_s[ls * 3 + 2], dq0 * F.ainv[0],
                      dq1 * F.ainv[1], dq2 * F.ainv[2], dp0, dp1, dp2);
-        float* acc = A.s.d_ovd + 6 * (size_t)ray_s[ls];
-        const float z = zk_s[ls];
-        atomicAdd(acc + 0, dp0); atomicAdd(acc + 1, dp1); atomicAdd(acc + 2, dp2);
-        atomicAdd(acc + 3, dp0 * z); atomicAdd(acc + 4, dp1 * z); atomicAdd(acc + 5, dp2 * z);
+        if (A.s.dpos) {          // one slot per (ray, sample): the density kernel sums them in a fixed order
+          float* dst = A.s.dpos + 3 * ((size_t)ray_s[ls] * S + kk_s[ls]);
+          dst[0] = dp0; dst[1] = dp1; dst[2] = dp2;
+        } else {
+          float* acc = A.s.d_ovd + 6 * (size_t)ray_s[ls];
+          const float z = zk_s[ls];
+          atomicAdd(acc + 0, dp0); atomicAdd(acc + 1, dp1); atomicAdd(acc + 2, dp2);
+          atomicAdd(acc + 3, dp0 * z); atomicAdd(acc + 4, dp1 * z); atomicAdd(acc + 5, dp2 * z);
+        }
       }
     }
     __syncthreads();
@@ -663,6 +670,11 @@ bwd_density_kernel(const FieldDev F, const BwdArgs A) {
       }
       const float excl = inc - term + suffix_carry;                      // sum_{j > k} gw_j w_j
       suffix_carry += __shfl_sync(0xffffffffu, inc, 0);
+      if (in && A.s.dpos) {                                              // colour-branch part (zero if not shaded)
+        const float* dp = A.s.dpos + 3 * (base + k);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) { d_o[a] += dp[a]; d_vd[a] += dp[a] * zk; }
+      }
       if (k < S - 1 && A.s.valid[base + k]) {                            // last / masked samples: constants
         const float al = A.s.alpha[base + k];
         const float dalpha = gwk * A.s.T[base + k] - __fdiv_rn(excl, (1.0f - al) + 1e-10f);
@@ -688,7 +700,7 @@ bwd_density_kernel(const FieldDev F, const BwdArgs A) {
     for (int a = 0; a < 3; ++a) { d_o[a] = warp_sum(d_o[a]); d_vd[a] = warp_sum(d_vd[a]); }
     const float depth = __fdiv_rn(warp_sum(dep_p), R.nrm);
     if (lane == 0) {
-      const float* acc = A.s.d_ovd + 6 * (size_t)ray;                    // colour-branch part
+      const float* acc = A.s.d_ovd + 6 * (size_t)ray;                    // colour-branch part (zero with dpos)
 #pragma unroll
       for (int a = 0; a < 3; ++a) { d_o[a] += acc[a]; d_vd[a] += acc[3 + a]; }
       const float dotv = R.vd[0] * d_vd[0] + R.vd[1] * d_vd[1] + R.vd[2] * d_vd[2];
@@ -737,10 +749,11 @@ cudaError_t launch_prepare_backward(const float* basis, const float* w1, const f
   return launch_prepare(basis, w1, b1, w2, b2, w3, b3, reinterpret_cast<unsigned char*>(bp), stream);
 }
 
-cudaError_t launch_render_backward(const FieldDev& F, BwdArgs A, void* scratch, int n_sms,
+cudaError_t launch_render_backward(const FieldDev& F, BwdArgs A, void* scratch, float* dpos, int n_sms,
                                    cudaStream_t stream) {
   size_t zero_bytes = 0;
   bwd_scratch_layout(A.n_rays, F.S, &A.s, static_cast<unsigned char*>(scratch), &zero_bytes);
+  A.s.dpos = dpos;
   cudaError_t e = cudaMemsetAsync(scratch, 0, zero_bytes, stream);
   if (e != cudaSuccess) return e;
   // tensor-core shade step by default; LRF_BWD_TC=0 selects the CUDA-core kernel (the independent fp32
@@ -777,7 +790,7 @@ cudaError_t launch_render_backward(const FieldDev& F, BwdArgs A, void* scratch, 
 cudaError_t launch_render_backward_abi(const FieldDev& F, const float* rays, long long n_rays,
                                        int white_bg, const float* g_rgb, const float* g_depth,
                                        const float* bp, const LrfGradients& G, void* scratch,
-                                       int n_sms, cudaStream_t stream) {
+                                       int n_sms, cudaStream_t stream, float* dpos) {
   BwdArgs A;
   A.n_rays = n_rays; A.rays = rays; A.g_rgb = g_rgb; A.g_depth = g_depth; A.bp = bp;
   A.white_bg = white_bg; A.d_rays = G.d_rays;
@@ -786,7 +799,7 @@ cudaError_t launch_render_backward_abi(const FieldDev& F, const float* rays, lon
     A.d_aplane[i] = G.d_aplane[i]; A.d_aline[i] = G.d_aline[i];
   }
   A.d_w1b = G.d_w1b; A.d_b1 = G.d_b1; A.d_w2 = G.d_w2; A.d_b2 = G.d_b2; A.d_w3 = G.d_w3; A.d_b3 = G.d_b3;
-  return launch_render_backward(F, A, scratch, n_sms, stream);
+  return launch_render_backward(F, A, scratch, dpos, n_sms, stream);
 }
 
 }  // namespace lrf

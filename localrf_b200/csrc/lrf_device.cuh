@@ -7,6 +7,17 @@
 
 #include "lrf_common.cuh"
 
+#ifndef __CUDACC__
+// host build of this header (tests/host_emul): the rounding intrinsics the ray setup and exposure spell out,
+// with the same IEEE single-rounding semantics
+#include <cmath>
+static inline float __fadd_rn(float a, float b) { return a + b; }
+static inline float __fsub_rn(float a, float b) { return a - b; }
+static inline float __fmul_rn(float a, float b) { return a * b; }
+static inline float __fmaf_rn(float a, float b, float c) { return std::fma(a, b, c); }
+static inline float __ll2float_rn(long long a) { return (float)a; }
+#endif
+
 namespace lrf {
 
 constexpr int TM = 128;      // appearance samples per MLP tile (two wgmma M = 64 halves)
@@ -257,6 +268,42 @@ __device__ __forceinline__ void normalize_ray(const float* o, const float* d, Ra
   for (int a = 0; a < 3; ++a) { R.o[a] = o[a]; R.vd[a] = __fdiv_rn(d[a], n); }
 }
 
+// Ray generation of ray r of view `view` (local_tensorfs.py:397-456): id -> pixel (col, row) -> camera-space
+// direction dc -> world (field) space o = t + world2rf, d = R dc.  Every rounding is an explicit _rn intrinsic, so
+// each kernel that calls this (the render kernel, the backward's ray prologue) gets the same bits: the backward
+// marches these rays again and must reproduce the forward's alphas and weights exactly.
+// dirs [3] and ij [2] (each may be NULL) receive dc and (col, row).
+__device__ __forceinline__ void generate_ray(const BatchDev& B, long long r, long long view, float* o, float* d,
+                                             float* dirs, long long* ij) {
+  const long long id = B.ray_ids[r];
+  const long long col = id % B.W, row = (id / B.W) % B.H;         // ids2pixel
+  float dc[3];
+  const float i = __fadd_rn(__ll2float_rn(col), 0.5f), j = __fadd_rn(__ll2float_rn(row), 0.5f);
+  if (B.fov360) {                                                 // get_ray_directions_360
+    const float pi = 3.14159265358979323846f;
+    const float phi = __fsub_rn(__fdiv_rn(__fmul_rn(j, pi), (float)B.H), pi / 2.0f);
+    const float theta = __fadd_rn(__fdiv_rn(__fmul_rn(__fadd_rn(i, i), pi), (float)B.W), pi);
+    float sp, cp, st, ct;
+    sincosf(phi, &sp, &cp);
+    sincosf(theta, &st, &ct);
+    dc[0] = __fmul_rn(cp, st); dc[1] = sp; dc[2] = __fmul_rn(cp, ct);
+  } else {                                                        // get_ray_directions_lean
+    float focal = B.focal, cx = B.cx, cy = B.cy;
+    if (B.intrinsics) { focal = B.intrinsics[0]; cx = B.intrinsics[1]; cy = B.intrinsics[2]; }
+    dc[0] = __fdiv_rn(__fsub_rn(i, cx), focal);
+    dc[1] = -__fdiv_rn(__fsub_rn(j, cy), focal);
+    dc[2] = -1.0f;
+  }
+  if (dirs) { dirs[0] = dc[0]; dirs[1] = dc[1]; dirs[2] = dc[2]; }
+  if (ij) { ij[0] = col; ij[1] = row; }
+  const float* c = B.c2w + 12 * view;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {                                   // get_rays_lean
+    o[a] = __fadd_rn(c[a * 4 + 3], B.w2rf ? B.w2rf[a] : 0.0f);
+    d[a] = __fmaf_rn(c[a * 4 + 2], dc[2], __fmaf_rn(c[a * 4 + 0], dc[0], __fmul_rn(c[a * 4 + 1], dc[1])));
+  }
+}
+
 __device__ __forceinline__ void setup_ray(const BatchDev& B, long long r, RaySm& R) {
   float o[3], d[3];
   long long view = 0;
@@ -267,36 +314,27 @@ __device__ __forceinline__ void setup_ray(const BatchDev& B, long long r, RaySm&
     if (B.rays_per_view > 0) view = r / B.rays_per_view;
   } else {
     view = r / B.rays_per_view;
-    long long id = B.ray_ids[r];
-    long long col = id % B.W, row = (id / B.W) % B.H;            // ids2pixel
-    float i = (float)col + 0.5f, j = (float)row + 0.5f;
-    float dc[3];
-    if (B.fov360) {                                               // get_ray_directions_360
-      const float pi = 3.14159265358979323846f;
-      float phi = j * pi / (float)B.H - pi / 2.0f;
-      float theta = i * 2.0f * pi / (float)B.W + pi;
-      float sp, cp, st, ct;
-      sincosf(phi, &sp, &cp);
-      sincosf(theta, &st, &ct);
-      dc[0] = cp * st; dc[1] = sp; dc[2] = cp * ct;
-    } else {                                                      // get_ray_directions_lean
-      float focal = B.focal, cx = B.cx, cy = B.cy;
-      if (B.intrinsics) { focal = B.intrinsics[0]; cx = B.intrinsics[1]; cy = B.intrinsics[2]; }
-      dc[0] = __fdiv_rn(i - cx, focal);
-      dc[1] = -__fdiv_rn(j - cy, focal);
-      dc[2] = -1.0f;
-    }
-    if (B.dirs) { B.dirs[3 * r] = dc[0]; B.dirs[3 * r + 1] = dc[1]; B.dirs[3 * r + 2] = dc[2]; }
-    if (B.ij) { B.ij[2 * r] = col; B.ij[2 * r + 1] = row; }
-    const float* c = B.c2w + 12 * view;
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {                                 // get_rays_lean
-      o[a] = c[a * 4 + 3] + (B.w2rf ? B.w2rf[a] : 0.0f);
-      d[a] = c[a * 4 + 0] * dc[0] + c[a * 4 + 1] * dc[1] + c[a * 4 + 2] * dc[2];
-    }
+    generate_ray(B, r, view, o, d, B.dirs ? B.dirs + 3 * r : nullptr, B.ij ? B.ij + 2 * r : nullptr);
   }
   normalize_ray(o, d, R);
   R.blend = B.blend ? B.blend[view * B.blend_stride] : 1.0f;
+}
+
+// ---- exposure + clamp of a finished pixel (local_tensorfs.py:481-497) ------------------------------
+// c = E c for one view's 3x3 exposure E (row-major); E == NULL leaves c unchanged
+__device__ __forceinline__ void expose_rgb(const float* E, float (&c)[3]) {
+  if (!E) return;
+  float o[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+    o[a] = __fmaf_rn(E[3 * a + 2], c[2], __fmaf_rn(E[3 * a + 0], c[0], __fmul_rn(E[3 * a + 1], c[1])));
+  c[0] = o[0]; c[1] = o[1]; c[2] = o[2];
+}
+// rgb = clamp(E c, 0, 1): the render kernel's finalize and lrf_exposure_clamp
+__device__ __forceinline__ void finalize_rgb(const float* E, float (&c)[3]) {
+  expose_rgb(E, c);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) c[a] = fminf(1.0f, fmaxf(0.0f, c[a]));
 }
 
 // sample position in the field's normalised [-1,1]^3 grid coordinates (tensorBase.py:438-440,602)

@@ -133,16 +133,9 @@ __device__ __forceinline__ void write_rgb(const BatchDev& B, long long r,
     for (int a = 0; a < 3; ++a) c[a] = B.rgb[B.rgb_stride * r + a] + c[a];
   }
   if (B.finalize) {
-    if (B.exposure) {
-      const long long view = B.rays_per_view > 0 ? r / B.rays_per_view : 0;
-      const float* E = B.exposure + 9 * view;
-      const float o0 = E[0] * c[0] + E[1] * c[1] + E[2] * c[2];
-      const float o1 = E[3] * c[0] + E[4] * c[1] + E[5] * c[2];
-      const float o2 = E[6] * c[0] + E[7] * c[1] + E[8] * c[2];
-      c[0] = o0; c[1] = o1; c[2] = o2;
-    }
-#pragma unroll
-    for (int a = 0; a < 3; ++a) c[a] = fminf(1.0f, fmaxf(0.0f, c[a]));
+    const float* E = nullptr;
+    if (B.exposure) E = B.exposure + 9 * (B.rays_per_view > 0 ? r / B.rays_per_view : 0);
+    finalize_rgb(E, c);
   }
   float* o = B.rgb + B.rgb_stride * r;
   o[0] = c[0]; o[1] = c[1]; o[2] = c[2];

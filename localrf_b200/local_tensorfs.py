@@ -15,13 +15,15 @@ last field's launch).  Differences that are deliberate:
 """
 import ctypes as C
 import math
+import os
 import re
 
 import torch
 
 from . import _lib
 from .optim import adam_step, zero_grad
-from .tensorf import AlphaGridMask, TensorVMSplit, _ptr, _require_cuda, _stream
+from .tensorf import (AlphaGridMask, TensorVMSplit, _check_field_state, _field_grad_buffers, _field_grads,
+                      _field_state, _ptr, _require_cuda, _stream)
 from .utils import N_to_reso, mtx_to_sixD, sixD_to_mtx
 
 
@@ -66,6 +68,96 @@ def _uva_pointer(t):
         raise RuntimeError("localrf_b200: host tensors handed to the render path must be pinned "
                            "(page-locked) memory; pageable memory is not device-accessible")
     return t.data_ptr()
+
+
+def _train_batch(ray_ids, W, H, fov360, cam2world, intr, exposure, w2rf, bg):
+    """LrfBatch of the training call: ray-generation mode, one field, no blend, finalize = 0 (the exposure and the
+    clamp run in lrf_exposure_clamp).  All tensors contiguous fp32 (ray_ids int64) on the device."""
+    b = _lib.LrfBatch()
+    b.n_rays = ray_ids.shape[0]
+    b.ray_ids = ray_ids.data_ptr()
+    b.W, b.H = int(W), int(H)
+    b.fov360 = int(fov360)
+    b.intrinsics = intr.data_ptr()
+    b.cam2world = cam2world.data_ptr()
+    b.n_views = cam2world.shape[0]
+    b.world2rf = w2rf.data_ptr()
+    b.exposure = exposure.data_ptr() if exposure is not None else None
+    b.white_bg = int(bg)
+    return b
+
+
+class _TrainRenderFn(torch.autograd.Function):
+    """The training call of LocalTensorfs.forward for one field (local_tensorfs.py:397-499 with is_train) as ONE
+    autograd node.  Forward: lrf_render generates the rays from the ids and cameras (finalize = 0), then
+    lrf_exposure_clamp.  Backward: lrf_render_backward_batch -- the field's gradients as _RenderFn's, plus those of
+    cam2world [V,3,4], the intrinsics [3] = (focal, cx, cy), the exposure [V,3,3] and world2rf [3], with
+    grad_directions joining the intrinsics' gradient.  -> (rgb, depth, directions, ij); ij is not differentiable.
+
+    `sources` are the leaves the camera inputs were built from (poses, exposure, intrinsics): like the field's
+    parameters, an in-place change to one of them between forward and backward raises."""
+
+    @staticmethod
+    def forward(ctx, rf, z, bg, ray_ids, W, H, fov360, sources, cam2world, intr, exposure, w2rf, *params):
+        dev, n = ray_ids.device, ray_ids.shape[0]
+        cams = [t.detach().to(dev, torch.float32).contiguous() if t is not None else None
+                for t in (cam2world, intr, exposure, w2rf)]
+        c2w, it, E, w2 = cams
+        rgb_lin = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        rgb = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        depth = torch.empty(n, dtype=torch.float32, device=dev)
+        dirs = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        ij = torch.empty(n, 2, dtype=torch.int64, device=dev)
+        lib = _lib.lib()
+        with torch.cuda.device(dev):
+            stream = _stream(dev)
+            fs, prep = rf.field_and_prepared(z, fp32=True)
+            b = _train_batch(ray_ids, W, H, fov360, c2w, it, None, w2, bg)
+            o = _lib.LrfOutputs()
+            o.rgb, o.depth, o.directions, o.ij = rgb_lin.data_ptr(), depth.data_ptr(), dirs.data_ptr(), ij.data_ptr()
+            _lib.check(lib.lrf_render(C.byref(fs), _ptr(prep), C.byref(b), C.byref(o), stream))
+            _lib.check(lib.lrf_exposure_clamp(_ptr(rgb_lin), _ptr(E), n, c2w.shape[0], _ptr(rgb), stream))
+        ctx.rf, ctx.bg, ctx.W, ctx.H, ctx.fov360 = rf, bg, W, H, fov360
+        ctx.seen = _field_state(rf, params)
+        ctx.sources = tuple(sources)
+        ctx.seen_cams = tuple((t.data_ptr(), t._version) for t in ctx.sources)
+        ctx.has_exposure = E is not None
+        ctx.save_for_backward(ray_ids, z, c2w, it, E, w2, rgb_lin)
+        ctx.mark_non_differentiable(ij)
+        return rgb, depth, dirs, ij
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_depth, g_dirs, g_ij):
+        ray_ids, z, c2w, it, E, w2, rgb_lin = ctx.saved_tensors
+        rf, dev, n, V = ctx.rf, ray_ids.device, ray_ids.shape[0], c2w.shape[0]
+        _check_field_state(rf, ctx.seen)
+        if tuple((t.data_ptr(), t._version) for t in ctx.sources) != ctx.seen_cams:
+            raise RuntimeError("localrf_b200: a pose, exposure or intrinsics parameter was modified between the "
+                               "fused training forward and its backward")
+        f32 = lambda g: g.detach().to(torch.float32).contiguous()
+        g_rgb = torch.zeros(n, 3, device=dev) if g_rgb is None else f32(g_rgb)
+        g_depth = torch.zeros(n, device=dev) if g_depth is None else f32(g_depth)
+        g_dirs = None if g_dirs is None else f32(g_dirs)
+        need = ctx.needs_input_grad
+        d_c2w = torch.empty(V, 3, 4, device=dev) if need[8] else None
+        d_intr = torch.empty(3, device=dev) if need[9] else None
+        d_expo = torch.empty(V, 3, 3, device=dev) if ctx.has_exposure and need[10] else None
+        d_w2 = torch.empty(3, device=dev) if need[11] else None
+        bufs, g = _field_grad_buffers(rf, dev)
+        cg = _lib.LrfCameraGrads()
+        cg.d_cam2world, cg.d_intrinsics = _ptr(d_c2w), _ptr(d_intr)
+        cg.d_exposure, cg.d_world2rf = _ptr(d_expo), _ptr(d_w2)
+        lib = _lib.lib()
+        with torch.cuda.device(dev):
+            fs, _ = rf.field_and_prepared(z, fp32=True)
+            bp = rf._prepared_backward()
+            b = _train_batch(ray_ids, ctx.W, ctx.H, ctx.fov360, c2w, it, E, w2, ctx.bg)
+            scratch = torch.empty(lib.lrf_backward_batch_scratch_bytes(n, z.numel(), V), dtype=torch.uint8,
+                                  device=dev)
+            _lib.check(lib.lrf_render_backward_batch(C.byref(fs), _ptr(bp), C.byref(b), _ptr(rgb_lin), _ptr(g_rgb),
+                                                     _ptr(g_depth), _ptr(g_dirs), C.byref(g), C.byref(cg),
+                                                     _ptr(scratch), scratch.numel(), _stream(dev)))
+        return (None,) * 8 + (d_c2w, d_intr, d_expo, d_w2) + _field_grads(rf, bufs)
 
 
 class LocalTensorfs(torch.nn.Module):
@@ -411,6 +503,46 @@ class LocalTensorfs(torch.nn.Module):
             rgbs = torch.bmm(exposure, rgbs[..., None])[..., 0]
         return rgbs.clamp(0, 1), depth_maps, directions, ij
 
+    def _forward_train(self, ray_ids, ids, W, H, white_bg, cam2world, world2rf, k, chunk, test_id):
+        """The training call under autograd for a field _RenderFn covers: one _TrainRenderFn node per chunk (each
+        with its own distance-table draw, then its background coin, in the composed path's RNG order)."""
+        dev = ray_ids.device
+        n, n_views = ray_ids.shape[0], len(ids)
+        rf = self.tensorfs[k]
+        sources = [self.init_focal, self.focal_offset, self.center_rel]
+        if cam2world is None:
+            cam2world = self.get_cam2world(ids)
+            sources += [self.r_c2w[i] for i in ids] + [self.t_c2w[i] for i in ids]
+        # focal(W) and center(W, H) without center()'s host-to-device copy: the same fp32 products
+        intr = torch.cat([self.focal(W).reshape(1), self.center_rel[0:1] * W, self.center_rel[1:2] * H])
+        exposure = None
+        if self.lr_exposure_init > 0:
+            if test_id:
+                exposure = self._exposure_for(ids, True, dev)
+            else:
+                exposure = torch.stack([self.exposure[v] for v in ids], dim=0)
+            sources += list(self.exposure) if test_id else [self.exposure[v] for v in ids]
+        w2 = world2rf[k]
+        sources.append(w2)
+        rays_i = ray_ids
+        if rays_i.dtype != torch.int64 or not rays_i.is_contiguous():
+            rays_i = rays_i.to(torch.int64).contiguous()
+        per_view = n // n_views
+        step = n if n <= chunk else max(per_view, (chunk // per_view) * per_view)
+        params = rf._grad_params()
+        outs = []
+        for lo in range(0, n, step):
+            hi = min(lo + step, n)
+            v_lo, v_hi = lo // per_view, hi // per_view
+            z = rf.sample_table(True, -1, dev)
+            bg = bool(white_bg) or bool(torch.rand((1,)) < 0.5)     # tensorBase.py:633, after the table's jitter
+            outs.append(_TrainRenderFn.apply(rf, z, bg, rays_i[lo:hi], W, H, self.fov == 360, sources,
+                                             cam2world[v_lo:v_hi], intr,
+                                             None if exposure is None else exposure[v_lo:v_hi], w2, *params))
+        if len(outs) == 1:
+            return outs[0]
+        return tuple(torch.cat([o[i] for o in outs]) for i in range(4))
+
     def _cached(self, slot, key, build, refs=()):
         """Small memo for tensors derived from parameters: rebuilt when the key changes.  Keys are made
         of ids + version counters of the source tensors; `refs` keeps those tensors alive while the
@@ -421,6 +553,13 @@ class LocalTensorfs(torch.nn.Module):
             hit = (key, build(), tuple(refs))
             c[slot] = hit
         return hit[1]
+
+    def _train_node_covers(self, k, floater_thresh):
+        """Whether a training call of field k runs as one _TrainRenderFn node: the fields _RenderFn covers
+        (pe = 0, no floater filter) unless LRF_TRAIN_PATH=composed selects the torch-op path."""
+        rf = self.tensorfs[k]
+        return (rf.fused_supported() and rf.fea_pe == 0 and rf.view_pe == 0 and floater_thresh == 0
+                and os.environ.get("LRF_TRAIN_PATH", "fused") != "composed")
 
     def _blend_host(self):
         bw = self.blending_weights
@@ -578,6 +717,9 @@ class LocalTensorfs(torch.nn.Module):
                 raise NotImplementedError("exchange= / out= are served by the fused eval path only")
             if not ray_ids.is_cuda:
                 ray_ids = ray_ids.to(dev)
+            if needs_composed and is_train and self._train_node_covers(active[0], floater_thresh):
+                return self._forward_train(ray_ids, ids, W, H, white_bg, cam2world, world2rf, active[0], chunk,
+                                           test_id)
             return self._forward_autograd(ray_ids, view_ids, ids, W, H, white_bg, is_train,
                                           cam2world, world2rf, blend, active, chunk, test_id,
                                           floater_thresh)

@@ -86,6 +86,53 @@ class _VMLookup(torch.autograd.Function):
         return (None, None, d_xyz, *d_planes, *d_lines)
 
 
+def _field_state(m, params):
+    """What a fused backward recomputes from: the parameters' storage and versions, the grid size and the alpha
+    mask.  The backward compares it with the forward's to catch in-place updates in between."""
+    am = m.alphaMask
+    return (tuple((p.data_ptr(), p._version) for p in params), tuple(m._grid_host),
+            None if am is None else (am.alpha_volume.data_ptr(), am.alpha_volume._version))
+
+
+def _check_field_state(m, seen):
+    if _field_state(m, m._grad_params()) != seen:
+        raise RuntimeError("localrf_b200: a parameter (or the grid size / alpha mask) of the field was "
+                           "modified between the fused forward and its backward; the backward "
+                           "recomputes from the live parameters and would return gradients of a "
+                           "different model")
+
+
+def _field_grad_buffers(m, dev):
+    """Zeroed gradient buffers laid out like the field's parameters (d_w1b = d(mlp[0].weight @ basis_mat.weight))
+    and the LrfGradients struct pointing at them (d_rays left NULL) -> (buffers, struct)."""
+    rm = m.renderModule
+    cl = torch.channels_last
+    d_dp = [torch.zeros_like(p, memory_format=cl) for p in m.density_plane]
+    d_dl = [torch.zeros_like(p, memory_format=cl) for p in m.density_line]
+    d_ap = [torch.zeros_like(p, memory_format=cl) for p in m.app_plane]
+    d_al = [torch.zeros_like(p, memory_format=cl) for p in m.app_line]
+    d_w1b = torch.zeros(rm.mlp[0].weight.shape[0], m.basis_mat.weight.shape[1], device=dev)
+    d_b1, d_w2, d_b2 = (torch.zeros_like(t) for t in (rm.mlp[0].bias, rm.mlp[2].weight, rm.mlp[2].bias))
+    d_w3, d_b3 = torch.zeros_like(rm.mlp_view[0].weight), torch.zeros_like(rm.mlp_view[0].bias)
+    g = _lib.LrfGradients()
+    for i in range(3):
+        g.d_dplane[i], g.d_dline[i] = d_dp[i].data_ptr(), d_dl[i].data_ptr()
+        g.d_aplane[i], g.d_aline[i] = d_ap[i].data_ptr(), d_al[i].data_ptr()
+    g.d_w1b, g.d_b1, g.d_w2 = d_w1b.data_ptr(), d_b1.data_ptr(), d_w2.data_ptr()
+    g.d_b2, g.d_w3, g.d_b3 = d_b2.data_ptr(), d_w3.data_ptr(), d_b3.data_ptr()
+    return (d_dp, d_dl, d_ap, d_al, d_w1b, d_b1, d_w2, d_b2, d_w3, d_b3), g
+
+
+def _field_grads(m, bufs):
+    """The buffers of _field_grad_buffers as gradients in _grad_params order.  W1B = mlp[0].weight @
+    basis_mat.weight was folded for the kernel: its gradient is unfolded here."""
+    d_dp, d_dl, d_ap, d_al, d_w1b, d_b1, d_w2, d_b2, d_w3, d_b3 = bufs
+    w1, basis = m.renderModule.mlp[0].weight, m.basis_mat.weight
+    d_w1 = d_w1b @ basis.detach().t()
+    d_basis = w1.detach().t() @ d_w1b
+    return (*d_dp, *d_dl, *d_ap, *d_al, d_basis, d_w1, d_b1, d_w2, d_b2, d_w3, d_b3)
+
+
 class _RenderFn(torch.autograd.Function):
     """TensorBase.forward as ONE autograd node: the forward is the fused render kernel (lrf_render),
     the backward is lrf_render_backward (march again -> MLP backward over the shaded samples ->
@@ -100,9 +147,7 @@ class _RenderFn(torch.autograd.Function):
         # the backward re-reads the module's live parameters (nothing per-sample is saved): remember
         # what the forward saw, so an in-place update / upsample / mask rebuild in between raises like
         # torch's own version-counter check would instead of producing gradients of a different model
-        am = module.alphaMask
-        ctx.seen = (tuple((p.data_ptr(), p._version) for p in params), tuple(module._grid_host),
-                    None if am is None else (am.alpha_volume.data_ptr(), am.alpha_volume._version))
+        ctx.seen = _field_state(module, params)
         ctx.save_for_backward(rays_c, z)
         return rgb, depth
 
@@ -110,27 +155,12 @@ class _RenderFn(torch.autograd.Function):
     def backward(ctx, g_rgb, g_depth):
         rays, z = ctx.saved_tensors
         m, dev, n = ctx.module, rays.device, rays.shape[0]
-        am = m.alphaMask
-        now = (tuple((p.data_ptr(), p._version) for p in m._grad_params()), tuple(m._grid_host),
-               None if am is None else (am.alpha_volume.data_ptr(), am.alpha_volume._version))
-        if now != ctx.seen:
-            raise RuntimeError("localrf_b200: a parameter (or the grid size / alpha mask) of the field was "
-                               "modified between the fused forward and its backward; the backward "
-                               "recomputes from the live parameters and would return gradients of a "
-                               "different model")
+        _check_field_state(m, ctx.seen)
         g_rgb = torch.zeros(n, 3, device=dev) if g_rgb is None else g_rgb.detach().to(torch.float32).contiguous()
         g_depth = torch.zeros(n, device=dev) if g_depth is None else g_depth.detach().to(torch.float32).contiguous()
-        rm = m.renderModule
-        cl = torch.channels_last
-        d_dp = [torch.zeros_like(p, memory_format=cl) for p in m.density_plane]
-        d_dl = [torch.zeros_like(p, memory_format=cl) for p in m.density_line]
-        d_ap = [torch.zeros_like(p, memory_format=cl) for p in m.app_plane]
-        d_al = [torch.zeros_like(p, memory_format=cl) for p in m.app_line]
-        w1, basis = rm.mlp[0].weight, m.basis_mat.weight
-        d_w1b = torch.zeros(w1.shape[0], basis.shape[1], device=dev)
-        d_b1, d_w2, d_b2 = (torch.zeros_like(t) for t in (rm.mlp[0].bias, rm.mlp[2].weight, rm.mlp[2].bias))
-        d_w3, d_b3 = torch.zeros_like(rm.mlp_view[0].weight), torch.zeros_like(rm.mlp_view[0].bias)
+        bufs, g = _field_grad_buffers(m, dev)
         d_rays = torch.empty_like(rays)
+        g.d_rays = d_rays.data_ptr()
         lib = _lib.lib()
         with torch.cuda.device(dev):
             fs, _ = m.field_and_prepared(z, fp32=True)
@@ -139,21 +169,10 @@ class _RenderFn(torch.autograd.Function):
             # per call, from torch's caching allocator (stream-ordered reuse): backwards of the same module on
             # different streams never share a scratch block
             scratch = torch.empty(need, dtype=torch.uint8, device=dev)
-            g = _lib.LrfGradients()
-            g.d_rays = d_rays.data_ptr()
-            for i in range(3):
-                g.d_dplane[i], g.d_dline[i] = d_dp[i].data_ptr(), d_dl[i].data_ptr()
-                g.d_aplane[i], g.d_aline[i] = d_ap[i].data_ptr(), d_al[i].data_ptr()
-            g.d_w1b, g.d_b1, g.d_w2 = d_w1b.data_ptr(), d_b1.data_ptr(), d_w2.data_ptr()
-            g.d_b2, g.d_w3, g.d_b3 = d_b2.data_ptr(), d_w3.data_ptr(), d_b3.data_ptr()
             _lib.check(lib.lrf_render_backward(C.byref(fs), _ptr(bp), _ptr(rays), n, int(ctx.white_bg),
                                                _ptr(g_rgb), _ptr(g_depth), C.byref(g), _ptr(scratch),
                                                scratch.numel(), _stream(dev)))
-        # W1B = mlp[0].weight @ basis_mat.weight was folded for the kernel: unfold its gradient
-        d_w1 = d_w1b @ basis.detach().t()
-        d_basis = w1.detach().t() @ d_w1b
-        return (None, None, None, d_rays, *d_dp, *d_dl, *d_ap, *d_al, d_basis, d_w1, d_b1, d_w2, d_b2,
-                d_w3, d_b3)
+        return (None, None, None, d_rays, *_field_grads(m, bufs))
 
 
 class _DensityL1Fn(torch.autograd.Function):
