@@ -153,7 +153,8 @@ typedef struct LrfOutputs {
 int lrf_version(void);
 const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
- * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor, 7 LrfCameraGrads (0 for any other index).  Bindings compare these with their own mirrors at load
+ * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor, 7 LrfCameraGrads, 8 LrfFrameStore,
+ * 9 LrfRayGather (0 for any other index).  Bindings compare these with their own mirrors at load
  * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
@@ -434,6 +435,44 @@ typedef struct LrfAdamTensor {
 /* t: HOST array of n entries, read before the call returns.  One launch per 448 tensors; no atomics, no host
  * synchronisation, bitwise repeatable.  n == 0 does nothing. */
 int lrf_adam_step(const LrfAdamTensor *t, int64_t n, lrf_stream_t stream);
+
+/* Training rays from device-resident frames.  replaces: the numpy gather of LocalRFDataset.sample
+ * (dataLoader/localrf_dataset.py:273-315, `self.all_*[idx_sample]`) and the uploads of train.py:352-356.  The host
+ * keeps drawing the view and pixel ids (the reference's RNG); the frames stay on the device.
+ * A ring of frame slots, one fp32 array per quantity; frame f lives in slot f % capacity. */
+typedef struct LrfFrameStore {
+  int64_t n_px;                /* pixels per frame */
+  int64_t capacity;            /* slots */
+  const int64_t *slot_frame;   /* [capacity] frame id each slot holds (anything negative = empty) */
+  const float *rgb;            /* [capacity][n_px][3] */
+  const float *loss_weight;    /* [capacity][n_px] */
+  const float *invdepth;       /* [capacity][n_px], or NULL (no depth) */
+  const float *fwd_flow;       /* [capacity][n_px][2] \                                          */
+  const float *fwd_mask;       /* [capacity][n_px]     | the flow group: all four, or all NULL   */
+  const float *bwd_flow;       /* [capacity][n_px][2]  | (no flow)                               */
+  const float *bwd_mask;       /* [capacity][n_px]    /                                          */
+} LrfFrameStore;
+
+/* One batch: view-major rays, ray r belongs to view r / (n_rays / n_views), as the reference orders them.  Outputs
+ * of a group the store has must be set; those of a group it lacks must be NULL. */
+typedef struct LrfRayGather {
+  int64_t n_rays;
+  int64_t n_views;             /* n_rays % n_views == 0 */
+  const int64_t *ids;          /* [n_views + n_rays]: the views' frame ids, then each ray's pixel within its frame */
+  int64_t *idx;                /* [n_rays] view * n_px + pixel (the reference's `idx`) */
+  float *rgb;                  /* [n_rays][3] */
+  float *loss_weight;          /* [n_rays] */
+  float *invdepth;             /* [n_rays] */
+  float *fwd_flow;             /* [n_rays][2] */
+  float *fwd_mask;             /* [n_rays] */
+  float *bwd_flow;             /* [n_rays][2] */
+  float *bwd_mask;             /* [n_rays] */
+} LrfRayGather;
+
+/* One launch, one thread per ray.  A ray whose view is not the frame its slot holds, or whose pixel is negative or
+ * >= n_px, gets NaN in every output row (its idx is still written); no other frame's data is read.  The ids are
+ * never read on the host.  No atomics, no host synchronisation. */
+int lrf_gather_rays(const LrfFrameStore *store, const LrfRayGather *g, lrf_stream_t stream);
 
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */

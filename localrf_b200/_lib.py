@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
-           "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_abi.cu"]
+           "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -66,6 +66,17 @@ class LrfAdamTensor(C.Structure):
                 ("eps", C.c_float), ("step_size", C.c_float), ("bc2_sqrt", C.c_float)]
 
 
+class LrfFrameStore(C.Structure):
+    _fields_ = [("n_px", C.c_int64), ("capacity", C.c_int64), ("slot_frame", _vp), ("rgb", _vp), ("loss_weight", _vp),
+                ("invdepth", _vp), ("fwd_flow", _vp), ("fwd_mask", _vp), ("bwd_flow", _vp), ("bwd_mask", _vp)]
+
+
+class LrfRayGather(C.Structure):
+    _fields_ = [("n_rays", C.c_int64), ("n_views", C.c_int64), ("ids", _vp), ("idx", _vp), ("rgb", _vp),
+                ("loss_weight", _vp), ("invdepth", _vp), ("fwd_flow", _vp), ("fwd_mask", _vp), ("bwd_flow", _vp),
+                ("bwd_mask", _vp)]
+
+
 class LrfBatch(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int64),
@@ -112,7 +123,7 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_tv_sums_backward", "lrf_sample_ray", "lrf_frame_to_u8", "lrf_pack_bf16",
            "lrf_image_metrics_scratch_bytes", "lrf_image_metrics", "lrf_supervision_scratch_bytes",
            "lrf_supervision_losses", "lrf_supervision_losses_backward", "lrf_adam_step",
-           "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch"]
+           "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch", "lrf_gather_rays"]
 
 
 def _stale():
@@ -166,7 +177,7 @@ def lib():
     L.lrf_sizeof.restype = C.c_size_t
     L.lrf_sizeof.argtypes = [C.c_int32]
     for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
-                                     LrfAdamTensor, LrfCameraGrads)):
+                                     LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather)):
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -216,6 +227,7 @@ def lib():
     L.lrf_supervision_losses_backward.argtypes = [C.POINTER(LrfLossBatch), _vp, C.POINTER(LrfLossGrads), _vp,
                                                   C.c_size_t, _vp]
     L.lrf_adam_step.argtypes = [_vp, C.c_int64, _vp]        # LrfAdamTensor array: a ctypes array or packed bytes
+    L.lrf_gather_rays.argtypes = [C.POINTER(LrfFrameStore), C.POINTER(LrfRayGather), _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

@@ -55,6 +55,7 @@ cudaError_t launch_supervision_losses(const LrfLossBatch& b, float* losses, void
 cudaError_t launch_supervision_losses_backward(const LrfLossBatch& b, const float* grad_losses, const LrfLossGrads& g,
                                                void* scratch, cudaStream_t stream);
 cudaError_t launch_adam_step(const LrfAdamTensor* t, long long n, cudaStream_t stream);
+cudaError_t launch_gather_rays(const LrfFrameStore& s, const LrfRayGather& g, cudaStream_t stream);
 cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
                                 cudaStream_t stream);
 cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
@@ -212,6 +213,8 @@ size_t lrf_sizeof(int32_t which) {
     case 5: return sizeof(LrfLossGrads);
     case 6: return sizeof(LrfAdamTensor);
     case 7: return sizeof(LrfCameraGrads);
+    case 8: return sizeof(LrfFrameStore);
+    case 9: return sizeof(LrfRayGather);
     default: return 0;
   }
 }
@@ -745,6 +748,31 @@ int lrf_adam_step(const LrfAdamTensor* t, int64_t n, lrf_stream_t stream) {
   }
   cudaError_t e = lrf::launch_adam_step(t, n, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e, "adam_kernel");
+  return LRF_OK;
+}
+
+int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t stream) {
+  if (!s || !g) return fail(LRF_ERR_INVALID, "store / gather is NULL");
+  if (s->n_px < 1) return fail(LRF_ERR_INVALID, "n_px must be >= 1");
+  if (s->capacity < 1) return fail(LRF_ERR_INVALID, "capacity must be >= 1");
+  if (!s->slot_frame || !s->rgb || !s->loss_weight)
+    return fail(LRF_ERR_INVALID, "slot_frame / rgb / loss_weight of the store is NULL");
+  const int n_flow = !!s->fwd_flow + !!s->fwd_mask + !!s->bwd_flow + !!s->bwd_mask;
+  if (n_flow != 0 && n_flow != 4)
+    return fail(LRF_ERR_INVALID, "the store's flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, "
+                                 "bwd_mask or none");
+  if (g->n_rays < 0 || g->n_views < 1 || g->n_rays % g->n_views != 0)
+    return fail(LRF_ERR_INVALID, "n_rays must be a multiple of n_views >= 1");
+  if (g->n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  if (!g->ids || !g->idx || !g->rgb || !g->loss_weight)
+    return fail(LRF_ERR_INVALID, "ids / idx / rgb / loss_weight of the gather is NULL");
+  if (!s->invdepth != !g->invdepth)
+    return fail(LRF_ERR_INVALID, "the invdepth output must be set exactly when the store has invdepth");
+  const int n_flow_out = !!g->fwd_flow + !!g->fwd_mask + !!g->bwd_flow + !!g->bwd_mask;
+  if (n_flow_out != n_flow)
+    return fail(LRF_ERR_INVALID, "the flow outputs must be set exactly when the store has the flow group");
+  cudaError_t e = lrf::launch_gather_rays(*s, *g, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "gather_rays_kernel");
   return LRF_OK;
 }
 
