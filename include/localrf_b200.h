@@ -398,7 +398,8 @@ size_t lrf_supervision_scratch_bytes(int64_t n_rays, int64_t n_views, int64_t n_
  * (the id cannot be checked on the host without a synchronisation).  A MAD of 0 gives NaN/inf, as in the
  * reference.  The scratch keeps the forward's decisions for the backward; its leading part is, in bytes:
  * e [N] fp32 at 0, d [N] fp32 at 4N (both before the cut), tau [2][V] fp32 at 8N (flow, then depth thresholds),
- * median ray indices [V][2] int32 at 8N + 8V (x, then g).  Entries of a term that is off are not written.
+ * median ray indices [V][2] int32 at 8N + 8V (x, then g: the lowest ray index holding the median value, which is
+ * NaN when the view holds a NaN, as torch.median's).  Entries of a term that is off are not written.
  * No atomics, no host synchronisation: bitwise repeatable.  R > 4096 is LRF_ERR_UNSUPPORTED. */
 int lrf_supervision_losses(const LrfLossBatch *batch, float *losses, void *scratch, size_t scratch_bytes,
                            lrf_stream_t stream);

@@ -5,7 +5,8 @@
 // 0.8 quantile.
 //
 // Forward: one CTA per view sorts (value, ray index) keys in shared memory (bitonic), so the selections are
-// exact: the medians are sorted[(R-1)/2] (torch.median's lower median; ties go to the lowest ray index) and
+// exact: the medians are torch.median's (the lower median sorted[(R-1)/2], or NaN when the view holds one; of the
+// rays holding that value, the one with the lowest index) and
 // each quantile is torch.quantile's linear interpolation, fp32 rank and fused two-branch lerp included, so the
 // thresholds are bit-identical to torch's over the same rows.  The per-ray e and d, both thresholds, the median
 // indices and the MAD scales go to caller scratch with the per-view partial sums; a one-CTA kernel sums the
@@ -66,8 +67,9 @@ static LossPtrs carve(void* scratch, long long N, long long V) {
 }
 
 // ---- device helpers -------------------------------------------------------------------------------------
-__device__ inline unsigned int f2key(float f) {      // order-preserving; +NaN sorts after +inf
-  const unsigned int u = __float_as_uint(f);
+// order-preserving; every NaN becomes the canonical +NaN first, so that NaNs of either sign sort after +inf
+__device__ inline unsigned int f2key(float f) {
+  const unsigned int u = isnan(f) ? 0x7fffffffu : __float_as_uint(f);
   return u ^ ((u >> 31) ? 0xffffffffu : 0x80000000u);
 }
 __device__ inline float key2f(unsigned long long k) {
@@ -104,6 +106,20 @@ __device__ inline float sorted_quantile(const unsigned long long* k, int R, floa
   const float a = key2f(k[lo]), b = key2f(k[hi]);
   const float diff = __fsub_rn(b, a);
   return fabsf(w) < 0.5f ? __fmaf_rn(w, diff, a) : __fmaf_rn(-diff, __fsub_rn(1.0f, w), b);
+}
+
+// torch.median(row) over R sorted keys: the lower median sorted[(R-1)/2], or NaN when the row holds one.  Keys order
+// equal values by ray index, so the first key of the value's run is the lowest ray holding it.
+__device__ inline unsigned long long sorted_median(const unsigned long long* k, int R) {
+  int hi = isnan(key2f(k[R - 1])) ? R - 1 : (R - 1) >> 1;
+  const unsigned long long run = k[hi] & 0xffffffff00000000ull;
+  int lo = 0;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (k[mid] < run) lo = mid + 1;
+    else hi = mid;
+  }
+  return k[lo];
 }
 
 __device__ inline double block_sum_d(double v, double* red) {      // result valid in thread 0
@@ -258,7 +274,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) losses_view_kernel(LrfLossBatch 
           keys[i] = i < R ? ((unsigned long long)f2key(b.invdepths[base + i]) << 32) | (unsigned int)i : ~0ull;
       }
       bitonic_sort(keys, P);
-      const unsigned long long mk = keys[(R - 1) >> 1];
+      const unsigned long long mk = sorted_median(keys, R);
       const float t = key2f(mk);
       double mad = 0.0;
       for (int i = threadIdx.x; i < R; i += blockDim.x) mad += (double)fabsf(key2f(keys[i]) - t);

@@ -2,6 +2,8 @@
 mono-depth terms), written from the formulas, and the fp32 selection formulas the kernels use.
 
     losses_f64(case)            -> (losses [3] float64, {name: gradient}) for a dict of inputs
+    losses_f64(case, decisions=decisions_of(arrays))
+                                -> the same with the kernel's cuts and medians (the arithmetic stays float64)
     quantile_fp32(rows, q)      -> torch.quantile(rows, q, dim=1) in fp32, restated (numpy)
     lower_median(rows)          -> (values, indices) of torch.median(rows, dim=1), ties to the lowest index
     torch_block(kw)             -> the three losses as the reference's train.py computes them, in torch ops on
@@ -56,15 +58,21 @@ def _quantile_f64(x, q):
     return s[:, lo] + w * (s[:, hi] - s[:, lo])
 
 
-def _median(x):
+def _median_index(x):
     k = (x.shape[1] - 1) // 2
-    idx = torch.sort(x, dim=1, stable=True).indices[:, k:k + 1]
-    return torch.gather(x, 1, idx)
+    return torch.sort(x, dim=1, stable=True).indices[:, k]
 
 
-def losses_f64(c, flow_weight=None, depth_weight=None, return_arrays=False):
+def losses_f64(c, flow_weight=None, depth_weight=None, return_arrays=False, decisions=None):
     """c: dict of the inputs (numpy or tensors, as stored in tests/golden/train_losses.npz).  Gradients of
-    L_rgb + L_flow + L_depth with respect to GRAD_NAMES, in float64."""
+    L_rgb + L_flow + L_depth with respect to GRAD_NAMES, in float64.
+
+    decisions: None (the selections are made here, in float64), or a dict of the hard decisions to use instead:
+    "flow_cut" and "depth_cut" (bool [V,R], the rays zeroed above the thresholds) and "median_x" / "median_g"
+    (int [V], the ray within each view whose 1 / clamp(depth) and invdepths are the medians).  The kernels'
+    return_arrays=True output gives all four (decisions_of); return_arrays=True here returns this call's own
+    under "decisions".  Everything else stays float64: at ties or within rounding of a threshold the float64
+    selections may differ from fp32 ones, and this keeps the arithmetic comparable there."""
     t = lambda k, dt=torch.float64: torch.as_tensor(np.asarray(c[k])).to(dt)
     p = {k: t(k).clone().requires_grad_() for k in GRAD_NAMES}
     view_ids = t("view_ids", torch.int64)
@@ -96,23 +104,44 @@ def losses_f64(c, flow_weight=None, depth_weight=None, return_arrays=False):
         v = -q[..., 1] / z * f + cy - 0.5 - ij[..., 1]
         fl = t(flow_key).reshape(V, -1, 2)
         e = e + (torch.abs(u - fl[..., 0]) + torch.abs(v - fl[..., 1])) * mask
+    given = {} if decisions is None else decisions
+    own = {}
+    pick = lambda k, dt: torch.as_tensor(given[k]).cpu().to(dt) if given.get(k) is not None else own[k]
     tau_f = _quantile_f64(e.detach(), 0.9)
-    flow = torch.where(e > tau_f[:, None], 0, e).mean() * fw
+    own["flow_cut"] = e.detach() > tau_f[:, None]
+    flow = torch.where(pick("flow_cut", torch.bool), 0, e).mean() * fw
 
     # depth: lower medians, mean absolute deviations
-    def norm(x):
-        m = _median(x)
+    def norm(x, key):
+        own[key] = _median_index(x.detach())
+        m = torch.gather(x, 1, pick(key, torch.int64)[:, None])
         return (x - m) / torch.abs(x - m).mean(dim=1, keepdim=True)
-    d = (norm(1 / torch.clamp(depth, min=1e-6)) - norm(t("invdepths").reshape(V, -1))) ** 2
+    d = (norm(1 / torch.clamp(depth, min=1e-6), "median_x") - norm(t("invdepths").reshape(V, -1), "median_g")) ** 2
     tau_d = _quantile_f64(d.detach(), 0.8)
-    dl = torch.where(d > tau_d[:, None], 0, d).mean() * dw
+    own["depth_cut"] = d.detach() > tau_d[:, None]
+    dl = torch.where(pick("depth_cut", torch.bool), 0, d).mean() * dw
 
     (rgb + flow + dl).backward()
     losses = torch.stack([rgb, flow, dl]).detach()
     grads = {k: p[k].grad for k in GRAD_NAMES}
     if return_arrays:
-        return losses, grads, {"flow": e.detach(), "depth": d.detach(), "flow_tau": tau_f, "depth_tau": tau_d}
+        return losses, grads, {"flow": e.detach(), "depth": d.detach(), "flow_tau": tau_f, "depth_tau": tau_d,
+                               "decisions": own}
     return losses, grads
+
+
+def decisions_of(arr, flow=True, depth=True):
+    """The hard decisions in supervision_losses(..., return_arrays=True)'s arrays, as losses_f64 takes them: the
+    cuts are the kernel's rows above the kernel's thresholds.  A term the call did not compute (flow / depth
+    False) leaves its parts out, and losses_f64 makes those selections itself."""
+    out = {}
+    if flow:
+        out["flow_cut"] = (arr["flow"] > arr["flow_tau"][:, None]).cpu()
+    if depth:
+        idx = arr["depth_median_index"].long().cpu()
+        out.update(depth_cut=(arr["depth"] > arr["depth_tau"][:, None]).cpu(), median_x=idx[:, 0],
+                   median_g=idx[:, 1])
+    return out
 
 
 def torch_block(kw):
