@@ -326,10 +326,15 @@ int lrf_sample_ray(const float *rays, const float *jitter, int64_t N, int32_t S,
  * (rgb_map.cpu() ... cv2.imwrite(255 * rgb[..., ::-1]); visualize_depth -> cv2.applyColorMap, utils/utils.py:
  * 179-197).  rgb [N] x 3 floats `rgb_stride` apart, depth [N] floats `depth_stride` apart (3 / 1, or 4 / 4 for the
  * interleaved pix layout) -> rgb8 [N][3] 8-bit BGR and depth8 [N][3] = lut[(uint8)(255 * clip((d - d_lo) /
- * (d_hi - d_lo + 1e-8), 0, 1))] with lut [256][3] (the caller's colour map, e.g. cv2.COLORMAP_JET).  Either
- * output may be NULL.  Outputs may live in pinned host memory (zero-copy). */
+ * (d_hi - d_lo + 1e-8), 0, 1))] with lut [256][3] (the caller's colour map, e.g. cv2.COLORMAP_JET).  NaN depths
+ * count as 0.  The bounds are doubles, as visualize_depth's Python numbers are: the denominator d_hi - d_lo + 1e-8
+ * is formed in double and rounded to float once, d_lo is rounded to float, and the rest is fp32, which is what numpy
+ * does with a float32 frame.  Either output may be NULL.  Outputs may live in pinned host memory (zero-copy).
+ * Difference from the reference: rgb values with 255 * v >= 2^31 (and +inf) give 255, where OpenCV's float -> 8-bit
+ * conversion on x86-64 gives 0; below that, NaN and -inf give what OpenCV gives (NaN and -inf give 0).  The renderer
+ * clamps rgb to [0, 1] before this step. */
 int lrf_frame_to_u8(const float *rgb, int32_t rgb_stride, const float *depth, int32_t depth_stride, int64_t N,
-                    float d_lo, float d_hi, const unsigned char *lut, unsigned char *rgb8, unsigned char *depth8,
+                    double d_lo, double d_hi, const unsigned char *lut, unsigned char *rgb8, unsigned char *depth8,
                     lrf_stream_t stream);
 
 /* Test-frame metrics on the device.  replaces: renderer.py:162-163, `mse = ((gt_rgb - rgb_map) ** 2).mean()` and

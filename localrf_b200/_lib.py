@@ -153,7 +153,7 @@ def build(force=False, verbose=False):
 _lib = None
 
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 def lib():
@@ -216,7 +216,8 @@ def lib():
     L.lrf_tv_sums_backward.argtypes = [_vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_float, C.c_float, _vp, _vp]
     L.lrf_sample_ray.argtypes = [_vp, _vp, C.c_int64, C.c_int32, C.c_float * 6, C.c_float, C.c_float, C.c_float,
                                  _vp, _vp, _vp, _vp]
-    L.lrf_frame_to_u8.argtypes = [_vp, C.c_int32, _vp, C.c_int32, C.c_int64, C.c_float, C.c_float, _vp, _vp, _vp, _vp]
+    L.lrf_frame_to_u8.argtypes = [_vp, C.c_int32, _vp, C.c_int32, C.c_int64, C.c_double, C.c_double, _vp, _vp, _vp,
+                                  _vp]
     L.lrf_image_metrics_scratch_bytes.restype = C.c_size_t
     L.lrf_image_metrics_scratch_bytes.argtypes = [C.c_int32] * 3
     L.lrf_image_metrics.argtypes = [_vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32,

@@ -44,7 +44,7 @@ cudaError_t launch_sample_ray(const float* rays, const float* jitter, long long 
 cudaError_t launch_peer_barrier(unsigned long long* const* peer_flags, int rank, int world,
                                 unsigned long long seq, unsigned long long wait_seq, cudaStream_t stream);
 cudaError_t launch_frame_u8(const float* rgb, int rgb_stride, const float* depth, int depth_stride, long long N,
-                            float d_lo, float d_hi, const unsigned char* lut, unsigned char* rgb8,
+                            double d_lo, double d_hi, const unsigned char* lut, unsigned char* rgb8,
                             unsigned char* depth8, int n_sms, cudaStream_t stream);
 size_t metrics_scratch_bytes(int H, int W);
 cudaError_t launch_image_metrics(const float* img, int img_stride, const float* gt, int gt_stride, int H, int W,
@@ -201,7 +201,7 @@ int make_field(const LrfField* f, bool need_mlp, bool need_table, const void* pr
 
 extern "C" {
 
-int lrf_version(void) { return 3; }
+int lrf_version(void) { return 4; }
 
 size_t lrf_sizeof(int32_t which) {
   switch (which) {
@@ -655,7 +655,7 @@ int lrf_sample_ray(const float* rays, const float* jitter, int64_t N, int32_t S,
 }
 
 int lrf_frame_to_u8(const float* rgb, int32_t rgb_stride, const float* depth, int32_t depth_stride, int64_t N,
-                    float d_lo, float d_hi, const unsigned char* lut, unsigned char* rgb8, unsigned char* depth8,
+                    double d_lo, double d_hi, const unsigned char* lut, unsigned char* rgb8, unsigned char* depth8,
                     lrf_stream_t stream) {
   if (N < 0) return fail(LRF_ERR_INVALID, "N < 0");
   if (rgb8 && (!rgb || rgb_stride < 3)) return fail(LRF_ERR_INVALID, "rgb8 requested without rgb / stride >= 3");

@@ -313,8 +313,13 @@ __global__ void sample_ray_kernel(const float* __restrict__ rays, const float* _
 // depth -> colour-mapped 8-bit BGR through a 256-entry lookup table (cv2.applyColorMap of
 // (255 * clip((d - lo) / (hi - lo + 1e-8), 0, 1)).astype(uint8)); both are written where the caller points --
 // pinned host memory included, so a finished frame leaves the GPU as 6 bytes per pixel.
+// The depth bounds arrive as lo = (float)d_lo and den = (float)(d_hi - d_lo + 1e-8), the denominator formed in
+// double on the host: numpy does exactly this with a float32 frame and Python-number bounds.
+// rgb equals OpenCV's x86-64 float -> 8U conversion for |255 v| < 2^31, NaN and -inf (both 0).  At or above 2^31
+// and at +inf this writes 255 where OpenCV's cvRound overflows to INT_MIN and writes 0; the renderer clamps rgb
+// to [0, 1] first, so a rendered frame never reaches that range.
 __global__ void frame_u8_kernel(const float* __restrict__ rgb, int rgb_stride, const float* __restrict__ depth,
-                                int depth_stride, long long N, float d_lo, float d_hi,
+                                int depth_stride, long long N, float d_lo, float d_den,
                                 const unsigned char* __restrict__ lut, unsigned char* __restrict__ rgb8,
                                 unsigned char* __restrict__ depth8) {
   for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < N;
@@ -329,7 +334,7 @@ __global__ void frame_u8_kernel(const float* __restrict__ rgb, int rgb_stride, c
     if (depth8) {
       float d = depth[(long long)depth_stride * r];
       if (d != d) d = 0.0f;                                                     // np.nan_to_num
-      float x = __fdiv_rn(__fsub_rn(d, d_lo), __fadd_rn(__fsub_rn(d_hi, d_lo), 1e-8f));
+      float x = __fdiv_rn(__fsub_rn(d, d_lo), d_den);
       x = fminf(fmaxf(x, 0.0f), 1.0f);
       const int idx = (int)__fmul_rn(255.0f, x);                                // astype(uint8) truncates
       depth8[3 * r] = lut[3 * idx]; depth8[3 * r + 1] = lut[3 * idx + 1]; depth8[3 * r + 2] = lut[3 * idx + 2];
@@ -338,13 +343,13 @@ __global__ void frame_u8_kernel(const float* __restrict__ rgb, int rgb_stride, c
 }
 
 cudaError_t launch_frame_u8(const float* rgb, int rgb_stride, const float* depth, int depth_stride, long long N,
-                            float d_lo, float d_hi, const unsigned char* lut, unsigned char* rgb8,
+                            double d_lo, double d_hi, const unsigned char* lut, unsigned char* rgb8,
                             unsigned char* depth8, int n_sms, cudaStream_t stream) {
   if (N == 0) return cudaSuccess;
   long long b = (N + 255) / 256;
   if (b > (long long)n_sms * 16) b = (long long)n_sms * 16;
-  frame_u8_kernel<<<(unsigned)b, 256, 0, stream>>>(rgb, rgb_stride, depth, depth_stride, N, d_lo, d_hi, lut, rgb8,
-                                                  depth8);
+  frame_u8_kernel<<<(unsigned)b, 256, 0, stream>>>(rgb, rgb_stride, depth, depth_stride, N, (float)d_lo,
+                                                  (float)(d_hi - d_lo + 1e-8), lut, rgb8, depth8);
   return cudaGetLastError();
 }
 

@@ -26,7 +26,7 @@ def test_header_symbols_exported():
 
 def test_version_and_prepared_size():
     L = _lib.lib()
-    assert L.lrf_version() == _lib.ABI_VERSION
+    assert L.lrf_version() == _lib.ABI_VERSION == 4
     # bf16 hi+lo images of W1B [128][80] and W2 [128][128], then fp32 b1, b2, W3[3][132], b3[4]
     assert L.lrf_prepared_bytes() == 2 * 2 * (128 * 80 + 128 * 128) + 4 * (128 + 128 + 3 * 132 + 4)
 

@@ -6,6 +6,8 @@ import numpy as np
 import pytest
 import torch
 
+import metrics_oracle as orc
+
 pytestmark = pytest.mark.gpu
 
 
@@ -29,15 +31,38 @@ def test_pipeline_frames_match_direct_calls_and_host_conversions():
         rgb, depth = rgb.cpu().numpy().reshape(H, W, 3), depth.cpu().numpy().reshape(H, W)
         np.testing.assert_array_equal(fr["rgb"], rgb)                     # zero-copy float outputs, bit-exact
         np.testing.assert_array_equal(fr["depth"], depth)
-        want_rgb8 = np.clip(np.rint(255.0 * rgb[..., ::-1].astype(np.float32)), 0, 255).astype(np.uint8)
-        np.testing.assert_array_equal(fr["rgb8"], want_rgb8)
-        x = (np.nan_to_num(depth) - 0.0) / (5.0 - 0.0 + 1e-8)
+        np.testing.assert_array_equal(fr["rgb8"], orc.rgb8(rgb))
+        x = (np.nan_to_num(depth) - 0) / (5 - 0 + 1e-8)                  # visualize_depth(depth, [0, 5])
         idx = (255 * np.clip(x, 0, 1)).astype(np.uint8)
-        want_d8 = cv2.applyColorMap(idx, cv2.COLORMAP_JET)
-        mism = (fr["depth8"] != want_d8).any(-1)
-        # numpy evaluates (d - lo) / (hi - lo + 1e-8) in float64 (python scalars), the kernel in fp32: an index
-        # may differ by one where 255 * x sits on an integer to rounding
-        assert mism.mean() < 2e-3, float(mism.mean())
+        np.testing.assert_array_equal(fr["depth8"], cv2.applyColorMap(idx, cv2.COLORMAP_JET))
+
+
+def test_pipeline_depth_ranges_other_than_0_5():
+    """Depth ranges other than renderer.py's (0, 5), with a colour map that names its index: every pixel picks
+    the index visualize_depth picks.  (0.3, 2.9) lies below this scene's depths, so every pixel saturates; the
+    second range is the frames' 5th to 95th depth percentile, rounded to Python numbers, and spans most indices."""
+    import bench
+    import localrf_b200 as L
+    wl = bench.Workload("cfg5", 48)
+    lt = wl.build(L.LocalTensorfs, quiet=True).to("cuda")
+    W, H = 96, 80
+    lut = np.stack([np.arange(256), np.arange(256)[::-1], np.full(256, 7)], -1).astype(np.uint8)
+    frames = [torch.tensor([f], device="cuda") for f in (0, 6, 30, 63)]
+
+    def run(lo, hi):
+        pipe = L.FramePipeline(lt, W, H, depth_minmax=(lo, hi), n_buffers=2, lut=lut, keep_float=True)
+        got = [{k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in fr.items()}
+               for fr in pipe.render(frames, floater_thresh=0.5)]
+        for fr in got:
+            np.testing.assert_array_equal(fr["depth8"], orc.depth8(fr["depth"], lo, hi, lut))
+            np.testing.assert_array_equal(fr["rgb8"], orc.rgb8(fr["rgb"]))
+        return got, np.concatenate([fr["depth8"][..., 0].ravel() for fr in got])
+
+    got, _ = run(0.3, 2.9)
+    d = np.concatenate([fr["depth"].ravel() for fr in got])
+    lo, hi = (round(float(v), 2) for v in np.percentile(d[np.isfinite(d)], [5, 95]))
+    _, idx = run(lo, hi)
+    assert lo < hi and len(np.unique(idx)) > 64, (lo, hi, len(np.unique(idx)))
 
 
 def test_pipeline_refuses_overflow_and_cpu_model():

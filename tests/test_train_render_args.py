@@ -21,7 +21,7 @@ def test_exports_and_struct_mirror():
     for name in ("lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch"):
         assert hasattr(L, name) and name in _lib.EXPORTS
     assert L.lrf_sizeof(7) == C.sizeof(_lib.LrfCameraGrads) == 4 * 8
-    assert L.lrf_version() == _lib.ABI_VERSION == 3
+    assert L.lrf_version() == _lib.ABI_VERSION == 4
 
 
 def test_scratch_bytes():
