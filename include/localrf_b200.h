@@ -154,7 +154,7 @@ int lrf_version(void);
 const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
  * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor, 7 LrfCameraGrads, 8 LrfFrameStore,
- * 9 LrfRayGather (0 for any other index).  Bindings compare these with their own mirrors at load
+ * 9 LrfRayGather, 10 LrfPanelFrame (0 for any other index).  Bindings compare these with their own mirrors at load
  * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
@@ -479,6 +479,53 @@ typedef struct LrfRayGather {
  * >= n_px, gets NaN in every output row (its idx is still written); no other frame's data is read.  The ids are
  * never read on the host.  No atomics, no host synchronisation. */
 int lrf_gather_rays(const LrfFrameStore *store, const LrfRayGather *g, lrf_stream_t stream);
+
+/* Flow and depth comparison panels of one held-out frame.  replaces: renderer.py:79-124, the TensorBoard panels
+ * render(test=True) builds for every test frame (get_fwd_bwd_cam2cams / get_pred_flow / compute_depth_loss of
+ * utils/utils.py:15-59 and the inline numpy / cv2 lines around them).  The frame is rendered at W x H with
+ * rays_ids = arange(W H), so pixel p is (column p % W, row p / W).  The ground truth is h0 x w0 and is resized with
+ * OpenCV's INTER_NEAREST rule (flow values are not rescaled, as in the reference).  Pointers are device or pinned
+ * host memory, fp32 unless stated. */
+typedef struct LrfPanelFrame {
+  int32_t W, H;                /* render size */
+  int32_t h0, w0;              /* ground-truth size */
+  int64_t n_cams;              /* rows of cam2world = get_cam2world() (every frame, from 0) */
+  int64_t idx;                 /* the frame's camera, 0 <= idx < n_cams */
+  const float *depth;          /* [H W] rendered depth */
+  const float *directions;     /* [H W][3] camera-space ray directions (flow) */
+  const float *cam2world;      /* [n_cams][3][4] (flow) */
+  const float *intrinsics;     /* [3] focal(W), center(W, H) (flow) */
+  const float *fwd_flow;       /* [h0][w0][2] \                                          */
+  const float *fwd_mask;       /* [h0][w0]     | the flow group: all four, or all NULL  */
+  const float *bwd_flow;       /* [h0][w0][2]  | (no flow panels)                       */
+  const float *bwd_mask;       /* [h0][w0]    /                                          */
+  const float *invdepth;       /* [h0][w0], or NULL (no depth panel) */
+  float *fwd_panel;            /* [3H][2W] (flow) */
+  float *bwd_panel;            /* [3H][2W] (flow) */
+  float *depth_panel;          /* [3H][W] (depth) */
+  float *fwd_pred, *bwd_pred;  /* optional [H][W][2]: the predicted flows before scaling (flow) */
+  float *stats;                /* optional [8]: the 0.9 quantiles of fwd channel 0, 1 and bwd channel 0, 1, then
+                                  median and mean absolute deviation of x, then of g (NaN for a branch that is off) */
+} LrfPanelFrame;
+
+/* Device scratch bytes of one frame (8-byte aligned); 0 if W H is out of range. */
+size_t lrf_test_panels_scratch_bytes(int32_t W, int32_t H);
+/* Flow panel (per direction, cam2cam from camera idx to camera clamp(idx +- 1), the forward mask is kept also for
+ * the last camera): pred = pts2px(Rcc (directions * depth) + tcc) - (column, row); gt = the resized flow; per
+ * channel c, rows [0, H) = pred_c / q_c, rows [H, 2H) = gt_c / q_c with q_c = np.quantile([pred_c; gt_c], 0.9)
+ * (numpy 2.x's float32 arithmetic, bit for bit), rows [2H, 3H) = |pred_c - gt_c| * mask / W; channel c fills
+ * columns [c W, c W + W).  Depth panel: x = 1 / max(depth, 1e-6), g = the resized invdepth, each normalised as
+ * (v - t) / s with t its lower median (torch.median) and s the mean of |v - t| (fp64, fixed order, rounded once);
+ * rows 0.5 xn, 0.5 gn, (xn - gn)^2.  Every value is clamped to [0, 1] with NaN and -0 passed through.  One exception
+ * to "bit for bit": numpy and torch select by comparison, where -0 == +0, so the sign of a zero quantile or median
+ * depends on where the zeros lie in their input; this kernel orders -0 before +0.  A zero quantile then turns rows of
+ * nonzero values into infinities of the other sign, which clamp to the other bound.  A quantile <= 0
+ * gives inf or NaN rows and a NaN in an array gives a NaN statistic, as in the reference.  With neither group given
+ * nothing is launched.  LRF_ERR_INVALID before any device work for W or H < 1, 2 W H >= 2^31, h0 or w0 < 1, n_cams
+ * < 1, idx outside [0, n_cams), a NULL depth, a flow group partly given, a NULL input or panel of a branch that is
+ * on, and scratch that is NULL, not 8-byte aligned or too small.  No atomics on floats, no host synchronisation:
+ * bitwise repeatable. */
+int lrf_test_panels(const LrfPanelFrame *frame, void *scratch, size_t scratch_bytes, lrf_stream_t stream);
 
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */

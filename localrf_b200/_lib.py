@@ -11,8 +11,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
-           "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_abi.cu"]
-HEADERS = ["lrf_common.cuh", "lrf_device.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
+           "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_panels.cu", "lrf_abi.cu"]
+HEADERS = ["lrf_common.cuh", "lrf_device.cuh", "lrf_reproject.cuh", "lrf_select.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
@@ -77,6 +77,15 @@ class LrfRayGather(C.Structure):
                 ("bwd_mask", _vp)]
 
 
+class LrfPanelFrame(C.Structure):
+    _fields_ = [("W", C.c_int32), ("H", C.c_int32), ("h0", C.c_int32), ("w0", C.c_int32),
+                ("n_cams", C.c_int64), ("idx", C.c_int64),
+                ("depth", _vp), ("directions", _vp), ("cam2world", _vp), ("intrinsics", _vp),
+                ("fwd_flow", _vp), ("fwd_mask", _vp), ("bwd_flow", _vp), ("bwd_mask", _vp), ("invdepth", _vp),
+                ("fwd_panel", _vp), ("bwd_panel", _vp), ("depth_panel", _vp), ("fwd_pred", _vp), ("bwd_pred", _vp),
+                ("stats", _vp)]
+
+
 class LrfBatch(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int64),
@@ -123,7 +132,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_tv_sums_backward", "lrf_sample_ray", "lrf_frame_to_u8", "lrf_pack_bf16",
            "lrf_image_metrics_scratch_bytes", "lrf_image_metrics", "lrf_supervision_scratch_bytes",
            "lrf_supervision_losses", "lrf_supervision_losses_backward", "lrf_adam_step",
-           "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch", "lrf_gather_rays"]
+           "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch", "lrf_gather_rays",
+           "lrf_test_panels_scratch_bytes", "lrf_test_panels"]
 
 
 def _stale():
@@ -177,7 +187,7 @@ def lib():
     L.lrf_sizeof.restype = C.c_size_t
     L.lrf_sizeof.argtypes = [C.c_int32]
     for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
-                                     LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather)):
+                                     LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather, LrfPanelFrame)):
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -229,6 +239,9 @@ def lib():
                                                   C.c_size_t, _vp]
     L.lrf_adam_step.argtypes = [_vp, C.c_int64, _vp]        # LrfAdamTensor array: a ctypes array or packed bytes
     L.lrf_gather_rays.argtypes = [C.POINTER(LrfFrameStore), C.POINTER(LrfRayGather), _vp]
+    L.lrf_test_panels_scratch_bytes.restype = C.c_size_t
+    L.lrf_test_panels_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
+    L.lrf_test_panels.argtypes = [C.POINTER(LrfPanelFrame), _vp, C.c_size_t, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

@@ -56,6 +56,8 @@ cudaError_t launch_supervision_losses_backward(const LrfLossBatch& b, const floa
                                                void* scratch, cudaStream_t stream);
 cudaError_t launch_adam_step(const LrfAdamTensor* t, long long n, cudaStream_t stream);
 cudaError_t launch_gather_rays(const LrfFrameStore& s, const LrfRayGather& g, cudaStream_t stream);
+size_t panels_scratch_bytes(long long n_px);
+cudaError_t launch_test_panels(const LrfPanelFrame& f, void* scratch, int n_sms, cudaStream_t stream);
 cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
                                 cudaStream_t stream);
 cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
@@ -215,6 +217,7 @@ size_t lrf_sizeof(int32_t which) {
     case 7: return sizeof(LrfCameraGrads);
     case 8: return sizeof(LrfFrameStore);
     case 9: return sizeof(LrfRayGather);
+    case 10: return sizeof(LrfPanelFrame);
     default: return 0;
   }
 }
@@ -773,6 +776,40 @@ int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t 
     return fail(LRF_ERR_INVALID, "the flow outputs must be set exactly when the store has the flow group");
   cudaError_t e = lrf::launch_gather_rays(*s, *g, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e, "gather_rays_kernel");
+  return LRF_OK;
+}
+
+static bool panel_size_ok(int32_t W, int32_t H) {
+  return W >= 1 && H >= 1 && 2 * (int64_t)W * H <= 2147483647LL;
+}
+
+size_t lrf_test_panels_scratch_bytes(int32_t W, int32_t H) {
+  return panel_size_ok(W, H) ? lrf::panels_scratch_bytes((long long)W * H) : 0;
+}
+
+int lrf_test_panels(const LrfPanelFrame* f, void* scratch, size_t scratch_bytes, lrf_stream_t stream) {
+  if (!f) return fail(LRF_ERR_INVALID, "frame is NULL");
+  if (!panel_size_ok(f->W, f->H)) return fail(LRF_ERR_INVALID, "W and H must be >= 1 with 2 W H < 2^31");
+  if (f->h0 < 1 || f->w0 < 1) return fail(LRF_ERR_INVALID, "h0 and w0 must be >= 1");
+  if (f->n_cams < 1) return fail(LRF_ERR_INVALID, "n_cams must be >= 1");
+  if (f->idx < 0 || f->idx >= f->n_cams) return fail(LRF_ERR_INVALID, "idx must lie in [0, n_cams)");
+  if (!f->depth) return fail(LRF_ERR_INVALID, "depth is NULL");
+  const int n_flow = !!f->fwd_flow + !!f->fwd_mask + !!f->bwd_flow + !!f->bwd_mask;
+  if (n_flow != 0 && n_flow != 4)
+    return fail(LRF_ERR_INVALID, "the flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, bwd_mask "
+                                 "or none");
+  if (n_flow && (!f->directions || !f->cam2world || !f->intrinsics))
+    return fail(LRF_ERR_INVALID, "the flow panels need directions, cam2world and intrinsics");
+  if (n_flow && (!f->fwd_panel || !f->bwd_panel)) return fail(LRF_ERR_INVALID, "fwd_panel / bwd_panel is NULL");
+  if (f->invdepth && !f->depth_panel) return fail(LRF_ERR_INVALID, "depth_panel is NULL");
+  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
+  if (scratch_bytes < lrf_test_panels_scratch_bytes(f->W, f->H))
+    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_test_panels_scratch_bytes(W, H)");
+  DevInfo d;
+  int rc = device_info(d);
+  if (rc != LRF_OK) return rc;
+  cudaError_t e = lrf::launch_test_panels(*f, scratch, d.n_sms, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e, "test_panels");
   return LRF_OK;
 }
 

@@ -18,6 +18,9 @@
 #include <stdint.h>
 
 #include "../../include/localrf_b200.h"
+#include "lrf_reproject.cuh"
+#define LRF_SELECT_KEYS_ONLY
+#include "lrf_select.cuh"
 
 namespace lrf {
 
@@ -67,15 +70,6 @@ static LossPtrs carve(void* scratch, long long N, long long V) {
 }
 
 // ---- device helpers -------------------------------------------------------------------------------------
-// order-preserving; every NaN becomes the canonical +NaN first, so that NaNs of either sign sort after +inf
-__device__ inline unsigned int f2key(float f) {
-  const unsigned int u = isnan(f) ? 0x7fffffffu : __float_as_uint(f);
-  return u ^ ((u >> 31) ? 0xffffffffu : 0x80000000u);
-}
-__device__ inline float key2f(unsigned long long k) {
-  const unsigned int u = (unsigned int)(k >> 32);
-  return __uint_as_float(u ^ ((u >> 31) ? 0x80000000u : 0xffffffffu));
-}
 __device__ inline int key2idx(unsigned long long k) { return (int)(k & 0xffffffffu); }
 
 // ascending bitonic sort of P (a power of two) keys; every thread of the CTA calls it
@@ -142,7 +136,6 @@ __device__ inline double block_sum_all(double v, double* red) {
   return red[0];
 }
 
-__device__ inline float clamp_min(float x, float lo) { return x < lo ? lo : x; }   // NaN passes, as ATen's clamp
 __device__ inline float sgn(float x) { return (float)((x > 0.f) - (x < 0.f)); }
 
 // one view's two cam2cam transforms (index 0: k = rel - 1, the backward flow; 1: k = rel + 1, the forward flow)
@@ -165,32 +158,8 @@ __device__ void view_cams(const LrfLossBatch& b, int v, ViewCams& vc) {
       for (int i = 0; i < 12; ++i) vc.m[o][i] = __int_as_float(0x7fffffff);
       continue;
     }
-    const float* K = b.cam2world + 12 * k;          // [3][4]: R = [:, :3], t = [:, 3]
-    const float* Rl = b.cam2world + 12 * rel;
-    for (int i = 0; i < 3; ++i) {
-      for (int j = 0; j < 3; ++j)
-        vc.m[o][3 * i + j] = K[0 * 4 + i] * Rl[0 * 4 + j] + K[1 * 4 + i] * Rl[1 * 4 + j] + K[2 * 4 + i] * Rl[2 * 4 + j];
-      const float a = K[0 * 4 + i] * Rl[3] + K[1 * 4 + i] * Rl[7] + K[2 * 4 + i] * Rl[11];
-      const float c = K[0 * 4 + i] * K[3] + K[1 * 4 + i] * K[7] + K[2 * 4 + i] * K[11];
-      vc.m[o][9 + i] = a + (-c);
-    }
+    cam2cam(b.cam2world, rel, k, vc.m[o]);
   }
-}
-
-// the reprojection of one camera-space point through one cam2cam, minus the ray's pixel (get_pred_flow, pts2px)
-struct Proj {
-  float q[3], z, u, v;
-  int zpass;
-};
-__device__ inline Proj project(const float* m, const float p[3], float f, float cx, float cy, float i, float j) {
-  Proj r;
-  for (int a = 0; a < 3; ++a) r.q[a] = m[3 * a] * p[0] + m[3 * a + 1] * p[1] + m[3 * a + 2] * p[2] + m[9 + a];
-  const float nz = -r.q[2];
-  r.zpass = nz >= 1e-6f;
-  r.z = clamp_min(nz, 1e-6f);
-  r.u = r.q[0] / r.z * f + cx - 0.5f - i;
-  r.v = -r.q[1] / r.z * f + cy - 0.5f - j;
-  return r;
 }
 
 // ---- forward ----------------------------------------------------------------------------------------------

@@ -6,10 +6,14 @@ arithmetic: fp32 squares and cross products, an fp64 separable Gaussian filter a
 
     image_metrics(img, gt)          -> float64 device tensor [mse, ssim], no host synchronisation
     rgb_ssim(img0, img1, max_val)   -> the reference's function (numpy in, float / numpy map out), on the GPU
+    test_panels(depth, directions, ...) -> the flow and depth comparison panels of renderer.py:79-124
+                                       (lrf_test_panels), device tensors, no host synchronisation
 
 `renderer.rgb_ssim = localrf_b200.metrics.rgb_ssim` puts it into the reference's renderer.  There is no CPU
 fallback: without a CUDA device these raise RuntimeError.
 """
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -112,3 +116,154 @@ def rgb_ssim(img0, img1, max_val, filter_size=11, filter_sigma=1.5, k1=0.01, k2=
     if on_device:
         return ssim_map if return_map else out[1]
     return ssim_map.cpu().numpy() if return_map else float(out[1])
+
+
+def _readable(t, dev, name):
+    """t as a contiguous float32 tensor the kernel can read on `dev`: a CUDA tensor on `dev`, or a pinned host tensor.
+    Anything else raises ValueError: the kernel would dereference a pageable host or another device's pointer."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a tensor, got {type(t).__name__}")
+    if t.is_cuda:
+        if t.device != dev:
+            raise ValueError(f"{name} is on {t.device} but the frame is on {dev}")
+        return t.detach().to(torch.float32).contiguous()
+    if not t.is_pinned():
+        raise ValueError(f"{name} must be a CUDA tensor on {dev} or a pinned host tensor")
+    if t.dtype != torch.float32 or not t.is_contiguous():
+        t = t.detach().to(torch.float32).contiguous().pin_memory()
+    return t
+
+
+def _gt_map(a, dev, name, shape, stage=None):
+    """A ground-truth array of the test dataset as a contiguous float32 tensor the kernel can read: CUDA tensors on
+    `dev` and pinned tensors as they are (CUDA tensors on another device raise ValueError); numpy arrays and pageable
+    tensors copied to `dev` (as rgb_ssim stages its inputs), or handed to `stage(name, array)`, which returns a pinned
+    copy (FramePipeline: a host copy into the frame slot's buffer, which does not wait for the device)."""
+    if a is None:
+        return None
+    if isinstance(a, torch.Tensor) and (a.is_cuda or a.is_pinned()):
+        if a.dtype != torch.float32:
+            raise TypeError(f"{name} must be float32, got {a.dtype}")
+        a = _readable(a, dev, name)
+    else:
+        x = a.detach().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+        if x.dtype != np.float32:
+            raise TypeError(f"{name} must be float32, got {x.dtype}")
+        if shape is not None and tuple(x.shape) != shape:
+            raise ValueError(f"{name} is {tuple(x.shape)}, expected {shape}")
+        a = stage(name, x) if stage is not None else torch.from_numpy(np.ascontiguousarray(x)).to(dev)
+    if shape is not None and tuple(a.shape) != shape:
+        raise ValueError(f"{name} is {tuple(a.shape)}, expected {shape}")
+    return a
+
+
+def _intrinsics(focal, center, dev):
+    """[focal, cx, cy] as a float32 device tensor, built on the device from tensors (no synchronisation)."""
+    parts = [torch.as_tensor(v, dtype=torch.float32).reshape(-1).to(dev) for v in (focal, center)]
+    intr = torch.cat(parts)
+    if intr.numel() != 3:
+        raise ValueError("focal must hold 1 value and center 2")
+    return intr
+
+
+def _enqueue_panels(depth, directions, cam2world, idx, intrinsics, W, H, gts, outs, dev):
+    """Enqueues lrf_test_panels on the current stream of `dev`.  gts: (fwd_flow, fwd_mask, bwd_flow, bwd_mask,
+    invdepth) staged by _gt_map; outs: dict of fwd_panel / bwd_panel / depth_panel / fwd_pred / bwd_pred / stats
+    (device or pinned).  Returns the scratch tensor, which must stay alive until the work has run."""
+    fwd_flow, fwd_mask, bwd_flow, bwd_mask, invdepth = gts
+    first = next(g for g in gts if g is not None)
+    h0, w0 = int(first.shape[0]), int(first.shape[1])
+    f = _lib.LrfPanelFrame()
+    f.W, f.H, f.h0, f.w0 = int(W), int(H), h0, w0
+    f.n_cams = int(cam2world.shape[0]) if cam2world is not None else int(idx) + 1   # depth only: no camera read
+    f.idx = int(idx)
+    for name, t in (("depth", depth), ("directions", directions), ("cam2world", cam2world),
+                    ("intrinsics", intrinsics), ("fwd_flow", fwd_flow), ("fwd_mask", fwd_mask),
+                    ("bwd_flow", bwd_flow), ("bwd_mask", bwd_mask), ("invdepth", invdepth)):
+        setattr(f, name, _ptr(t).value if t is not None else None)
+    for name in ("fwd_panel", "bwd_panel", "depth_panel", "fwd_pred", "bwd_pred", "stats"):
+        t = outs.get(name)
+        setattr(f, name, _ptr(t).value if t is not None else None)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        nbytes = int(L.lrf_test_panels_scratch_bytes(f.W, f.H))
+        if nbytes == 0:
+            raise ValueError(f"W x H = {W} x {H} is out of range for lrf_test_panels")
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _lib.check(L.lrf_test_panels(C.byref(f), _ptr(scratch), nbytes, _stream(dev)))
+    return scratch
+
+
+def _panel_inputs(depth, directions, cam2world, W, H, fwd_flow, fwd_mask, bwd_flow, bwd_mask, invdepth, stage=None,
+                  dev=None):
+    """Checks and stages the inputs of test_panels -> (dev, depth, directions, cam2world, gts).  The frame's device is
+    depth's; depth may be pinned only when `dev` names the device.  directions and cam2world must be on that device
+    or pinned."""
+    if not isinstance(depth, torch.Tensor) or depth.dtype != torch.float32 or depth.numel() != W * H:
+        raise ValueError(f"depth must be a float32 tensor of W x H = {W * H} values")
+    if depth.is_cuda:
+        dev = depth.device
+    elif dev is None or not depth.is_pinned():
+        raise ValueError("depth must be a CUDA tensor (the frame's device)")
+    depth = _readable(depth, dev, "depth")
+    flows = (fwd_flow, fwd_mask, bwd_flow, bwd_mask)
+    n_flow = sum(x is not None for x in flows)
+    if n_flow not in (0, 4):
+        raise ValueError("the flow panels need all of fwd_flow, fwd_mask, bwd_flow and bwd_mask (or none)")
+    if n_flow:
+        if directions is None or cam2world is None:
+            raise ValueError("the flow panels need directions and cam2world")
+        if not isinstance(directions, torch.Tensor) or directions.dtype != torch.float32 or \
+                directions.numel() != 3 * W * H:
+            raise ValueError("directions must be a float32 [W*H, 3] tensor")
+        directions = _readable(directions, dev, "directions").reshape(-1, 3)
+        cam2world = _readable(cam2world, dev, "cam2world")
+        if cam2world.numel() == 0 or cam2world.numel() % 12:
+            raise ValueError(f"cam2world must be [n_cams, 3, 4], got {tuple(cam2world.shape)}")
+        cam2world = cam2world.reshape(-1, 3, 4)
+    else:
+        directions = cam2world = None
+    first = next((np.shape(x) for x in flows + (invdepth,) if x is not None), None)
+    h0, w0 = (int(first[0]), int(first[1])) if first is not None and len(first) >= 2 else (0, 0)
+    gts = tuple(_gt_map(x, dev, name, shape, stage) for x, name, shape in (
+        (fwd_flow, "fwd_flow", (h0, w0, 2)), (fwd_mask, "fwd_mask", (h0, w0)), (bwd_flow, "bwd_flow", (h0, w0, 2)),
+        (bwd_mask, "bwd_mask", (h0, w0)), (invdepth, "invdepth", (h0, w0))))
+    return dev, depth.reshape(-1), directions, cam2world, gts
+
+
+@torch.no_grad()
+def test_panels(depth, directions, cam2world, idx, focal, center, W, H, fwd_flow=None, fwd_mask=None, bwd_flow=None,
+                bwd_mask=None, invdepth=None, return_arrays=False):
+    """The comparison panels renderer.render(test=True) builds for a held-out frame (renderer.py:79-124) ->
+    (fwd_flow_cmp [3H,2W] | None, bwd_flow_cmp [3H,2W] | None, depth_cmp [3H,W] | None): float32 tensors on
+    depth's CUDA device, clamped to [0, 1], enqueued without synchronising.  They are what render appends to
+    fwd_flow_cmp_tb, bwd_flow_cmp_tb and depth_cmp_tb.
+
+    depth [W*H] and directions [W*H,3] come from the forward of the frame (rays_ids = arange(W*H)); cam2world =
+    LocalTensorfs.get_cam2world() (every frame); idx is the frame's camera; focal = focal(W), center = center(W, H)
+    (tensors or numbers).  The ground truth is the test dataset's arrays of the frame at its own resolution h0 x w0:
+    fwd_flow / bwd_flow [h0,w0,2] and fwd_mask / bwd_mask [h0,w0] (all four, or none: no flow panels), invdepth
+    [h0,w0] (or None: no depth panel); float32 numpy arrays (copied to the device) or CUDA / pinned tensors.
+    return_arrays=True adds a dict with the unscaled predicted flows fwd_pred / bwd_pred [H,W,2] and `stats`
+    [8]: the four 0.9 quantiles (fwd c0, c1, bwd c0, c1), then median and mean absolute deviation of x and of g."""
+    W, H = int(W), int(H)
+    dev, depth, directions, cam2world, gts = _panel_inputs(depth, directions, cam2world, W, H, fwd_flow, fwd_mask,
+                                                          bwd_flow, bwd_mask, invdepth)
+    flow, dep = gts[0] is not None, gts[4] is not None
+    new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
+    outs = {}
+    if flow:
+        outs.update(fwd_panel=new(3 * H, 2 * W), bwd_panel=new(3 * H, 2 * W))
+    if dep:
+        outs["depth_panel"] = new(3 * H, W)
+    if return_arrays:
+        outs["stats"] = new(8)
+        if flow:
+            outs.update(fwd_pred=new(H, W, 2), bwd_pred=new(H, W, 2))
+    if flow or dep:
+        intr = _intrinsics(focal, center, dev) if flow else None
+        _enqueue_panels(depth, directions, cam2world, idx, intr, W, H, gts, outs, dev)
+    panels = (outs.get("fwd_panel"), outs.get("bwd_panel"), outs.get("depth_panel"))
+    if return_arrays:
+        return panels + ({k: outs.get(k) for k in ("fwd_pred", "bwd_pred", "stats")},)
+    return panels
