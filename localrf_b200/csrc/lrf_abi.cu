@@ -1,6 +1,7 @@
 // lrf_abi.cu -- the C ABI declared in include/localrf_b200.h (validation + launches).
 #include <cuda_runtime.h>
 
+#include <climits>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
@@ -97,6 +98,9 @@ int cuda_fail(cudaError_t e, const char* where) {
   snprintf(g_err, sizeof(g_err), "%s: %s", where, cudaGetErrorString(e));
   return LRF_ERR_CUDA;
 }
+
+// the status an entry point returns for the launch it ends with
+int cuda_status(cudaError_t e, const char* where) { return e == cudaSuccess ? LRF_OK : cuda_fail(e, where); }
 
 struct DevInfo {
   int n_sms = 0;
@@ -199,6 +203,49 @@ int make_field(const LrfField* f, bool need_mlp, bool need_table, const void* pr
   return LRF_OK;
 }
 
+// validates a batch of n_rays >= 1 -- its split into views when `per_view`, n_rays <= max_rays, and in ray-generation
+// mode (rays == NULL) its camera -- and fills the batch fields the render and its backward both read
+int make_batch(const LrfBatch* b, bool per_view, long long max_rays, lrf::BatchDev& B) {
+  memset(&B, 0, sizeof(B));
+  if (per_view) {
+    if (b->n_rays < 1 || b->n_views < 1 || b->n_rays % b->n_views != 0)
+      return fail(LRF_ERR_INVALID, "n_rays must be a positive multiple of n_views");
+    B.rays_per_view = b->n_rays / b->n_views;
+  }
+  if (b->n_rays > max_rays) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  if (!b->rays) {
+    if (!b->ray_ids || !b->cam2world) return fail(LRF_ERR_INVALID, "ray_ids/cam2world is NULL");
+    if (b->W < 1 || b->H < 1) return fail(LRF_ERR_INVALID, "W/H must be positive");
+    if (!b->fov360 && !b->intrinsics && !(b->focal != 0.0f))
+      return fail(LRF_ERR_INVALID, "focal must be non-zero");
+  }
+  B.n_rays = b->n_rays;
+  B.rays = b->rays;
+  B.ray_ids = reinterpret_cast<const long long*>(b->ray_ids);
+  B.W = b->W; B.H = b->H; B.fov360 = b->fov360;
+  B.focal = b->focal; B.cx = b->cx; B.cy = b->cy;
+  B.intrinsics = b->intrinsics;
+  B.c2w = b->cam2world;
+  B.w2rf = b->world2rf;
+  B.exposure = b->exposure;
+  B.white_bg = b->white_bg;
+  return LRF_OK;
+}
+
+// the field's gradient buffers of lrf_render_backward (d_rays too) and lrf_render_backward_batch
+int check_field_grads(const LrfGradients* g, bool need_d_rays) {
+  if ((need_d_rays && !g->d_rays) || !g->d_w1b || !g->d_b1 || !g->d_w2 || !g->d_b2 || !g->d_w3 || !g->d_b3)
+    return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
+  for (int i = 0; i < 3; ++i) {
+    if (!g->d_dplane[i] || !g->d_dline[i] || !g->d_aplane[i] || !g->d_aline[i])
+      return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
+    if (((uintptr_t)g->d_dplane[i] | (uintptr_t)g->d_dline[i] | (uintptr_t)g->d_aplane[i] |
+         (uintptr_t)g->d_aline[i]) & 15)
+      return fail(LRF_ERR_INVALID, "plane/line gradient buffers must be 16-byte aligned");
+  }
+  return LRF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -243,15 +290,13 @@ int lrf_field_prepare(const LrfField* f, void* prepared, lrf_stream_t stream) {
     return fail(LRF_ERR_INVALID, "MLP / basis pointer is NULL");
   if (f->fea_pe != 0 || f->view_pe != 0) {
     if ((uintptr_t)prepared & 1023) return fail(LRF_ERR_INVALID, "the prepared block of a field with positional encodings must be 1024-byte aligned");
-    cudaError_t e = lrf::launch_prepare_pe(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3, f->fea_pe, f->view_pe,
-                                           static_cast<unsigned char*>(prepared), (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "prepare_pe_kernel");
-    return LRF_OK;
+    return cuda_status(lrf::launch_prepare_pe(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3, f->fea_pe, f->view_pe,
+                                              static_cast<unsigned char*>(prepared),
+                                              (cudaStream_t)stream), "prepare_pe_kernel");
   }
-  cudaError_t e = lrf::launch_prepare(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3,
-                                      static_cast<unsigned char*>(prepared), (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "prepare_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_prepare(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3,
+                                         static_cast<unsigned char*>(prepared),
+                                         (cudaStream_t)stream), "prepare_kernel");
 }
 
 int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const LrfOutputs* o,
@@ -271,40 +316,18 @@ int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const
     if (o->signal_seq && o->n_peers >= 1 && o->rank >= 0 && o->rank < o->n_peers) {
       for (int p = 0; p < o->n_peers; ++p)
         if (!o->peer_flags[p]) return fail(LRF_ERR_INVALID, "peer_flags pointer is NULL");
-      cudaError_t e = lrf::launch_peer_barrier(o->peer_flags, o->rank, o->n_peers, o->signal_seq, 0ull,
-                                               (cudaStream_t)stream);
-      if (e != cudaSuccess) return cuda_fail(e, "peer_barrier_kernel");
+      return cuda_status(lrf::launch_peer_barrier(o->peer_flags, o->rank, o->n_peers, o->signal_seq, 0ull,
+                                                  (cudaStream_t)stream), "peer_barrier_kernel");
     }
     return LRF_OK;
   }
   if (!o->pix && (!o->rgb || !o->depth)) return fail(LRF_ERR_INVALID, "rgb/depth output is NULL");
   lrf::BatchDev B;
-  memset(&B, 0, sizeof(B));
-  B.n_rays = b->n_rays;
-  B.rays = b->rays;
-  B.rays_per_view = 0;
-  const bool per_view = b->blend || b->exposure || !b->rays;
-  if (per_view) {
-    if (b->n_views < 1 || b->n_rays % b->n_views != 0)
-      return fail(LRF_ERR_INVALID, "n_rays must be a positive multiple of n_views");
-    B.rays_per_view = b->n_rays / b->n_views;
-  }
-  if (!b->rays) {
-    if (!b->ray_ids || !b->cam2world) return fail(LRF_ERR_INVALID, "ray_ids/cam2world is NULL");
-    if (b->W < 1 || b->H < 1) return fail(LRF_ERR_INVALID, "W/H must be positive");
-    if (!b->fov360 && !b->intrinsics && !(b->focal != 0.0f))
-      return fail(LRF_ERR_INVALID, "focal must be non-zero");
-  }
-  B.ray_ids = reinterpret_cast<const long long*>(b->ray_ids);
-  B.W = b->W; B.H = b->H; B.fov360 = b->fov360;
-  B.focal = b->focal; B.cx = b->cx; B.cy = b->cy;
-  B.intrinsics = b->intrinsics;
-  B.c2w = b->cam2world;
-  B.w2rf = b->world2rf;
+  rc = make_batch(b, b->blend || b->exposure || !b->rays, LLONG_MAX, B);
+  if (rc != LRF_OK) return rc;
   B.blend = b->blend;
   B.blend_stride = b->blend_stride;
-  B.exposure = b->exposure;
-  B.accumulate = b->accumulate; B.finalize = b->finalize; B.white_bg = b->white_bg;
+  B.accumulate = b->accumulate; B.finalize = b->finalize;
   B.floater_thresh = b->floater_thresh;
   B.refine = b->refine;
   if (o->pix) {
@@ -351,9 +374,7 @@ int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const
     return fail(LRF_ERR_UNSUPPORTED, "sample table too long for the shared-memory budget");
   B.sched = d.sched + 2 * d.next;                                   // [ray counter, finished-CTA counter]
   B.done_ctr = reinterpret_cast<unsigned int*>(d.sched + 2 * d.next + 1);
-  cudaError_t e = lrf::launch_render(F, B, d.n_sms, d.max_smem, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "render_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_render(F, B, d.n_sms, d.max_smem, (cudaStream_t)stream), "render_kernel");
 }
 
 int lrf_mlp_forward(const void* prepared, const float* feats, const float* viewdirs, int64_t M,
@@ -363,10 +384,8 @@ int lrf_mlp_forward(const void* prepared, const float* feats, const float* viewd
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_mlp(static_cast<const float*>(prepared), feats, viewdirs, M, rgb,
-                                  d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "mlp_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_mlp(static_cast<const float*>(prepared), feats, viewdirs, M, rgb,
+                                     d.n_sms, (cudaStream_t)stream), "mlp_kernel");
 }
 
 int lrf_density_feature(const LrfField* f, const float* xyz, int64_t M, float* out,
@@ -375,9 +394,7 @@ int lrf_density_feature(const LrfField* f, const float* xyz, int64_t M, float* o
   int rc = make_field(f, false, false, nullptr, F, false, /*allow_bf16=*/true);
   if (rc != LRF_OK) return rc;
   if (M < 0 || (M > 0 && (!xyz || !out))) return fail(LRF_ERR_INVALID, "bad xyz/out/M");
-  cudaError_t e = lrf::launch_density_feature(F, xyz, M, out, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "density_feature_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_density_feature(F, xyz, M, out, (cudaStream_t)stream), "density_feature_kernel");
 }
 
 int lrf_app_feature(const LrfField* f, const float* xyz, int64_t M, float* out,
@@ -388,9 +405,7 @@ int lrf_app_feature(const LrfField* f, const float* xyz, int64_t M, float* out,
   if (f->app_dim != lrf::APP_DIM) return fail(LRF_ERR_UNSUPPORTED, "only app_dim=27 is built");
   if (!f->basis) return fail(LRF_ERR_INVALID, "basis is NULL");
   if (M < 0 || (M > 0 && (!xyz || !out))) return fail(LRF_ERR_INVALID, "bad xyz/out/M");
-  cudaError_t e = lrf::launch_app_feature(F, f->basis, xyz, M, out, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "app_feature_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_app_feature(F, f->basis, xyz, M, out, (cudaStream_t)stream), "app_feature_kernel");
 }
 
 int lrf_app_products(const LrfField* f, const float* xyz, int64_t M, float* out,
@@ -399,9 +414,7 @@ int lrf_app_products(const LrfField* f, const float* xyz, int64_t M, float* out,
   int rc = make_field(f, false, false, nullptr, F);
   if (rc != LRF_OK) return rc;
   if (M < 0 || (M > 0 && (!xyz || !out))) return fail(LRF_ERR_INVALID, "bad xyz/out/M");
-  cudaError_t e = lrf::launch_app_products(F, xyz, M, out, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "app_products_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_app_products(F, xyz, M, out, (cudaStream_t)stream), "app_products_kernel");
 }
 
 static int check_grads(float* const d_plane[3], float* const d_line[3]) {
@@ -419,10 +432,8 @@ int lrf_density_feature_backward(const LrfField* f, const float* xyz, const floa
   if (rc != LRF_OK) return rc;
   if ((rc = check_grads(d_plane, d_line)) != LRF_OK) return rc;
   if (M < 0 || (M > 0 && (!xyz || !gout))) return fail(LRF_ERR_INVALID, "bad xyz/grad_out/M");
-  cudaError_t e = lrf::launch_density_backward(F, d_plane, d_line, xyz, gout, M, d_xyz,
-                                               (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "density_backward_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_density_backward(F, d_plane, d_line, xyz, gout, M, d_xyz,
+                                                  (cudaStream_t)stream), "density_backward_kernel");
 }
 
 int lrf_app_products_backward(const LrfField* f, const float* xyz, const float* gout, int64_t M,
@@ -433,10 +444,8 @@ int lrf_app_products_backward(const LrfField* f, const float* xyz, const float* 
   if (rc != LRF_OK) return rc;
   if ((rc = check_grads(d_plane, d_line)) != LRF_OK) return rc;
   if (M < 0 || (M > 0 && (!xyz || !gout))) return fail(LRF_ERR_INVALID, "bad xyz/grad_out/M");
-  cudaError_t e = lrf::launch_app_products_backward(F, d_plane, d_line, xyz, gout, M, d_xyz,
-                                                    (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "app_products_backward_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_app_products_backward(F, d_plane, d_line, xyz, gout, M, d_xyz,
+                                                       (cudaStream_t)stream), "app_products_backward_kernel");
 }
 
 size_t lrf_prepared_backward_bytes(void) { return lrf::backward_prepared_bytes(); }
@@ -455,10 +464,9 @@ int lrf_field_prepare_backward(const LrfField* f, void* prepared_bwd, lrf_stream
     return fail(LRF_ERR_UNSUPPORTED, "positional encodings (fea_pe/view_pe > 0) are not built yet");
   if (!f->basis || !f->w1 || !f->b1 || !f->w2 || !f->b2 || !f->w3 || !f->b3)
     return fail(LRF_ERR_INVALID, "MLP / basis pointer is NULL");
-  cudaError_t e = lrf::launch_prepare_backward(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3,
-                                               static_cast<float*>(prepared_bwd), (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "prepare_backward_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_prepare_backward(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3,
+                                                  static_cast<float*>(prepared_bwd),
+                                                  (cudaStream_t)stream), "prepare_backward_kernel");
 }
 
 int lrf_render_backward(const LrfField* f, const void* prepared_bwd, const float* rays,
@@ -473,26 +481,16 @@ int lrf_render_backward(const LrfField* f, const void* prepared_bwd, const float
   if (n_rays == 0) return LRF_OK;
   if (n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
   if (!rays || !grad_rgb || !grad_depth || !g) return fail(LRF_ERR_INVALID, "rays / grad_rgb / grad_depth / grads is NULL");
-  if (!g->d_rays || !g->d_w1b || !g->d_b1 || !g->d_w2 || !g->d_b2 || !g->d_w3 || !g->d_b3)
-    return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
-  for (int i = 0; i < 3; ++i) {
-    if (!g->d_dplane[i] || !g->d_dline[i] || !g->d_aplane[i] || !g->d_aline[i])
-      return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
-    if (((uintptr_t)g->d_dplane[i] | (uintptr_t)g->d_dline[i] | (uintptr_t)g->d_aplane[i] |
-         (uintptr_t)g->d_aline[i]) & 15)
-      return fail(LRF_ERR_INVALID, "plane/line gradient buffers must be 16-byte aligned");
-  }
+  if ((rc = check_field_grads(g, true)) != LRF_OK) return rc;
   if (!scratch || ((uintptr_t)scratch & 15)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 16-byte aligned");
   if (scratch_bytes < lrf::backward_scratch_bytes(n_rays, F.S))
     return fail(LRF_ERR_INVALID, "scratch is smaller than lrf_backward_scratch_bytes(n_rays, n_samples)");
   DevInfo d;
   rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_render_backward_abi(F, rays, n_rays, white_bg, grad_rgb, grad_depth,
-                                                  static_cast<const float*>(prepared_bwd), *g, scratch,
-                                                  d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "render_backward");
-  return LRF_OK;
+  return cuda_status(lrf::launch_render_backward_abi(F, rays, n_rays, white_bg, grad_rgb, grad_depth,
+                                                     static_cast<const float*>(prepared_bwd), *g, scratch,
+                                                     d.n_sms, (cudaStream_t)stream), "render_backward");
 }
 
 int lrf_exposure_clamp(const float* x, const float* exposure, int64_t n_rays, int64_t n_views, float* rgb,
@@ -503,9 +501,8 @@ int lrf_exposure_clamp(const float* x, const float* exposure, int64_t n_rays, in
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_exposure_clamp(x, exposure, n_rays, n_views, rgb, d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "exposure_clamp_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_exposure_clamp(x, exposure, n_rays, n_views, rgb, d.n_sms,
+                                                (cudaStream_t)stream), "exposure_clamp_kernel");
 }
 
 size_t lrf_backward_batch_scratch_bytes(int64_t n_rays, int32_t n_samples, int64_t n_views) {
@@ -525,45 +522,19 @@ int lrf_render_backward_batch(const LrfField* f, const void* prepared_bwd, const
   if (b->rays) return fail(LRF_ERR_INVALID, "the batch backward generates its rays: batch->rays must be NULL");
   if (b->accumulate) return fail(LRF_ERR_INVALID, "accumulate is not supported by the batch backward");
   if (b->blend) return fail(LRF_ERR_INVALID, "a blend pointer is not supported by the batch backward");
-  if (b->n_rays < 1 || b->n_views < 1 || b->n_rays % b->n_views != 0)
-    return fail(LRF_ERR_INVALID, "n_rays must be a positive multiple of n_views");
-  if (b->n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
-  if (!b->ray_ids || !b->cam2world) return fail(LRF_ERR_INVALID, "ray_ids/cam2world is NULL");
-  if (b->W < 1 || b->H < 1) return fail(LRF_ERR_INVALID, "W/H must be positive");
-  if (!b->fov360 && !b->intrinsics && !(b->focal != 0.0f)) return fail(LRF_ERR_INVALID, "focal must be non-zero");
+  lrf::BatchDev B;
+  if ((rc = make_batch(b, true, 2147483647LL, B)) != LRF_OK) return rc;
   if (!x || !grad_rgb || !grad_depth) return fail(LRF_ERR_INVALID, "rgb_linear / grad_rgb / grad_depth is NULL");
-  if (!g->d_w1b || !g->d_b1 || !g->d_w2 || !g->d_b2 || !g->d_w3 || !g->d_b3)
-    return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
-  for (int i = 0; i < 3; ++i) {
-    if (!g->d_dplane[i] || !g->d_dline[i] || !g->d_aplane[i] || !g->d_aline[i])
-      return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
-    if (((uintptr_t)g->d_dplane[i] | (uintptr_t)g->d_dline[i] | (uintptr_t)g->d_aplane[i] |
-         (uintptr_t)g->d_aline[i]) & 15)
-      return fail(LRF_ERR_INVALID, "plane/line gradient buffers must be 16-byte aligned");
-  }
+  if ((rc = check_field_grads(g, false)) != LRF_OK) return rc;
   if (!scratch || ((uintptr_t)scratch & 15)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 16-byte aligned");
   if (scratch_bytes < lrf::train_backward_scratch_bytes(b->n_rays, F.S, b->n_views))
     return fail(LRF_ERR_INVALID, "scratch is smaller than lrf_backward_batch_scratch_bytes(n_rays, n_samples, n_views)");
   if (b->floater_thresh > 0.0f) return fail(LRF_ERR_UNSUPPORTED, "the backward is built for floater_thresh = 0");
-  lrf::BatchDev B;
-  memset(&B, 0, sizeof(B));
-  B.n_rays = b->n_rays;
-  B.rays_per_view = b->n_rays / b->n_views;
-  B.ray_ids = reinterpret_cast<const long long*>(b->ray_ids);
-  B.W = b->W; B.H = b->H; B.fov360 = b->fov360;
-  B.focal = b->focal; B.cx = b->cx; B.cy = b->cy;
-  B.intrinsics = b->intrinsics;
-  B.c2w = b->cam2world;
-  B.w2rf = b->world2rf;
-  B.exposure = b->exposure;
-  B.white_bg = b->white_bg;
   DevInfo d;
   if ((rc = device_info(d)) != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_render_backward_batch(F, B, static_cast<const float*>(prepared_bwd), x, grad_rgb,
-                                                    grad_depth, grad_directions, *g, *cg, scratch, b->n_views,
-                                                    d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "render_backward_batch");
-  return LRF_OK;
+  return cuda_status(lrf::launch_render_backward_batch(F, B, static_cast<const float*>(prepared_bwd), x, grad_rgb,
+                                                       grad_depth, grad_directions, *g, *cg, scratch, b->n_views,
+                                                       d.n_sms, (cudaStream_t)stream), "render_backward_batch");
 }
 
 int lrf_alpha_mask_build(const LrfField* f, const int32_t dims[3], float length, float thres,
@@ -577,10 +548,8 @@ int lrf_alpha_mask_build(const LrfField* f, const int32_t dims[3], float length,
   DevInfo d;
   if ((rc = device_info(d)) != LRF_OK) return rc;
   const int dd[3] = {dims[0], dims[1], dims[2]};
-  cudaError_t e = lrf::launch_alpha_mask_build(F, f->aabb + 3, dd, length, thres, alpha_scratch, mask, kept,
-                                               d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "alpha_mask_build");
-  return LRF_OK;
+  return cuda_status(lrf::launch_alpha_mask_build(F, f->aabb + 3, dd, length, thres, alpha_scratch, mask, kept,
+                                                  d.n_sms, (cudaStream_t)stream), "alpha_mask_build");
 }
 
 int lrf_upsample(const float* src, int32_t H, int32_t W, float* dst, int32_t H2, int32_t W2, int32_t C,
@@ -591,9 +560,7 @@ int lrf_upsample(const float* src, int32_t H, int32_t W, float* dst, int32_t H2,
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_upsample(src, H, W, dst, H2, W2, C, d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "upsample_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_upsample(src, H, W, dst, H2, W2, C, d.n_sms, (cudaStream_t)stream), "upsample_kernel");
 }
 
 int lrf_density_l1(const LrfField* f, double* sum, lrf_stream_t stream) {
@@ -603,9 +570,7 @@ int lrf_density_l1(const LrfField* f, double* sum, lrf_stream_t stream) {
   if (!sum) return fail(LRF_ERR_INVALID, "sum is NULL");
   DevInfo d;
   if ((rc = device_info(d)) != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_density_l1(F, sum, d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "density_l1_fwd_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_density_l1(F, sum, d.n_sms, (cudaStream_t)stream), "density_l1_fwd_kernel");
 }
 
 int lrf_density_l1_backward(const LrfField* f, const float* grad_out, float* const d_plane[3],
@@ -614,12 +579,9 @@ int lrf_density_l1_backward(const LrfField* f, const float* grad_out, float* con
   int rc = make_field(f, false, false, nullptr, F);
   if (rc != LRF_OK) return rc;
   if (!grad_out) return fail(LRF_ERR_INVALID, "grad_out is NULL");
-  if (!d_plane || !d_line) return fail(LRF_ERR_INVALID, "gradient pointer arrays are NULL");
-  for (int i = 0; i < 3; ++i)
-    if (!d_plane[i] || !d_line[i]) return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
-  cudaError_t e = lrf::launch_density_l1_backward(F, grad_out, d_plane, d_line, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "density_l1_bwd_kernel");
-  return LRF_OK;
+  if ((rc = check_grads(d_plane, d_line)) != LRF_OK) return rc;
+  return cuda_status(lrf::launch_density_l1_backward(F, grad_out, d_plane, d_line,
+                                                     (cudaStream_t)stream), "density_l1_bwd_kernel");
 }
 
 int lrf_tv_sums(const float* x, int32_t H, int32_t W, int32_t C, double* sums, lrf_stream_t stream) {
@@ -627,9 +589,7 @@ int lrf_tv_sums(const float* x, int32_t H, int32_t W, int32_t C, double* sums, l
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_tv(x, H, W, C, sums, d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "tv_fwd_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_tv(x, H, W, C, sums, d.n_sms, (cudaStream_t)stream), "tv_fwd_kernel");
 }
 
 int lrf_tv_sums_backward(const float* x, int32_t H, int32_t W, int32_t C, const float* grad_out, float kh,
@@ -638,9 +598,8 @@ int lrf_tv_sums_backward(const float* x, int32_t H, int32_t W, int32_t C, const 
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_tv_backward(x, H, W, C, grad_out, kh, kw, dx, d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "tv_bwd_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_tv_backward(x, H, W, C, grad_out, kh, kw, dx, d.n_sms,
+                                             (cudaStream_t)stream), "tv_bwd_kernel");
 }
 
 int lrf_sample_ray(const float* rays, const float* jitter, int64_t N, int32_t S, const float aabb[6],
@@ -651,10 +610,8 @@ int lrf_sample_ray(const float* rays, const float* jitter, int64_t N, int32_t S,
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_sample_ray(rays, jitter, N, S, aabb, near, far, step, pts, z, inside, d.n_sms,
-                                         (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "sample_ray_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_sample_ray(rays, jitter, N, S, aabb, near, far, step, pts, z, inside, d.n_sms,
+                                            (cudaStream_t)stream), "sample_ray_kernel");
 }
 
 int lrf_frame_to_u8(const float* rgb, int32_t rgb_stride, const float* depth, int32_t depth_stride, int64_t N,
@@ -666,10 +623,8 @@ int lrf_frame_to_u8(const float* rgb, int32_t rgb_stride, const float* depth, in
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_frame_u8(rgb, rgb_stride, depth, depth_stride, N, d_lo, d_hi, lut, rgb8, depth8,
-                                       d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "frame_u8_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_frame_u8(rgb, rgb_stride, depth, depth_stride, N, d_lo, d_hi, lut, rgb8, depth8,
+                                          d.n_sms, (cudaStream_t)stream), "frame_u8_kernel");
 }
 
 size_t lrf_image_metrics_scratch_bytes(int32_t H, int32_t W, int32_t filter_size) {
@@ -692,10 +647,8 @@ int lrf_image_metrics(const float* img, int32_t img_stride, const float* gt, int
   if (scratch_bytes < lrf::metrics_scratch_bytes(H, W))
     return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_image_metrics_scratch_bytes(H, W, filter_size)");
   const double c1 = (k1 * max_val) * (k1 * max_val), c2 = (k2 * max_val) * (k2 * max_val);
-  cudaError_t e = lrf::launch_image_metrics(img, img_stride, gt, gt_stride, H, W, filter_size, filter_sigma, c1, c2,
-                                            out, ssim_map, scratch, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "metrics_tile_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_image_metrics(img, img_stride, gt, gt_stride, H, W, filter_size, filter_sigma, c1, c2,
+                                               out, ssim_map, scratch, (cudaStream_t)stream), "metrics_tile_kernel");
 }
 
 static int check_loss_batch(const LrfLossBatch* b, const void* scratch, size_t scratch_bytes) {
@@ -727,9 +680,7 @@ int lrf_supervision_losses(const LrfLossBatch* b, float* losses, void* scratch, 
   const int rc = check_loss_batch(b, scratch, scratch_bytes);
   if (rc != LRF_OK) return rc;
   if (!losses) return fail(LRF_ERR_INVALID, "losses is NULL");
-  cudaError_t e = lrf::launch_supervision_losses(*b, losses, scratch, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "supervision_losses");
-  return LRF_OK;
+  return cuda_status(lrf::launch_supervision_losses(*b, losses, scratch, (cudaStream_t)stream), "supervision_losses");
 }
 
 int lrf_supervision_losses_backward(const LrfLossBatch* b, const float* grad_losses, const LrfLossGrads* g,
@@ -737,9 +688,8 @@ int lrf_supervision_losses_backward(const LrfLossBatch* b, const float* grad_los
   const int rc = check_loss_batch(b, scratch, scratch_bytes);
   if (rc != LRF_OK) return rc;
   if (!grad_losses || !g) return fail(LRF_ERR_INVALID, "grad_losses / grads is NULL");
-  cudaError_t e = lrf::launch_supervision_losses_backward(*b, grad_losses, *g, scratch, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "supervision_losses_backward");
-  return LRF_OK;
+  return cuda_status(lrf::launch_supervision_losses_backward(*b, grad_losses, *g, scratch,
+                                                             (cudaStream_t)stream), "supervision_losses_backward");
 }
 
 int lrf_adam_step(const LrfAdamTensor* t, int64_t n, lrf_stream_t stream) {
@@ -749,9 +699,7 @@ int lrf_adam_step(const LrfAdamTensor* t, int64_t n, lrf_stream_t stream) {
     if (t[i].numel > 0 && (!t[i].param || !t[i].grad || !t[i].exp_avg || !t[i].exp_avg_sq))
       return fail(LRF_ERR_INVALID, "param / grad / exp_avg / exp_avg_sq of a tensor with elements is NULL");
   }
-  cudaError_t e = lrf::launch_adam_step(t, n, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "adam_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_adam_step(t, n, (cudaStream_t)stream), "adam_kernel");
 }
 
 int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t stream) {
@@ -774,9 +722,7 @@ int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t 
   const int n_flow_out = !!g->fwd_flow + !!g->fwd_mask + !!g->bwd_flow + !!g->bwd_mask;
   if (n_flow_out != n_flow)
     return fail(LRF_ERR_INVALID, "the flow outputs must be set exactly when the store has the flow group");
-  cudaError_t e = lrf::launch_gather_rays(*s, *g, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "gather_rays_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_gather_rays(*s, *g, (cudaStream_t)stream), "gather_rays_kernel");
 }
 
 static bool panel_size_ok(int32_t W, int32_t H) {
@@ -808,9 +754,7 @@ int lrf_test_panels(const LrfPanelFrame* f, void* scratch, size_t scratch_bytes,
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_test_panels(*f, scratch, d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "test_panels");
-  return LRF_OK;
+  return cuda_status(lrf::launch_test_panels(*f, scratch, d.n_sms, (cudaStream_t)stream), "test_panels");
 }
 
 int lrf_peer_barrier(unsigned long long* const* peer_flags, int32_t rank, int32_t world,
@@ -826,9 +770,8 @@ int lrf_peer_signal_wait(unsigned long long* const* peer_flags, int32_t rank, in
   for (int p = 0; p < world; ++p)
     if (!peer_flags[p] || ((uintptr_t)peer_flags[p] & 7))
       return fail(LRF_ERR_INVALID, "peer flag arrays must be non-NULL and 8-byte aligned");
-  cudaError_t e = lrf::launch_peer_barrier(peer_flags, rank, world, seq, wait_seq, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "peer_barrier_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_peer_barrier(peer_flags, rank, world, seq, wait_seq,
+                                              (cudaStream_t)stream), "peer_barrier_kernel");
 }
 
 int lrf_pack_bf16(const float* src, void* dst, int64_t n, lrf_stream_t stream) {
@@ -837,17 +780,13 @@ int lrf_pack_bf16(const float* src, void* dst, int64_t n, lrf_stream_t stream) {
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
-  cudaError_t e = lrf::launch_pack_bf16(src, dst, n, d.n_sms, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "pack_bf16_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_pack_bf16(src, dst, n, d.n_sms, (cudaStream_t)stream), "pack_bf16_kernel");
 }
 
 int lrf_repack_nchw_to_nhwc(const float* src, float* dst, int32_t C, int32_t H, int32_t W,
                             lrf_stream_t stream) {
   if (!src || !dst || C < 1 || H < 1 || W < 1) return fail(LRF_ERR_INVALID, "bad repack arguments");
-  cudaError_t e = lrf::launch_repack(src, dst, C, (long long)H * W, (cudaStream_t)stream);
-  if (e != cudaSuccess) return cuda_fail(e, "repack_kernel");
-  return LRF_OK;
+  return cuda_status(lrf::launch_repack(src, dst, C, (long long)H * W, (cudaStream_t)stream), "repack_kernel");
 }
 
 int lrf_launch_info(int32_t* n_sms, int32_t* threads_per_cta, int32_t* smem_bytes_per_cta) {

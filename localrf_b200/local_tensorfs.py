@@ -37,16 +37,17 @@ def ids2pixel(W, H, ids):
     return ids % W, (ids // W) % H
 
 
-class _EvalPlan:
-    """Everything an eval-mode `LocalTensorfs.forward` call derives from the module state, resolved
-    once: active fields, per-launch LrfBatch structs, the device copies of cameras / intrinsics /
-    exposure / blending rows.  A repeated call (the renderer's per-frame or per-batch loop) then only
-    re-checks the guards, allocates outputs and enqueues the launches.
+class _LaunchPlan:
+    """Everything a fused `LocalTensorfs.forward` call derives from the module state: one entry per lrf_render
+    launch (field, distance table, LrfBatch, first ray of its chunk, whether it is the chunk's last launch) and the
+    device copies of cameras / intrinsics / exposure / blending rows the batches point at.  An eval call without
+    autograd caches its plan, so a repeated call (the renderer's per-frame or per-batch loop) only re-checks the
+    guards, allocates outputs and enqueues the launches.
 
     `guards` = (container, index, tensor, version): the plan is valid while every guarded slot still
     holds the same tensor object at the same version (optimiser steps, load_state_dict, append_* all
     bump one of them).  Field parameters are guarded by TensorBase.field_and_prepared's own memo."""
-    __slots__ = ("guards", "launches", "keep", "n", "dev", "out_struct", "key_refs")
+    __slots__ = ("guards", "launches", "keep", "dev", "key_refs")
 
     def valid(self):
         for cont, idx, t, ver in self.guards:
@@ -70,21 +71,47 @@ def _uva_pointer(t):
     return t.data_ptr()
 
 
-def _train_batch(ray_ids, W, H, fov360, cam2world, intr, exposure, w2rf, bg):
-    """LrfBatch of the training call: ray-generation mode, one field, no blend, finalize = 0 (the exposure and the
-    clamp run in lrf_exposure_clamp).  All tensors contiguous fp32 (ray_ids int64) on the device."""
-    b = _lib.LrfBatch()
-    b.n_rays = ray_ids.shape[0]
-    b.ray_ids = ray_ids.data_ptr()
-    b.W, b.H = int(W), int(H)
-    b.fov360 = int(fov360)
-    b.intrinsics = intr.data_ptr()
-    b.cam2world = cam2world.data_ptr()
-    b.n_views = cam2world.shape[0]
-    b.world2rf = w2rf.data_ptr()
-    b.exposure = exposure.data_ptr() if exposure is not None else None
-    b.white_bg = int(bg)
+def _ray_ids(ray_ids):
+    """(contiguous int64 ids, their device-usable address).  The address is that of the tensor the kernel reads: an
+    int32 or strided pinned batch converts to a pageable copy, which is refused like pageable ids."""
+    if ray_ids.dtype != torch.int64 or not ray_ids.is_contiguous():
+        ray_ids = ray_ids.to(torch.int64).contiguous()
+    return ray_ids, _uva_pointer(ray_ids)
+
+
+def _chunks(n, n_views, budget):
+    """(lo, hi, v_lo, v_hi) of consecutive chunks of whole views, at most `budget` rays each (but at least one view);
+    one chunk when n <= budget.  Chunks stay on view boundaries because the kernel derives a ray's view from its
+    position in the launch."""
+    per_view = n // n_views
+    step = n if n <= budget else max(per_view, (budget // per_view) * per_view)
+    for lo in range(0, n, step):
+        hi = min(lo + step, n)
+        yield lo, hi, lo // per_view, hi // per_view
+
+
+def _ray_batch(ids_ptr, n_rays, W, H, fov360, intr, cam2world, w2rf, v_lo, v_hi, exposure=None, blend=None, k=0,
+               **flags):
+    """LrfBatch in ray-generation mode: `n_rays` ids at `ids_ptr` over the views [v_lo, v_hi) of cam2world [V,3,4],
+    of exposure [V,3,3] and of column k of blend [V, n_fields] (the last two when given); `flags` are the remaining
+    scalar fields (white_bg, accumulate, finalize, floater_thresh, refine).  All tensors contiguous fp32 on the
+    device."""
+    b = _lib.LrfBatch(n_rays=n_rays, ray_ids=ids_ptr, W=int(W), H=int(H), fov360=int(fov360),
+                      intrinsics=intr.data_ptr(), cam2world=cam2world.data_ptr() + 48 * v_lo, n_views=v_hi - v_lo,
+                      world2rf=w2rf.data_ptr(), **flags)
+    if exposure is not None:
+        b.exposure = exposure.data_ptr() + 36 * v_lo
+    if blend is not None:
+        b.blend = blend.data_ptr() + 4 * (v_lo * blend.shape[1] + k)
+        b.blend_stride = blend.shape[1]
     return b
+
+
+def _train_batch(ray_ids, W, H, fov360, cam2world, intr, exposure, w2rf, bg):
+    """LrfBatch of the training call: one field, no blend, finalize = 0 (the exposure and the clamp run in
+    lrf_exposure_clamp), every view of cam2world.  All tensors contiguous fp32 (ray_ids int64) on the device."""
+    return _ray_batch(ray_ids.data_ptr(), ray_ids.shape[0], W, H, fov360, intr, cam2world, w2rf, 0, cam2world.shape[0],
+                      exposure=exposure, white_bg=int(bg))
 
 
 class _TrainRenderFn(torch.autograd.Function):
@@ -430,24 +457,27 @@ class LocalTensorfs(torch.nn.Module):
     # ---------------------------------------------------------------------------------------------
     # the hot path (local_tensorfs.py:382-499)
     # ---------------------------------------------------------------------------------------------
+    def _intrinsics(self, W, H):
+        """[focal(W), cx, cy]: center(W, H) as the same fp32 products, without its host-to-device copy."""
+        return torch.cat([self.focal(W).reshape(1), self.center_rel[0:1] * W, self.center_rel[1:2] * H])
+
     def _exposure_for(self, ids, test_id, dev):
-        """Per-view 3x3 exposure [V,3,3]; held-out frames average their neighbours with the
-        reference's edge rules (:481-493).  `ids` is the host list of view ids."""
+        """Per-view 3x3 exposure [V,3,3], fp32 on `dev`, of the host list of view ids: the stacked parameters (with
+        their graph); held-out frames (`test_id`) average their neighbours, detached, with the reference's edge rules
+        (:481-493)."""
         if not test_id:
-            mats = [self.exposure[i] for i in ids]
-        else:
-            n = len(self.exposure)
-            mats = []
-            for v in ids:
-                lo = max(v - 1, 0)
-                if lo == v:
-                    lo = 1
-                hi = min(v + 1, n - 1)
-                if lo == v:                     # the reference re-tests the rewritten lower index
-                    hi = n - 2
-                mats.append((self.exposure[lo].detach() + self.exposure[hi].detach()) / 2)
-        out = mats[0].detach()[None] if len(mats) == 1 else torch.stack([m.detach() for m in mats])
-        return out.to(dev, torch.float32).contiguous()
+            return torch.stack([self.exposure[i] for i in ids]).to(dev, torch.float32)
+        n = len(self.exposure)
+        mats = []
+        for v in ids:
+            lo = max(v - 1, 0)
+            if lo == v:
+                lo = 1
+            hi = min(v + 1, n - 1)
+            if lo == v:                     # the reference re-tests the rewritten lower index
+                hi = n - 2
+            mats.append((self.exposure[lo].detach() + self.exposure[hi].detach()) / 2)
+        return torch.stack(mats).to(dev, torch.float32)
 
     def _forward_autograd(self, ray_ids, view_ids, ids, W, H, white_bg, is_train, cam2world,
                           world2rf, blend, active, chunk, test_id, floater_thresh):
@@ -468,13 +498,8 @@ class LocalTensorfs(torch.nn.Module):
         if cam2world is None:
             cam2world = self.get_cam2world(ids)
         per_view = n // n_views
-        rgbs = torch.zeros_like(directions)
-        depth_maps = torch.zeros_like(directions[..., 0])
-        budget = max(chunk // len(active), 1)
-        step = n if n <= budget else max(per_view, (budget // per_view) * per_view)
         outs_rgb, outs_depth = [], []
-        for lo in range(0, n, step):
-            hi = min(lo + step, n)
+        for lo, hi, _, _ in _chunks(n, n_views, max(chunk // len(active), 1)):
             rgb_c = torch.zeros(hi - lo, 3, device=dev)
             depth_c = torch.zeros(hi - lo, device=dev)
             for k in active:
@@ -495,11 +520,7 @@ class LocalTensorfs(torch.nn.Module):
             outs_rgb.append(rgb_c); outs_depth.append(depth_c)
         rgbs = torch.cat(outs_rgb); depth_maps = torch.cat(outs_depth)
         if self.lr_exposure_init > 0:
-            if test_id:
-                exposure = self._exposure_for(ids, True, dev)
-            else:
-                exposure = torch.stack([self.exposure[v] for v in ids], dim=0)
-            exposure = exposure.repeat_interleave(per_view, dim=0)
+            exposure = self._exposure_for(ids, test_id, dev).repeat_interleave(per_view, dim=0)
             rgbs = torch.bmm(exposure, rgbs[..., None])[..., 0]
         return rgbs.clamp(0, 1), depth_maps, directions, ij
 
@@ -507,33 +528,22 @@ class LocalTensorfs(torch.nn.Module):
         """The training call under autograd for a field _RenderFn covers: one _TrainRenderFn node per chunk (each
         with its own distance-table draw, then its background coin, in the composed path's RNG order)."""
         dev = ray_ids.device
-        n, n_views = ray_ids.shape[0], len(ids)
         rf = self.tensorfs[k]
         sources = [self.init_focal, self.focal_offset, self.center_rel]
         if cam2world is None:
             cam2world = self.get_cam2world(ids)
             sources += [self.r_c2w[i] for i in ids] + [self.t_c2w[i] for i in ids]
-        # focal(W) and center(W, H) without center()'s host-to-device copy: the same fp32 products
-        intr = torch.cat([self.focal(W).reshape(1), self.center_rel[0:1] * W, self.center_rel[1:2] * H])
+        intr = self._intrinsics(W, H)
         exposure = None
         if self.lr_exposure_init > 0:
-            if test_id:
-                exposure = self._exposure_for(ids, True, dev)
-            else:
-                exposure = torch.stack([self.exposure[v] for v in ids], dim=0)
+            exposure = self._exposure_for(ids, test_id, dev)
             sources += list(self.exposure) if test_id else [self.exposure[v] for v in ids]
         w2 = world2rf[k]
         sources.append(w2)
-        rays_i = ray_ids
-        if rays_i.dtype != torch.int64 or not rays_i.is_contiguous():
-            rays_i = rays_i.to(torch.int64).contiguous()
-        per_view = n // n_views
-        step = n if n <= chunk else max(per_view, (chunk // per_view) * per_view)
+        rays_i, _ = _ray_ids(ray_ids)
         params = rf._grad_params()
         outs = []
-        for lo in range(0, n, step):
-            hi = min(lo + step, n)
-            v_lo, v_hi = lo // per_view, hi // per_view
+        for lo, hi, v_lo, v_hi in _chunks(ray_ids.shape[0], len(ids), chunk):
             z = rf.sample_table(True, -1, dev)
             bg = bool(white_bg) or bool(torch.rand((1,)) < 0.5)     # tensorBase.py:633, after the table's jitter
             outs.append(_TrainRenderFn.apply(rf, z, bg, rays_i[lo:hi], W, H, self.fov == 360, sources,
@@ -593,32 +603,84 @@ class LocalTensorfs(torch.nn.Module):
                 exchange[0].skip_step(_stream(dev))       # ... but the peers still need this rank's step flag
             return (torch.empty(0, 3, device=dev), torch.empty(0, device=dev), torch.empty(0, 3, device=dev),
                     torch.empty(0, 2, dtype=torch.int64, device=dev))
+        key = plan = None
         if not is_train and not torch.is_grad_enabled():
-            # eval fast path: reuse the resolved plan of an identical earlier call
+            # eval: the plan of an identical earlier call serves this one while its guards hold
             vkey = (id(view_ids), view_ids._version) if torch.is_tensor(view_ids) else tuple(view_ids)
             key = (vkey, n, W, H, bool(white_bg), bool(test_id), float(floater_thresh),
                    None if cam2world is None else (id(cam2world), cam2world._version),
                    None if world2rf is None else id(world2rf),
                    None if blending_weights is None else (id(blending_weights), blending_weights._version),
                    id(self.blending_weights), len(self.tensorfs), exchange is not None, bool(self.is_refining), dev)
-            plans = self.__dict__.setdefault("_plans", {})
-            plan = plans.get(key)
-            if plan is not None and plan.valid():
-                return self._run_plan(plan, ray_ids, stats, exchange, out)
-            res = self._forward_general(ray_ids, view_ids, W, H, white_bg, is_train, cam2world, world2rf,
-                                        blending_weights, chunk, test_id, floater_thresh, stats, exchange,
-                                        out, dev, want_plan=True)
-            if isinstance(res, tuple) and len(res) == 2 and isinstance(res[0], _EvalPlan):
-                plan, res = res
+            plan = self.__dict__.setdefault("_plans", {}).get(key)
+            if plan is not None and not plan.valid():
+                plan = None
+        if plan is None:
+            # (not memoised: a new tensor can reuse a freed tensor's id and storage)
+            ids = view_ids.tolist() if torch.is_tensor(view_ids) else [int(v) for v in view_ids]
+            n_views = len(ids)
+            if n_views == 0 or n % n_views != 0:
+                raise ValueError("ray_ids must hold the same number of rays for every view")
+            n_fields = len(self.tensorfs)
+
+            # -- which fields render, with which per-view weights (:403-418) ------------------------
+            blend = None                                   # device [V, n_fields] or None (= weight 1)
+            if is_train:                                   # one field trains at a time (:411-416)
+                active = [n_fields - 1]
+            elif blending_weights is None:
+                rows = self._blend_host()[ids]
+                active = torch.nonzero(rows.sum(dim=0))[:, 0].tolist()
+                bw = self.blending_weights
+                blend = bw.detach()[ids[0]:ids[0] + 1] if n_views == 1 else bw.detach()[view_ids]
+                blend = blend.to(dev, torch.float32).contiguous()
+            else:
+                blend = blending_weights.detach().to(dev, torch.float32).contiguous()
+                active = torch.nonzero(blend.sum(dim=0))[:, 0].tolist()
+            if len(active) == 0:
+                print("****** No valid RF")
+                i, j = ids2pixel(W, H, ray_ids)
+                ones = torch.ones_like(ray_ids).float()
+                return torch.ones([n, 3], device=dev), ones, torch.zeros(n, 3, device=dev), torch.stack([i, j], -1)
+
+            if world2rf is None:
+                world2rf = self.world2rf
+            if torch.is_grad_enabled():
+                tracked = [self.init_focal, self.focal_offset, self.center_rel]
+                tracked += [cam2world] if cam2world is not None else \
+                    [self.r_c2w[i] for i in ids] + [self.t_c2w[i] for i in ids]
+                tracked += [self.exposure[i] for i in ids] if self.lr_exposure_init > 0 else []
+                for k in active:
+                    tracked += list(self.tensorfs[k].parameters())
+                needs_composed = any(t is not None and t.requires_grad for t in tracked)
+            else:
+                needs_composed = False
+            if needs_composed or not all(self.tensorfs[k].fused_supported() for k in active):
+                if exchange is not None or out is not None:
+                    raise NotImplementedError("exchange= / out= are served by the fused eval path only")
+                if not ray_ids.is_cuda:
+                    ray_ids = ray_ids.to(dev)
+                if needs_composed and is_train and self._train_node_covers(active[0], floater_thresh):
+                    return self._forward_train(ray_ids, ids, W, H, white_bg, cam2world, world2rf, active[0], chunk,
+                                               test_id)
+                return self._forward_autograd(ray_ids, view_ids, ids, W, H, white_bg, is_train,
+                                              cam2world, world2rf, blend, active, chunk, test_id,
+                                              floater_thresh)
+            if exchange is not None and is_train:
+                raise ValueError("the fused pixel exchange serves eval batches (is_train=False)")
+
+        rays_i, ids_ptr = _ray_ids(ray_ids)               # (rays_i holds the ids until the launches are enqueued)
+        outs = self._alloc_outputs(n, dev, exchange, out)
+        if plan is None:
+            plan = self._resolve(ids, n, W, H, white_bg, is_train, cam2world, world2rf, blending_weights, blend,
+                                 active, chunk, test_id, floater_thresh, dev)
+            if key is not None:
                 # the key holds ids of caller objects: keep them alive so the ids cannot be recycled
                 plan.key_refs = (view_ids, cam2world, world2rf, blending_weights)
+                plans = self.__dict__["_plans"]
                 if len(plans) >= 256:
                     plans.clear()
                 plans[key] = plan
-            return res
-        return self._forward_general(ray_ids, view_ids, W, H, white_bg, is_train, cam2world, world2rf,
-                                     blending_weights, chunk, test_id, floater_thresh, stats, exchange,
-                                     out, dev, want_plan=False)
+        return self._run(plan, ids_ptr, outs, stats, exchange)
 
     def _alloc_outputs(self, n, dev, exchange, out):
         """(pix or None, rgbs, depth, directions, ij) -- fresh tensors owned by the caller."""
@@ -639,94 +701,13 @@ class LocalTensorfs(torch.nn.Module):
         ij = torch.empty(n, 2, dtype=torch.int64, device=dev)
         return pix, rgbs, depth, directions, ij
 
-    def _run_plan(self, plan, ray_ids, stats, exchange, out):
-        dev, n = plan.dev, plan.n
-        rays_i = ray_ids
-        if rays_i.dtype != torch.int64 or not rays_i.is_contiguous():
-            rays_i = rays_i.to(torch.int64).contiguous()
-        pix, rgbs, depth, directions, ij = self._alloc_outputs(n, dev, exchange, out)
-        lib = _lib.lib()
-        o = plan.out_struct
-        o.pix = o.rgb = o.depth = None
-        o.n_peers, o.signal_seq, o.wait_seq, o.mc_pix = 0, 0, 0, None   # (exchange fields are set for the last launch only)
-        if pix is not None:
-            o.pix = pix.data_ptr()
-        else:
-            o.rgb, o.depth = rgbs.data_ptr(), depth.data_ptr()
-        o.directions, o.ij = directions.data_ptr(), ij.data_ptr()
-        o.stats = stats.data_ptr() if stats is not None else None
-        ids_ptr = rays_i.data_ptr()
-        with torch.cuda.device(dev):
-            stream = _stream(dev)
-            last = len(plan.launches) - 1
-            for pos, (rf, z, b) in enumerate(plan.launches):
-                fs, prep = rf.field_and_prepared(z)
-                b.ray_ids = ids_ptr
-                if pos == last and exchange is not None:
-                    exchange[0].fill_outputs(o, exchange[1])
-                _lib.check(lib.lrf_render(C.byref(fs), _ptr(prep), C.byref(b), C.byref(o), stream))
-            if exchange is not None:
-                exchange[0].close_step(stream)
-        return rgbs, depth, directions, ij
-
-    def _forward_general(self, ray_ids, view_ids, W, H, white_bg, is_train, cam2world, world2rf,
-                         blending_weights, chunk, test_id, floater_thresh, stats, exchange, out, dev,
-                         want_plan):
-        n = ray_ids.shape[0]
-        # (not memoised: a new tensor can reuse a freed tensor's id and storage)
-        ids = view_ids.tolist() if torch.is_tensor(view_ids) else [int(v) for v in view_ids]
-        n_views = len(ids)
-        if n_views == 0 or n % n_views != 0:
-            raise ValueError("ray_ids must hold the same number of rays for every view")
-        n_fields = len(self.tensorfs)
+    def _resolve(self, ids, n, W, H, white_bg, is_train, cam2world, world2rf, blending_weights, blend, active,
+                 chunk, test_id, floater_thresh, dev):
+        """The _LaunchPlan of a fused call: the device copies of the cameras, intrinsics and exposure (memoised on
+        parameter versions), then per chunk and active field its distance table, background coin and LrfBatch.  Train
+        mode draws fresh jitter per chunk like the reference, in the composed path's RNG order; eval has no
+        randomness, so the whole batch is one launch per field."""
         guards = []
-
-        # -- which fields render, with which per-view weights (:403-418) ----------------------------
-        blend = None                                   # device [V, n_fields] or None (= weight 1)
-        if is_train:                                   # one field trains at a time (:411-416)
-            active = [n_fields - 1]
-        elif blending_weights is None:
-            rows = self._blend_host()[ids]
-            active = torch.nonzero(rows.sum(dim=0))[:, 0].tolist()
-            bw = self.blending_weights
-            blend = bw.detach()[ids[0]:ids[0] + 1] if n_views == 1 else bw.detach()[view_ids]
-            blend = blend.to(dev, torch.float32).contiguous()
-        else:
-            blend = blending_weights.detach().to(dev, torch.float32).contiguous()
-            active = torch.nonzero(blend.sum(dim=0))[:, 0].tolist()
-        if len(active) == 0:
-            print("****** No valid RF")
-            i, j = ids2pixel(W, H, ray_ids)
-            ones = torch.ones_like(ray_ids).float()
-            return torch.ones([n, 3], device=dev), ones, torch.zeros(n, 3, device=dev), torch.stack([i, j], -1)
-
-        if world2rf is None:
-            world2rf = self.world2rf
-        if torch.is_grad_enabled():
-            tracked = [self.init_focal, self.focal_offset, self.center_rel]
-            tracked += [cam2world] if cam2world is not None else \
-                [self.r_c2w[i] for i in ids] + [self.t_c2w[i] for i in ids]
-            tracked += [self.exposure[i] for i in ids] if self.lr_exposure_init > 0 else []
-            for k in active:
-                tracked += list(self.tensorfs[k].parameters())
-            needs_composed = any(t is not None and t.requires_grad for t in tracked)
-        else:
-            needs_composed = False
-        if needs_composed or not all(self.tensorfs[k].fused_supported() for k in active):
-            if exchange is not None or out is not None:
-                raise NotImplementedError("exchange= / out= are served by the fused eval path only")
-            if not ray_ids.is_cuda:
-                ray_ids = ray_ids.to(dev)
-            if needs_composed and is_train and self._train_node_covers(active[0], floater_thresh):
-                return self._forward_train(ray_ids, ids, W, H, white_bg, cam2world, world2rf, active[0], chunk,
-                                           test_id)
-            return self._forward_autograd(ray_ids, view_ids, ids, W, H, white_bg, is_train,
-                                          cam2world, world2rf, blend, active, chunk, test_id,
-                                          floater_thresh)
-        if exchange is not None and is_train:
-            raise ValueError("the fused pixel exchange serves eval batches (is_train=False)")
-
-        # -- cameras, intrinsics, exposure (memoised on parameter versions) ---------------------------
         P = self._parameters
         if blending_weights is None and not is_train:
             guards.append((P, "blending_weights", self.blending_weights, self.blending_weights._version))
@@ -740,12 +721,10 @@ class LocalTensorfs(torch.nn.Module):
                 guards.append((self.t_c2w._parameters, str(i), self.t_c2w[i], self.t_c2w[i]._version))
         else:
             cam2world = cam2world.detach().to(dev, torch.float32).contiguous()
-        fov360 = self.fov == 360
         src = [self.init_focal, self.focal_offset, self.center_rel]
         key = (W, H, self.W, tuple((id(t), t._version) for t in src), str(dev))
-        intr = self._cached("intr", key, lambda: torch.cat(
-            [self.focal(W).detach().reshape(1), self.center(W, H).detach().reshape(2)])
-            .to(dev, torch.float32).contiguous(), refs=src)
+        intr = self._cached("intr", key, lambda: self._intrinsics(W, H).detach().to(dev, torch.float32).contiguous(),
+                            refs=src)
         for name in ("init_focal", "focal_offset", "center_rel"):
             guards.append((P, name, P[name], P[name]._version))
         exposure = None
@@ -755,89 +734,66 @@ class LocalTensorfs(torch.nn.Module):
                                      + [min(1, n_e - 1), max(n_e - 2, 0)] if test_id else [])))
             src = [self.exposure[i] for i in used]
             key = (tuple(ids), bool(test_id), n_e, tuple((id(t), t._version) for t in src), str(dev))
-            exposure = self._cached("expo", key, lambda: self._exposure_for(ids, test_id, dev), refs=src)
+            exposure = self._cached("expo", key, lambda: self._exposure_for(ids, test_id, dev).detach(), refs=src)
             for i, t in zip(used, src):
                 guards.append((self.exposure._parameters, str(i), t, t._version))
-        rays_i = ray_ids.detach()
-        if rays_i.dtype != torch.int64 or not rays_i.is_contiguous():
-            rays_i = rays_i.to(torch.int64).contiguous()
-        ids_ptr = _uva_pointer(rays_i)
 
-        pix, rgbs, depth, directions, ij = self._alloc_outputs(n, dev, exchange, out)
+        plan = _LaunchPlan()
+        plan.guards, plan.launches, plan.dev, plan.key_refs = guards, [], dev, None
+        plan.keep = [cam2world, intr, exposure, blend]
+        fov360 = self.fov == 360
+        for lo, hi, v_lo, v_hi in _chunks(n, len(ids), max(chunk // len(active), 1) if is_train else n):
+            for pos, k in enumerate(active):
+                rf = self.tensorfs[k]
+                if rf.basis_mat.weight.device != dev:
+                    rf.to(dev)
+                z = rf.sample_table(is_train, -1, dev)
+                w2 = world2rf[k]
+                w2rf = w2.detach() if (w2.device == dev and w2.dtype == torch.float32 and w2.is_contiguous()) else \
+                    w2.detach().to(dev, torch.float32).contiguous()
+                last = pos == len(active) - 1
+                b = _ray_batch(None, hi - lo, W, H, fov360, intr, cam2world, w2rf, v_lo, v_hi, exposure, blend, k,
+                               accumulate=int(pos > 0), finalize=int(last),
+                               white_bg=int(bool(white_bg) or bool(is_train and torch.rand((1,)) < 0.5)),
+                               floater_thresh=float(floater_thresh),
+                               refine=int(bool(self.is_refining)))        # local_tensorfs.py:463
+                plan.launches.append((rf, z, b, lo, last))
+                plan.keep.append(w2rf)
+                guards.append((self.tensorfs._modules, str(k), rf, None))
+                if isinstance(world2rf, torch.nn.ParameterList):
+                    guards.append((world2rf._parameters, str(k), w2, w2._version))
+                else:
+                    guards.append((world2rf, k, w2, w2._version))
+                guards.append((rf.__dict__, "nSamples", rf.nSamples, "eq"))
+        return plan
 
-        # train mode: the reference draws fresh jitter per chunk; eval has no randomness, so the
-        # whole batch is one launch per field.  Chunks are kept on view boundaries (the kernel
-        # derives a ray's view from its position in the launch).
-        per_view = n // n_views
-        budget = max(chunk // len(active), 1)
-        if is_train and n > budget:
-            chunk = max(per_view, (budget // per_view) * per_view)
+    def _run(self, plan, ids_ptr, outs, stats, exchange):
+        """Enqueues the plan's launches on the ids at `ids_ptr` into `outs` (_alloc_outputs).  With an exchange the
+        last launch of a chunk also stores every finished pixel into the peers' buffers (exchange calls are eval
+        calls: one chunk)."""
+        pix, rgbs, depth, directions, ij = outs
+        o = _lib.LrfOutputs()
+        if stats is not None:
+            o.stats = stats.data_ptr()
+        if pix is not None:
+            p_pix = pix.data_ptr()
         else:
-            chunk = n
+            p_rgb, p_depth = rgbs.data_ptr(), depth.data_ptr()
+        p_dirs, p_ij = directions.data_ptr(), ij.data_ptr()
         lib = _lib.lib()
-        launches, keep = [], [cam2world, intr, exposure, blend]
-        with torch.cuda.device(dev):
-            stream = _stream(dev)
-            for lo in range(0, n, chunk):
-                hi = min(lo + chunk, n)
-                v_lo, v_hi = lo // per_view, (hi + per_view - 1) // per_view
-                for pos, k in enumerate(active):
-                    rf = self.tensorfs[k]
-                    if rf.basis_mat.weight.device != dev:
-                        rf.to(dev)
-                    z = rf.sample_table(is_train, -1, dev)
-                    fs, prep = rf.field_and_prepared(z)
-                    w2 = world2rf[k]
-                    w2rf = w2.detach() if (w2.device == dev and w2.dtype == torch.float32
-                                            and w2.is_contiguous()) else \
-                        w2.detach().to(dev, torch.float32).contiguous()
-                    b = _lib.LrfBatch()
-                    b.n_rays = hi - lo
-                    b.ray_ids = ids_ptr + 8 * lo
-                    b.W, b.H = int(W), int(H)
-                    b.fov360 = int(fov360)
-                    b.intrinsics = intr.data_ptr()
-                    b.cam2world = cam2world.data_ptr() + 48 * v_lo
-                    b.n_views = v_hi - v_lo
-                    b.world2rf = w2rf.data_ptr()
-                    if blend is not None:
-                        b.blend = blend.data_ptr() + 4 * (v_lo * blend.shape[1] + k)
-                        b.blend_stride = blend.shape[1]
-                    b.accumulate = int(pos > 0)
-                    b.finalize = int(pos == len(active) - 1)
-                    if exposure is not None:
-                        b.exposure = exposure.data_ptr() + 36 * v_lo
-                    b.white_bg = int(bool(white_bg) or bool(is_train and torch.rand((1,)) < 0.5))
-                    b.floater_thresh = float(floater_thresh)
-                    b.refine = int(bool(self.is_refining))        # local_tensorfs.py:463
-                    o = _lib.LrfOutputs()
-                    if pix is not None:
-                        o.pix = pix.data_ptr() + 16 * lo
-                        if pos == len(active) - 1:
-                            exchange[0].fill_outputs(o, exchange[1] + lo)
-                    else:
-                        o.rgb = _uva_pointer(rgbs) + 12 * lo
-                        o.depth = _uva_pointer(depth) + 4 * lo
-                    o.directions = directions.data_ptr() + 12 * lo
-                    o.ij = ij.data_ptr() + 16 * lo
-                    if stats is not None:
-                        o.stats = stats.data_ptr()
-                    _lib.check(lib.lrf_render(C.byref(fs), _ptr(prep), C.byref(b), C.byref(o), stream))
-                    if want_plan:
-                        launches.append((rf, z, b))
-                        keep.append(w2rf)
-                        guards.append((self.tensorfs._modules, str(k), rf, None))
-                        if isinstance(world2rf, torch.nn.ParameterList):
-                            guards.append((world2rf._parameters, str(k), w2, w2._version))
-                        else:
-                            guards.append((world2rf, k, w2, w2._version))
-                        guards.append((rf.__dict__, "nSamples", rf.nSamples, "eq"))
+        with torch.cuda.device(plan.dev):
+            stream = _stream(plan.dev)
+            for rf, z, b, lo, last in plan.launches:
+                fs, prep = rf.field_and_prepared(z)
+                b.ray_ids = ids_ptr + 8 * lo
+                if pix is not None:
+                    o.pix = p_pix + 16 * lo
+                    if last:
+                        exchange[0].fill_outputs(o, exchange[1] + lo)
+                else:
+                    o.rgb, o.depth = p_rgb + 12 * lo, p_depth + 4 * lo
+                o.directions, o.ij = p_dirs + 12 * lo, p_ij + 16 * lo
+                _lib.check(lib.lrf_render(C.byref(fs), _ptr(prep), C.byref(b), C.byref(o), stream))
             if exchange is not None:
                 exchange[0].close_step(stream)
-        result = (rgbs, depth, directions, ij)
-        if want_plan and chunk == n:
-            plan = _EvalPlan()
-            plan.guards, plan.launches, plan.keep = guards, launches, keep
-            plan.n, plan.dev, plan.out_struct, plan.key_refs = n, dev, _lib.LrfOutputs(), None
-            return plan, result
-        return result
+        return rgbs, depth, directions, ij

@@ -704,19 +704,11 @@ class TensorBase(torch.nn.Module):
             rgb = torch.empty(n, 3, dtype=torch.float32, device=dev)
             depth = torch.empty(n, dtype=torch.float32, device=dev)
             weights = torch.empty(n, z.numel(), dtype=torch.float32, device=dev) if return_weights else None
-            b = _lib.LrfBatch()
-            b.n_rays = n
-            b.rays = rays.data_ptr()
-            b.n_views = 1
-            b.white_bg = int(bg)
-            b.floater_thresh = float(floater_thresh)
-            b.refine = int(bool(refine))
-            o = _lib.LrfOutputs()
-            o.rgb, o.depth = rgb.data_ptr(), depth.data_ptr()
-            if weights is not None:
-                o.weights = weights.data_ptr()
-            if stats is not None:
-                o.stats = stats.data_ptr()
+            b = _lib.LrfBatch(n_rays=n, rays=rays.data_ptr(), n_views=1, white_bg=int(bg),
+                              floater_thresh=float(floater_thresh), refine=int(bool(refine)))
+            o = _lib.LrfOutputs(rgb=rgb.data_ptr(), depth=depth.data_ptr(),
+                                weights=None if weights is None else weights.data_ptr(),
+                                stats=None if stats is None else stats.data_ptr())
             _lib.check(_lib.lib().lrf_render(C.byref(fs), _ptr(prep), C.byref(b), C.byref(o),
                                              _stream(dev)))
         self.last_weights = weights

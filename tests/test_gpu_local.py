@@ -62,3 +62,28 @@ def test_train_mode_multi_view(scene):
         _call(lt, g, "train", g["train.ray_ids"], g["train.view_ids"], is_train=True)
     finally:
         rf.sample_table = orig
+
+
+def test_repeated_call_refuses_pageable_id_copy(scene, monkeypatch):
+    """A repeated eval call reuses the first call's plan.  Pinned int32 ids convert to a pageable int64 copy, which
+    the kernel cannot read: the repeated call refuses it like the first call does, before anything is launched."""
+    from localrf_b200 import _lib
+    g, lt = scene
+    W, H = int(g["W"]), int(g["H"])
+    ids = torch.from_numpy(g["ray_ids"]).to(torch.int64).pin_memory()
+    with torch.no_grad():
+        lt(ids, [2], W, H, is_train=False)
+    torch.cuda.synchronize()
+    real = _lib.lib()
+
+    class NoRender:
+        def __getattr__(self, name):
+            if name == "lrf_render":
+                def launched(*args):
+                    raise AssertionError("launched")
+                return launched
+            return getattr(real, name)
+
+    monkeypatch.setattr(_lib, "lib", NoRender)
+    with torch.no_grad(), pytest.raises(RuntimeError, match="must be pinned"):
+        lt(ids.to(torch.int32).pin_memory(), [2], W, H, is_train=False)
