@@ -480,6 +480,50 @@ typedef struct LrfRayGather {
  * never read on the host.  No atomics, no host synchronisation. */
 int lrf_gather_rays(const LrfFrameStore *store, const LrfRayGather *g, lrf_stream_t stream);
 
+/* One frame into a slot of the store, from its files' decoded pixels.  replaces: the per-frame conversions of
+ * LocalRFDataset.read_meta (dataLoader/localrf_dataset.py:143-258) after cv2.imread, bit for bit.  The output frame
+ * is w x h = store->n_px pixels.  Planes are device memory, row-major with row strides in elements.  INTER_AREA
+ * resizes to w x h in three forms: the same size is a copy; a reduction by k in {2, 4} (source k w x k h) sums each
+ * block in a fixed order (k = 2: ((a + b) + c) + d in row-major order; k = 4: each row in order, then the rows in
+ * order), times 1 / k^2, as cv2 does for 3-channel float32 images; an enlargement (source <= w x h on both axes) is
+ * cv2's separable area-weighted linear rule in fp32, horizontal then vertical, rounded to nearest even and saturated
+ * for uint16.  Any other ratio is LRF_ERR_UNSUPPORTED. */
+typedef struct LrfIngestFrame {
+  int64_t slot;                /* 0 <= slot < store->capacity; the caller tags slot_frame */
+  int32_t w, h;                /* the frame's size: w h == store->n_px */
+  const uint8_t *image;        /* [h0][image_stride] BGR, 3 per pixel: rgb = (float)v / 255, reduced when k > 1 */
+  int32_t w0, h0;              /* (w, h) or (k w, k h), k in {2, 4} */
+  int64_t image_stride;        /* >= 3 w0 */
+  const uint16_t *invdepth;    /* [hd][invdepth_stride]: (float)v, resized; set exactly when the store has invdepth */
+  int32_t wd, hd;              /* same size, reduction or enlargement */
+  int64_t invdepth_stride;     /* >= wd */
+  const uint16_t *fwd_flow;    /* [hf][flow_stride], 3 per pixel, the file's channel order: resized as uint16, then */
+  const uint16_t *bwd_flow;    /* flow = (e0,1 - 32768) / 256 * flow_scale, mask = e2 > 32768 (1 or 0); both set   */
+                               /* exactly when the store has the flow group */
+  int32_t wf, hf;              /* both flows: same size or enlargement */
+  int64_t flow_stride;         /* >= 3 wf */
+  float flow_scale;            /* float32(h / hf_of_the_forward_file) */
+  const uint8_t *mask;         /* [h][mask_stride] motion mask (> 0 keeps the pixel), or NULL (every pixel kept) */
+  int32_t wm, hm;              /* (w, h): a mask of another size is LRF_ERR_UNSUPPORTED */
+  int64_t mask_stride;         /* >= wm */
+} LrfIngestFrame;
+
+/* Device scratch bytes of one frame of n_px pixels (8-byte aligned); 0 if n_px < 1 or the frame is too large (the
+ * variance's summation tree is built for up to 2^16 leaves of 128 pixels, a little over 8.3 M pixels). */
+size_t lrf_ingest_scratch_bytes(int64_t n_px);
+/* Writes rgb, loss_weight and, when the store has them, invdepth, the flows and the flow masks of slot `slot`
+ * (through the store's pointers, which must be writable here).  loss_weight = the variance of the 4-neighbour
+ * Laplacian (reflect-101 borders, fp32) of cv2's 15-bit RGB2GRAY of (uint8)(rgb * 255), as numpy's float32 var()
+ * computes it (pairwise summation of the mean, then of the squared deviations, each divided by n), times the mask.
+ * The variance is summed by a fixed tree in the scratch: no atomics, no host synchronisation, bitwise repeatable.
+ * Nine launches on `stream`.  LRF_ERR_INVALID before any device work for NULL store / frame / scratch, a store
+ * without slot_frame, rgb or loss_weight, a partly given flow group, a slot outside [0, capacity), w h != n_px, a
+ * plane sized below 1 or with a short stride, a NULL plane of a group the store has or a plane of a group it lacks,
+ * and scratch not 8-byte aligned or smaller than lrf_ingest_scratch_bytes(n_px); LRF_ERR_UNSUPPORTED for the
+ * ratios above and frames too large for the scratch. */
+int lrf_ingest_frame(const LrfFrameStore *store, const LrfIngestFrame *frame, void *scratch, size_t scratch_bytes,
+                     lrf_stream_t stream);
+
 /* Flow and depth comparison panels of one held-out frame.  replaces: renderer.py:79-124, the TensorBoard panels
  * render(test=True) builds for every test frame (get_fwd_bwd_cam2cams / get_pred_flow / compute_depth_loss of
  * utils/utils.py:15-59 and the inline numpy / cv2 lines around them).  The frame is rendered at W x H with

@@ -11,7 +11,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
-           "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_panels.cu", "lrf_abi.cu"]
+           "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_panels.cu", "lrf_ingest.cu",
+           "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", "lrf_reproject.cuh", "lrf_select.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -86,6 +87,15 @@ class LrfPanelFrame(C.Structure):
                 ("stats", _vp)]
 
 
+class LrfIngestFrame(C.Structure):
+    _fields_ = [("slot", C.c_int64), ("w", C.c_int32), ("h", C.c_int32),
+                ("image", _vp), ("w0", C.c_int32), ("h0", C.c_int32), ("image_stride", C.c_int64),
+                ("invdepth", _vp), ("wd", C.c_int32), ("hd", C.c_int32), ("invdepth_stride", C.c_int64),
+                ("fwd_flow", _vp), ("bwd_flow", _vp), ("wf", C.c_int32), ("hf", C.c_int32), ("flow_stride", C.c_int64),
+                ("flow_scale", C.c_float),
+                ("mask", _vp), ("wm", C.c_int32), ("hm", C.c_int32), ("mask_stride", C.c_int64)]
+
+
 class LrfBatch(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int64),
@@ -133,7 +143,7 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_image_metrics_scratch_bytes", "lrf_image_metrics", "lrf_supervision_scratch_bytes",
            "lrf_supervision_losses", "lrf_supervision_losses_backward", "lrf_adam_step",
            "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch", "lrf_gather_rays",
-           "lrf_test_panels_scratch_bytes", "lrf_test_panels"]
+           "lrf_test_panels_scratch_bytes", "lrf_test_panels", "lrf_ingest_scratch_bytes", "lrf_ingest_frame"]
 
 
 def _stale():
@@ -187,7 +197,8 @@ def lib():
     L.lrf_sizeof.restype = C.c_size_t
     L.lrf_sizeof.argtypes = [C.c_int32]
     for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
-                                     LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather, LrfPanelFrame)):
+                                     LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather, LrfPanelFrame,
+                                     LrfIngestFrame)):
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -242,6 +253,9 @@ def lib():
     L.lrf_test_panels_scratch_bytes.restype = C.c_size_t
     L.lrf_test_panels_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
     L.lrf_test_panels.argtypes = [C.POINTER(LrfPanelFrame), _vp, C.c_size_t, _vp]
+    L.lrf_ingest_scratch_bytes.restype = C.c_size_t
+    L.lrf_ingest_scratch_bytes.argtypes = [C.c_int64]
+    L.lrf_ingest_frame.argtypes = [C.POINTER(LrfFrameStore), C.POINTER(LrfIngestFrame), _vp, C.c_size_t, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

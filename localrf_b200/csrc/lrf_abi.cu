@@ -59,6 +59,9 @@ cudaError_t launch_adam_step(const LrfAdamTensor* t, long long n, cudaStream_t s
 cudaError_t launch_gather_rays(const LrfFrameStore& s, const LrfRayGather& g, cudaStream_t stream);
 size_t panels_scratch_bytes(long long n_px);
 cudaError_t launch_test_panels(const LrfPanelFrame& f, void* scratch, int n_sms, cudaStream_t stream);
+size_t ingest_scratch_bytes(long long n_px);
+int ingest_resize_mode(int ws, int hs, int w, int h);
+cudaError_t launch_ingest_frame(const LrfFrameStore& st, const LrfIngestFrame& f, void* scratch, cudaStream_t stream);
 cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
                                 cudaStream_t stream);
 cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
@@ -265,6 +268,7 @@ size_t lrf_sizeof(int32_t which) {
     case 8: return sizeof(LrfFrameStore);
     case 9: return sizeof(LrfRayGather);
     case 10: return sizeof(LrfPanelFrame);
+    case 11: return sizeof(LrfIngestFrame);
     default: return 0;
   }
 }
@@ -755,6 +759,59 @@ int lrf_test_panels(const LrfPanelFrame* f, void* scratch, size_t scratch_bytes,
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_test_panels(*f, scratch, d.n_sms, (cudaStream_t)stream), "test_panels");
+}
+
+size_t lrf_ingest_scratch_bytes(int64_t n_px) { return n_px >= 1 ? lrf::ingest_scratch_bytes(n_px) : 0; }
+
+// a plane of ws x hs with `per_px` values per pixel and a row stride of `stride` elements
+static int check_plane(const void* p, int32_t ws, int32_t hs, int64_t stride, int per_px, const char* name) {
+  if (!p) return fail(LRF_ERR_INVALID, "%s is NULL", name);
+  if (ws < 1 || hs < 1) return fail(LRF_ERR_INVALID, "the %s plane's sizes must be >= 1", name);
+  if (stride < (int64_t)per_px * ws) return fail(LRF_ERR_INVALID, "the %s plane's row stride is shorter than a row", name);
+  return LRF_OK;
+}
+
+int lrf_ingest_frame(const LrfFrameStore* s, const LrfIngestFrame* f, void* scratch, size_t scratch_bytes,
+                     lrf_stream_t stream) {
+  if (!s || !f) return fail(LRF_ERR_INVALID, "store / frame is NULL");
+  if (s->n_px < 1) return fail(LRF_ERR_INVALID, "n_px must be >= 1");
+  if (s->capacity < 1) return fail(LRF_ERR_INVALID, "capacity must be >= 1");
+  if (!s->slot_frame || !s->rgb || !s->loss_weight)
+    return fail(LRF_ERR_INVALID, "slot_frame / rgb / loss_weight of the store is NULL");
+  const int n_flow = !!s->fwd_flow + !!s->fwd_mask + !!s->bwd_flow + !!s->bwd_mask;
+  if (n_flow != 0 && n_flow != 4)
+    return fail(LRF_ERR_INVALID, "the store's flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, "
+                                 "bwd_mask or none");
+  if (f->slot < 0 || f->slot >= s->capacity) return fail(LRF_ERR_INVALID, "slot must lie in [0, capacity)");
+  if (f->w < 1 || f->h < 1 || (int64_t)f->w * f->h != s->n_px)
+    return fail(LRF_ERR_INVALID, "w and h must be >= 1 with w h == the store's n_px");
+  int rc = check_plane(f->image, f->w0, f->h0, f->image_stride, 3, "image");
+  if (rc != LRF_OK) return rc;
+  if (!s->invdepth != !f->invdepth)
+    return fail(LRF_ERR_INVALID, "invdepth must be set exactly when the store has invdepth");
+  if (f->invdepth && (rc = check_plane(f->invdepth, f->wd, f->hd, f->invdepth_stride, 1, "invdepth")) != LRF_OK)
+    return rc;
+  if (!!f->fwd_flow != !!n_flow || !!f->bwd_flow != !!n_flow)
+    return fail(LRF_ERR_INVALID, "fwd_flow and bwd_flow must be set exactly when the store has the flow group");
+  if (n_flow && ((rc = check_plane(f->fwd_flow, f->wf, f->hf, f->flow_stride, 3, "fwd_flow")) != LRF_OK ||
+                 (rc = check_plane(f->bwd_flow, f->wf, f->hf, f->flow_stride, 3, "bwd_flow")) != LRF_OK))
+    return rc;
+  if (f->mask && (rc = check_plane(f->mask, f->wm, f->hm, f->mask_stride, 1, "mask")) != LRF_OK) return rc;
+  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
+  const size_t need = lrf_ingest_scratch_bytes(s->n_px);
+  if (need == 0) return fail(LRF_ERR_UNSUPPORTED, "frames above 2^16 leaves of 128 pixels are not built");
+  if (scratch_bytes < need)
+    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_ingest_scratch_bytes(n_px)");
+  const int image_mode = lrf::ingest_resize_mode(f->w0, f->h0, f->w, f->h);
+  if (image_mode < 1)
+    return fail(LRF_ERR_UNSUPPORTED, "the image must be w x h or a reduction by 2 or 4 of it (k w x k h)");
+  if (f->invdepth && lrf::ingest_resize_mode(f->wd, f->hd, f->w, f->h) < 0)
+    return fail(LRF_ERR_UNSUPPORTED, "invdepth must be w x h, a reduction by 2 or 4 of it or at most w x h");
+  const int flow_mode = n_flow ? lrf::ingest_resize_mode(f->wf, f->hf, f->w, f->h) : 1;
+  if (flow_mode != 0 && flow_mode != 1)
+    return fail(LRF_ERR_UNSUPPORTED, "the flows must be w x h or at most w x h on both axes (an enlargement)");
+  if (f->mask && (f->wm != f->w || f->hm != f->h)) return fail(LRF_ERR_UNSUPPORTED, "the mask must be w x h");
+  return cuda_status(lrf::launch_ingest_frame(*s, *f, scratch, (cudaStream_t)stream), "ingest_frame");
 }
 
 int lrf_peer_barrier(unsigned long long* const* peer_flags, int32_t rank, int32_t world,

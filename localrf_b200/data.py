@@ -30,7 +30,8 @@ class DeviceRaySampler:
     """LocalRFDataset.sample with the active frames resident on `device`.
 
     Reads only the dataset's state -- active_frames_bounds, test_mask, n_px_per_frame, load_depth, load_flow and
-    the all_* arrays -- and never calls its sample().  On each call the resident frames follow active_frames_bounds:
+    the all_* arrays -- and never calls its sample().  A DeviceFrameDataset has no all_* arrays: it converts each new
+    frame into its slot on the device (lrf_ingest_frame), with the same result.  On each call the resident frames follow active_frames_bounds:
     new frames are uploaded (each through a fresh pinned buffer of torch's caching host allocator, which is not
     reused before its copy has finished), frames below the first active one are forgotten.  Frame f lives in slot
     f % capacity of a ring of frame slots.  The ring grows, to max(span, 2 * capacity) slots with a device copy of
@@ -77,7 +78,13 @@ class DeviceRaySampler:
         self._cstore = s
 
     def _upload(self, f, b0):
-        """Enqueues frame f (rows (f - b0) * n_px of the dataset's arrays) into its slot."""
+        """Enqueues frame f (rows (f - b0) * n_px of the dataset's arrays) into its slot; a DeviceFrameDataset
+        converts the frame's raw pixels into the slot instead."""
+        slot = f % self.capacity
+        if isinstance(self.ds, DeviceFrameDataset):
+            self.ds.ingest_frame(f, self._cstore, slot, self.dev)
+            self.store["slot_frame"][slot].fill_(f)
+            return
         stage = torch.empty(self.n_px * self.floats_per_px, dtype=torch.float32, pin_memory=True)
         host = stage.numpy()
         rows = slice((f - b0) * self.n_px, (f - b0 + 1) * self.n_px)
@@ -87,7 +94,6 @@ class DeviceRaySampler:
             host[off:off + n] = getattr(self.ds, attr)[rows].reshape(-1)
             parts.append((key, off, n))
             off += n
-        slot = f % self.capacity
         for key, o, n in parts:
             dst = self.store[key][slot]
             dst.copy_(stage[o:o + n].view(dst.shape), non_blocking=True)
@@ -161,3 +167,196 @@ class DeviceRaySampler:
             _lib.check(_lib.lib().lrf_gather_rays(C.byref(self._cstore), C.byref(g), _stream(dev)))
         blob.update(idx=idx, view_ids=ids[:V], train_test_poses=train_test_poses, view_ids_host=view_ids)
         return blob
+
+
+class DeviceFrameDataset:
+    """The train split of LocalRFDataset (dataLoader/localrf_dataset.py) with its frames converted on the device.
+
+    Same constructor and the same state train.py reads -- img_wh, num_images, active_frames_bounds, test_mask,
+    n_px_per_frame, load_depth / load_flow, activate_frames, deactivate_frames, has_left_frames, get_frame_fbase,
+    all_fbases, all_image_paths, and with preprocessed poses transforms, first_pose, rel_poses, pose_scale.  Frames are
+    read `frames_chunk` at a time from the same files, with the same fallbacks (masks/all.png, the frame_step flow
+    names) and joblib threads, as read_meta reads them; but only the decoded 8-bit image, 16-bit inverse depth,
+    16-bit encoded flows and 8-bit motion mask are kept, in pinned host memory, until a DeviceRaySampler places the
+    frame in its ring: then they are uploaded (with flow and depth 8 bytes per output pixel when the flows are at
+    half size, 17 when they are at the image size, against the 44 bytes per pixel of float32 the reference builds
+    and keeps) and lrf_ingest_frame writes the slot, bit-identical to the
+    arrays read_meta builds.  The host keeps no float copy of any frame, and a frame's raw bytes are dropped once its
+    upload is enqueued.  There is no `sample`: draw batches with DeviceRaySampler(dataset, device).
+
+    Supported layouts (anything else raises NotImplementedError; such datasets keep using LocalRFDataset): the
+    image at its size or reduced by downsampling = 2 or 4 when both sides divide; inverse depth at the image size, a
+    reduction of it by 2 or 4, or smaller; flows at the image size or smaller on both axes (scripts/run_flow.py
+    writes them at half size), both flows of one frame the same size; motion masks at the image size.
+    """
+
+    def __init__(self, datadir, split="train", frames_chunk=20, downsampling=-1, load_depth=False, load_flow=False,
+                 with_preprocessed_poses=False, n_init_frames=7, subsequence=[0, -1], test_frame_every=10,
+                 frame_step=1):
+        import json
+        import os
+        if split != "train":
+            raise ValueError("DeviceFrameDataset is the train split; the test split is LocalRFDataset's")
+        self.root_dir, self.split = datadir, split
+        self.frames_chunk = max(frames_chunk, n_init_frames)
+        self.downsampling = downsampling
+        self.load_depth, self.load_flow = load_depth, load_flow
+        self.frame_step = frame_step
+        if with_preprocessed_poses:
+            with open(os.path.join(datadir, "transforms.json"), "r") as fh:
+                self.transforms = json.load(fh)
+            by_name = {os.path.basename(m["file_path"]): m["transform_matrix"] for m in self.transforms["frames"]}
+            paths = sorted(by_name)
+            poses = [np.array(by_name[p], dtype=np.float32) for p in paths]
+            self.first_pose = np.array(by_name[paths[0]], dtype=np.float32)
+            rel = np.stack([np.eye(4, dtype=np.float32)] +
+                           [np.linalg.inv(poses[i - 1]) @ poses[i] for i in range(1, len(poses))], axis=0)
+            self.pose_scale = 2e-2 / np.median(np.linalg.norm(rel[:, :3, 3], axis=-1))
+            rel[:, :3, 3] *= self.pose_scale
+            self.rel_poses = rel[::frame_step]
+        else:
+            paths = sorted(os.listdir(os.path.join(datadir, "images")))
+        if subsequence != [0, -1]:
+            paths = paths[subsequence[0]:subsequence[1]]
+        self.image_paths = self.all_image_paths = paths[::frame_step]
+        test = []
+        for i, p in enumerate(self.image_paths):
+            fbase = os.path.splitext(p)[0]
+            index = int(fbase) if fbase.isnumeric() else i
+            test.append(1 if test_frame_every > 0 and index % test_frame_every == 0 else 0)
+        self.test_mask = np.array(test)
+        self.num_images = len(self.image_paths)
+        self.all_fbases = {os.path.splitext(p)[0]: i for i, p in enumerate(self.image_paths)}
+        self.white_bg = False
+        self.near_far = [0.1, 1e3]
+        self.scene_bbox = 2 * torch.tensor([[-1.0, -1.0, -1.0], [1.0, 1.0, 1.0]])
+        self._raw = {}                                 # frame -> its decoded planes (pinned), until ingested
+        self._scratch = {}                             # device -> scratch of lrf_ingest_frame
+        self.active_frames_bounds = [0, 0]
+        self.loaded_frames = 0
+        self.activate_frames(n_init_frames)
+
+    def activate_frames(self, n_frames=1):
+        b = self.active_frames_bounds
+        b[1] = min(b[1] + n_frames, self.num_images)
+        if b[1] > self.loaded_frames:
+            self._read_chunk()
+
+    def has_left_frames(self):
+        return self.active_frames_bounds[1] < self.num_images
+
+    def deactivate_frames(self, first_frame):
+        self.active_frames_bounds[0] = first_frame
+        for f in [f for f in self._raw if f < first_frame]:
+            del self._raw[f]
+
+    def get_frame_fbase(self, view_id):
+        return list(self.all_fbases.keys())[view_id]
+
+    def _paths(self, i):
+        import os
+        name = self.image_paths[i]
+        base = os.path.splitext(name)[0]
+        mask = os.path.join(self.root_dir, "masks", f"{base}.png")
+        if not os.path.isfile(mask):
+            mask = os.path.join(self.root_dir, "masks/all.png")
+        out = {"image": os.path.join(self.root_dir, "images", name), "mask": mask,
+               "invdepth": os.path.join(self.root_dir, "depth", f"{base}.png")}
+        g = self.all_image_paths.index(name)
+        nxt = os.path.splitext(self.all_image_paths[g + 1 if g + 1 < len(self.all_image_paths) else 0])[0]
+        step = f"step{self.frame_step}_" if self.frame_step != 1 else ""
+        out["fwd_flow"] = os.path.join(self.root_dir, "flow_ds", f"fwd_{step}{nxt}.png")
+        out["bwd_flow"] = os.path.join(self.root_dir, "flow_ds", f"bwd_{step}{base}.png")
+        return out
+
+    def _read(self, i):
+        """The decoded planes of frame i, each in a pinned buffer: image uint8 [h0][w0][3] BGR, invdepth uint16,
+        flows uint16 [hf][wf][3] as stored, mask uint8 (or None)."""
+        import os
+        import cv2
+        p = self._paths(i)
+        planes = {"image": cv2.imread(p["image"])}
+        if self.load_depth:
+            d = cv2.imread(p["invdepth"], -1)
+            if d.ndim != 2 or d.dtype not in (np.uint8, np.uint16):
+                raise NotImplementedError(f"{p['invdepth']}: inverse depth must be an 8- or 16-bit single-channel "
+                                          "image")
+            planes["invdepth"] = d.astype(np.uint16)
+        if self.load_flow:
+            for key in ("fwd_flow", "bwd_flow"):
+                e = cv2.imread(p[key], cv2.IMREAD_UNCHANGED)
+                if e.ndim != 3 or e.shape[2] != 3 or e.dtype != np.uint16:
+                    raise NotImplementedError(f"{p[key]}: encoded flow must be a 16-bit 3-channel image")
+                planes[key] = e
+        if os.path.isfile(p["mask"]):
+            m = cv2.imread(p["mask"], cv2.IMREAD_UNCHANGED)
+            if m.ndim != 2:
+                m = m[..., 0]
+            planes["mask"] = m if m.dtype == np.uint8 else (m > 0).astype(np.uint8)
+        pinned = {}
+        for key, a in planes.items():
+            t = torch.empty(a.shape, dtype=torch.uint8 if a.dtype == np.uint8 else torch.int16, pin_memory=True)
+            t.numpy().view(a.dtype)[...] = a
+            pinned[key] = t
+        return pinned
+
+    def _layout(self, raw):
+        """-> (w, h) of the frame after downsampling; raises NotImplementedError for an unsupported layout."""
+        h0, w0 = raw["image"].shape[:2]
+        k = 1 if self.downsampling == -1 else self.downsampling
+        if k not in (1, 2, 4) or w0 % k or h0 % k:
+            raise NotImplementedError(f"downsampling={self.downsampling} of a {w0}x{h0} image: only 2 and 4 of "
+                                      "sides they divide are converted on the device")
+        return w0 // int(k), h0 // int(k)
+
+    def _read_chunk(self):
+        from joblib import Parallel, delayed
+        n = min(self.frames_chunk, self.num_images - self.loaded_frames)
+        lo = self.loaded_frames
+        frames = Parallel(n_jobs=-1, backend="threading")(delayed(self._read)(i) for i in range(lo, lo + n))
+        self.loaded_frames += n
+        w, h = self._layout(frames[0])
+        for raw in frames:
+            if self._layout(raw) != (w, h):
+                raise NotImplementedError("frames of one dataset must share their size")
+        self.img_wh = [w, h]
+        self.n_px_per_frame = w * h
+        for i, raw in enumerate(frames):
+            self._raw[lo + i] = raw
+
+    def ingest_frame(self, f, store, slot, device):
+        """Uploads frame f's raw planes and enqueues lrf_ingest_frame into `slot` of `store` (an LrfFrameStore) on
+        the current stream of `device`; drops the host planes (torch's caching host allocator keeps a pinned block
+        from reuse until its copy has finished)."""
+        raw = self._raw.pop(f, None)
+        if raw is None:
+            raise RuntimeError(f"frame {f} is not loaded or was already placed in a ring (a DeviceFrameDataset "
+                               "hands each frame to one DeviceRaySampler)")
+        dev = torch.device(device)
+        w, h = self.img_wh
+        fr = _lib.LrfIngestFrame()
+        fr.slot, fr.w, fr.h = slot, w, h
+        with torch.cuda.device(dev):
+            up = {k: t.to(dev, non_blocking=True) for k, t in raw.items()}
+            img = up["image"]
+            fr.image, fr.h0, fr.w0, fr.image_stride = _ptr(img).value, img.shape[0], img.shape[1], img.shape[1] * 3
+            if "invdepth" in up:
+                d = up["invdepth"]
+                fr.invdepth, fr.hd, fr.wd, fr.invdepth_stride = _ptr(d).value, d.shape[0], d.shape[1], d.shape[1]
+            if "fwd_flow" in up:
+                a, b = up["fwd_flow"], up["bwd_flow"]
+                if a.shape != b.shape:
+                    raise NotImplementedError(f"frame {f}: the forward and backward flows differ in size")
+                fr.fwd_flow, fr.bwd_flow = _ptr(a).value, _ptr(b).value
+                fr.hf, fr.wf, fr.flow_stride = a.shape[0], a.shape[1], a.shape[1] * 3
+                fr.flow_scale = float(np.float32(h / a.shape[0]))
+            if "mask" in up:
+                m = up["mask"]
+                fr.mask, fr.hm, fr.wm, fr.mask_stride = _ptr(m).value, m.shape[0], m.shape[1], m.shape[1]
+            L = _lib.lib()
+            n = L.lrf_ingest_scratch_bytes(w * h)
+            s = self._scratch.get(dev)
+            if s is None or s.numel() < n:
+                s = self._scratch[dev] = torch.empty(max(n, 8), dtype=torch.uint8, device=dev)
+            _lib.check(L.lrf_ingest_frame(C.byref(store), C.byref(fr), C.c_void_p(_ptr(s).value), s.numel(),
+                                          _stream(dev)))
