@@ -524,6 +524,27 @@ size_t lrf_ingest_scratch_bytes(int64_t n_px);
 int lrf_ingest_frame(const LrfFrameStore *store, const LrfIngestFrame *frame, void *scratch, size_t scratch_bytes,
                      lrf_stream_t stream);
 
+/* A held-out frame's ground truth at the render size.  replaces: renderer.py:157, `gt_rgb = cv2.resize(gt_rgb, (W,
+ * H))` (INTER_LINEAR) of the test split's float32 rgb.  src is w0 x h0, dst W x H, 3 floats per pixel, row strides
+ * in floats; both device or pinned host memory, not overlapping.  dst equals OpenCV's portable implementation,
+ * cv2.resize(src, (W, H)) with IPP disabled (and on builds without IPP), bit for bit:
+ *   - the same size is a copy;
+ *   - w0 == 2 W and h0 == 2 H is INTER_AREA, as OpenCV switches it: (((a + b) + c) + d) * 0.25 in row-major order,
+ *     the 2x block sum of lrf_ingest_frame;
+ *   - anything else is separable linear: per column, scale_x = 1 / ((double)W / w0), fx = (float)((x + 0.5) scale_x
+ *     - 0.5) in double, sx = floor(fx), fx -= sx in float; sx < 0 gives sx = 0, fx = 0; a column with sx + 1 >= w0
+ *     copies pixel min(sx, w0 - 1) of the row, the others are S[sx] (1 - fx) + S[sx + 1] fx.  Rows take fy the same
+ *     way without the reset: rows clamp(sy) and clamp(sy + 1) into [0, h0) blended by (1 - fy, fy), the horizontal
+ *     results rounded to float first.  Every product and sum rounds once (no FMA).
+ * Difference from an IPP build (the opencv-python wheels; IPP picks its code path from the host CPU), measured with
+ * IPP 2022.2.0's AVX-512 path on values in [0, 1): at 2x, at most 2 ulp (5.96e-8) on about a fifth of the values at
+ * 960x540 -> 480x270; at other ratios up to 3.3e-5 (963x541 -> 481x270) and 6.9e-5 (1921x1081 -> 960x540).
+ * One launch, one thread per output pixel, no host synchronisation, bitwise repeatable.  LRF_ERR_INVALID before any
+ * device work for a NULL pointer, a size below 1, w0 h0 or W H at or above 2^31, and a stride below 3 times its
+ * width. */
+int lrf_resize_linear(const float *src, int32_t w0, int32_t h0, int64_t src_stride, float *dst, int32_t W,
+                      int32_t H, int64_t dst_stride, lrf_stream_t stream);
+
 /* Flow and depth comparison panels of one held-out frame.  replaces: renderer.py:79-124, the TensorBoard panels
  * render(test=True) builds for every test frame (get_fwd_bwd_cam2cams / get_pred_flow / compute_depth_loss of
  * utils/utils.py:15-59 and the inline numpy / cv2 lines around them).  The frame is rendered at W x H with

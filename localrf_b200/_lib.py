@@ -143,7 +143,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_image_metrics_scratch_bytes", "lrf_image_metrics", "lrf_supervision_scratch_bytes",
            "lrf_supervision_losses", "lrf_supervision_losses_backward", "lrf_adam_step",
            "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch", "lrf_gather_rays",
-           "lrf_test_panels_scratch_bytes", "lrf_test_panels", "lrf_ingest_scratch_bytes", "lrf_ingest_frame"]
+           "lrf_test_panels_scratch_bytes", "lrf_test_panels", "lrf_ingest_scratch_bytes", "lrf_ingest_frame",
+           "lrf_resize_linear"]
 
 
 def _stale():
@@ -256,6 +257,7 @@ def lib():
     L.lrf_ingest_scratch_bytes.restype = C.c_size_t
     L.lrf_ingest_scratch_bytes.argtypes = [C.c_int64]
     L.lrf_ingest_frame.argtypes = [C.POINTER(LrfFrameStore), C.POINTER(LrfIngestFrame), _vp, C.c_size_t, _vp]
+    L.lrf_resize_linear.argtypes = [_vp, C.c_int32, C.c_int32, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_int64, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

@@ -62,6 +62,8 @@ cudaError_t launch_test_panels(const LrfPanelFrame& f, void* scratch, int n_sms,
 size_t ingest_scratch_bytes(long long n_px);
 int ingest_resize_mode(int ws, int hs, int w, int h);
 cudaError_t launch_ingest_frame(const LrfFrameStore& st, const LrfIngestFrame& f, void* scratch, cudaStream_t stream);
+cudaError_t launch_resize_linear(const float* src, int w0, int h0, long long src_stride, float* dst, int W, int H,
+                                 long long dst_stride, cudaStream_t stream);
 cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
                                 cudaStream_t stream);
 cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
@@ -812,6 +814,18 @@ int lrf_ingest_frame(const LrfFrameStore* s, const LrfIngestFrame* f, void* scra
     return fail(LRF_ERR_UNSUPPORTED, "the flows must be w x h or at most w x h on both axes (an enlargement)");
   if (f->mask && (f->wm != f->w || f->hm != f->h)) return fail(LRF_ERR_UNSUPPORTED, "the mask must be w x h");
   return cuda_status(lrf::launch_ingest_frame(*s, *f, scratch, (cudaStream_t)stream), "ingest_frame");
+}
+
+int lrf_resize_linear(const float* src, int32_t w0, int32_t h0, int64_t src_stride, float* dst, int32_t W, int32_t H,
+                      int64_t dst_stride, lrf_stream_t stream) {
+  if (!src || !dst) return fail(LRF_ERR_INVALID, "src / dst is NULL");
+  if (w0 < 1 || h0 < 1 || W < 1 || H < 1) return fail(LRF_ERR_INVALID, "w0, h0, W and H must be >= 1");
+  if ((int64_t)w0 * h0 >= 2147483648LL || (int64_t)W * H >= 2147483648LL)
+    return fail(LRF_ERR_INVALID, "w0 h0 and W H must be below 2^31");
+  if (src_stride < 3 * (int64_t)w0) return fail(LRF_ERR_INVALID, "src_stride must be >= 3 w0");
+  if (dst_stride < 3 * (int64_t)W) return fail(LRF_ERR_INVALID, "dst_stride must be >= 3 W");
+  return cuda_status(lrf::launch_resize_linear(src, w0, h0, src_stride, dst, W, H, dst_stride, (cudaStream_t)stream),
+                     "resize_linear_kernel");
 }
 
 int lrf_peer_barrier(unsigned long long* const* peer_flags, int32_t rank, int32_t world,

@@ -240,6 +240,54 @@ __global__ void __launch_bounds__(INGEST_THREADS) depth_kernel(const LrfIngestFr
   out[p] = d;
 }
 
+// One row or column coefficient of cv2's INTER_LINEAR: f = float((d + 0.5) scale - 0.5) in double, s = floor(f),
+// f -= s in float.  Each double step rounds once (no DFMA), as the host computes it.
+__device__ __forceinline__ void linear_coeff(int d, double scale, int& s, float& f) {
+  f = __double2float_rn(__dadd_rn(__dmul_rn(d + 0.5, scale), -0.5));
+  s = (int)floorf(f);
+  f = __fsub_rn(f, (float)s);
+}
+
+// cv2.resize(src, (W, H)) of a 3-channel float32 image without IPP (include/localrf_b200.h, lrf_resize_linear):
+// mode 1 copies, mode 2 is the exact 2x reduction (INTER_AREA, the same block sum as image_kernel), mode 0 is the
+// separable linear rule, the horizontal blend rounded to float before the vertical one.
+__global__ void __launch_bounds__(INGEST_THREADS) resize_linear_kernel(const float* src, int w0, int h0,
+                                                                       long long src_stride, float* dst, int W, int H,
+                                                                       long long dst_stride, int mode, double scale_x,
+                                                                       double scale_y) {
+  const long long p = (long long)blockIdx.x * INGEST_THREADS + threadIdx.x;
+  if (p >= (long long)W * H) return;
+  const int x = (int)(p % W), y = (int)(p / W);
+  float* out = dst + y * dst_stride + 3 * x;
+  if (mode == 1) {
+    for (int c = 0; c < 3; ++c) out[c] = src[y * src_stride + 3 * x + c];
+    return;
+  }
+  if (mode == 2) {
+    for (int c = 0; c < 3; ++c) {
+      auto v = [&](int dy, int dx) { return src[(long long)(2 * y + dy) * src_stride + 3 * (2 * x + dx) + c]; };
+      out[c] = reduce_block(2, v);
+    }
+    return;
+  }
+  int sx, sy;
+  float fx, fy;
+  linear_coeff(x, scale_x, sx, fx);
+  if (sx < 0) sx = 0, fx = 0.f;
+  const bool copy = sx + 1 >= w0;                         // cv2's xmax: every later column copies too
+  if (copy) sx = w0 - 1;
+  linear_coeff(y, scale_y, sy, fy);                       // rows are not reset at the borders
+  const int sy0 = min(max(sy, 0), h0 - 1), sy1 = min(max(sy + 1, 0), h0 - 1);
+  const float ax = __fsub_rn(1.f, fx), ay = __fsub_rn(1.f, fy);
+  const float* r0 = src + sy0 * src_stride + 3 * sx;
+  const float* r1 = src + sy1 * src_stride + 3 * sx;
+  for (int c = 0; c < 3; ++c) {
+    const float h0v = copy ? r0[c] : __fadd_rn(__fmul_rn(r0[c], ax), __fmul_rn(r0[3 + c], fx));
+    const float h1v = copy ? r1[c] : __fadd_rn(__fmul_rn(r1[c], ax), __fmul_rn(r1[3 + c], fx));
+    out[c] = __fadd_rn(__fmul_rn(h0v, ay), __fmul_rn(h1v, fy));
+  }
+}
+
 // Scratch layout (bytes): stats [2] fp32 at 0 (mean, variance), the Laplacian [n] fp32 at 16, the tree's slot sums
 // [2^D] fp32, its flags [2^D] u8, the grey image [n] u8.
 struct Scratch {
@@ -330,6 +378,16 @@ cudaError_t launch_ingest_frame(const LrfFrameStore& st, const LrfIngestFrame& f
   if (st.invdepth)
     depth_kernel<<<blocks, INGEST_THREADS, 0, stream>>>(f, resize_mode(f.wd, f.hd, f.w, f.h),
                                                         (float*)st.invdepth + at);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_resize_linear(const float* src, int w0, int h0, long long src_stride, float* dst, int W, int H,
+                                 long long dst_stride, cudaStream_t stream) {
+  const int mode = (w0 == W && h0 == H) ? 1 : (w0 == 2 * W && h0 == 2 * H) ? 2 : 0;
+  const double scale_x = 1.0 / ((double)W / w0), scale_y = 1.0 / ((double)H / h0);
+  const long long n = (long long)W * H;
+  resize_linear_kernel<<<(unsigned)((n + INGEST_THREADS - 1) / INGEST_THREADS), INGEST_THREADS, 0, stream>>>(
+      src, w0, h0, src_stride, dst, W, H, dst_stride, mode, scale_x, scale_y);
   return cudaGetLastError();
 }
 

@@ -30,8 +30,8 @@ class DeviceRaySampler:
     """LocalRFDataset.sample with the active frames resident on `device`.
 
     Reads only the dataset's state -- active_frames_bounds, test_mask, n_px_per_frame, load_depth, load_flow and
-    the all_* arrays -- and never calls its sample().  A DeviceFrameDataset has no all_* arrays: it converts each new
-    frame into its slot on the device (lrf_ingest_frame), with the same result.  On each call the resident frames follow active_frames_bounds:
+    the all_* arrays -- and never calls its sample().  A train-split DeviceFrameDataset has no all_* arrays: it
+    converts each new frame into its slot on the device (lrf_ingest_frame), with the same result.  On each call the resident frames follow active_frames_bounds:
     new frames are uploaded (each through a fresh pinned buffer of torch's caching host allocator, which is not
     reused before its copy has finished), frames below the first active one are forgotten.  Frame f lives in slot
     f % capacity of a ring of frame slots.  The ring grows, to max(span, 2 * capacity) slots with a device copy of
@@ -40,9 +40,14 @@ class DeviceRaySampler:
 
     Memory: 4 * (3 + 1 + 1 + 2 + 1 + 2 + 1) = 44 bytes per pixel with depth and flow on -- 22.8 MB per 960x540
     frame, 28.2 MB per 800x800 frame, 2.3-2.8 GB for 100 slots.  The reference holds the same data on the host.
+    The test split (DeviceFrameDataset(split="test"), which this sampler refuses with ValueError, as the reference
+    never samples it) holds every test frame the same way without the loss weight: 40 bytes per pixel.
     """
 
     def __init__(self, dataset, device, capacity=None):
+        if isinstance(dataset, DeviceFrameDataset) and dataset.split != "train":
+            raise ValueError(f"DeviceRaySampler draws from the train split, not the {dataset.split} split (the "
+                             "reference never samples the test split)")
         self.ds = dataset
         self.dev = torch.device(device)
         if self.dev.type != "cuda":
@@ -170,7 +175,7 @@ class DeviceRaySampler:
 
 
 class DeviceFrameDataset:
-    """The train split of LocalRFDataset (dataLoader/localrf_dataset.py) with its frames converted on the device.
+    """LocalRFDataset (dataLoader/localrf_dataset.py), train or test split, with its frames converted on the device.
 
     Same constructor and the same state train.py reads -- img_wh, num_images, active_frames_bounds, test_mask,
     n_px_per_frame, load_depth / load_flow, activate_frames, deactivate_frames, has_left_frames, get_frame_fbase,
@@ -184,6 +189,21 @@ class DeviceFrameDataset:
     arrays read_meta builds.  The host keeps no float copy of any frame, and a frame's raw bytes are dropped once its
     upload is enqueued.  There is no `sample`: draw batches with DeviceRaySampler(dataset, device).
 
+    split="test" is the reference's test split: the frames with index % test_frame_every == 0, all read and
+    converted at construction on `device` (the current CUDA device by default; the train split's frames go to its
+    sampler's device instead) into the stacked float32 CUDA tensors the reference builds with np.stack: all_rgbs
+    [N,h,w,3], all_invdepths [N,h,w] (load_depth), all_fwd_flow / all_bwd_flow [N,h,w,2] and all_fwd_mask /
+    all_bwd_mask [N,h,w] (load_flow), None where the reference's are; all_loss_weights is None, as there.  Each
+    frame's decoded planes go through lrf_ingest_frame exactly as a train frame's do, so its arrays are
+    bit-identical to read_meta's, and are dropped once its upload is enqueued; the loss weight, which the reference
+    computes and discards, is written to one shared scratch plane that is freed with the ingest scratch after
+    construction.  img_wh, n_px_per_frame, num_images, all_fbases, get_frame_fbase and test_mask (over every frame,
+    as in the reference) are there; active_frames_bounds = [0, min(n_init_frames, N)], loaded_frames = N and
+    has_left_frames() keep the reference's values.  A DeviceRaySampler refuses this split.  Device memory: 4 * (3 +
+    1 + 2 + 1 + 2 + 1) = 40 bytes per pixel and test frame with flow and depth (12 with neither), 20.7 MB per
+    960x540 frame, 2.07 GB for 100 such frames; during construction 4 bytes per pixel more, once, plus
+    lrf_ingest_scratch_bytes.  The host keeps no float copy (the reference keeps the same 40 B/px in numpy arrays).
+
     Supported layouts (anything else raises NotImplementedError; such datasets keep using LocalRFDataset): the
     image at its size or reduced by downsampling = 2 or 4 when both sides divide; inverse depth at the image size, a
     reduction of it by 2 or 4, or smaller; flows at the image size or smaller on both axes (scripts/run_flow.py
@@ -192,11 +212,11 @@ class DeviceFrameDataset:
 
     def __init__(self, datadir, split="train", frames_chunk=20, downsampling=-1, load_depth=False, load_flow=False,
                  with_preprocessed_poses=False, n_init_frames=7, subsequence=[0, -1], test_frame_every=10,
-                 frame_step=1):
+                 frame_step=1, device=None):
         import json
         import os
-        if split != "train":
-            raise ValueError("DeviceFrameDataset is the train split; the test split is LocalRFDataset's")
+        if split not in ("train", "test"):
+            raise ValueError(f"DeviceFrameDataset is the train or the test split, got split={split!r}")
         self.root_dir, self.split = datadir, split
         self.frames_chunk = max(frames_chunk, n_init_frames)
         self.downsampling = downsampling
@@ -225,6 +245,16 @@ class DeviceFrameDataset:
             index = int(fbase) if fbase.isnumeric() else i
             test.append(1 if test_frame_every > 0 and index % test_frame_every == 0 else 0)
         self.test_mask = np.array(test)
+        if split == "test":
+            self.image_paths = [p for p, t in zip(self.image_paths, test) if t]
+            self.frames_chunk = len(self.image_paths)
+            dev = torch.device("cuda" if device is None else device)
+            if dev.type != "cuda" or not torch.cuda.is_available():
+                raise RuntimeError("DeviceFrameDataset keeps the test split on a CUDA device (there is no CPU "
+                                   "fallback)")
+            self.device = dev if dev.index is not None else torch.device("cuda", torch.cuda.current_device())
+            self.all_rgbs = self.all_invdepths = self.all_loss_weights = None
+            self.all_fwd_flow = self.all_fwd_mask = self.all_bwd_flow = self.all_bwd_mask = None
         self.num_images = len(self.image_paths)
         self.all_fbases = {os.path.splitext(p)[0]: i for i, p in enumerate(self.image_paths)}
         self.white_bg = False
@@ -323,6 +353,35 @@ class DeviceFrameDataset:
         self.n_px_per_frame = w * h
         for i, raw in enumerate(frames):
             self._raw[lo + i] = raw
+        if self.split == "test":
+            self._ingest_test_split(lo, n)
+
+    def _ingest_test_split(self, lo, n):
+        """Converts frames [lo, lo + n) -- the whole test split, read at once -- into the stacked all_* tensors: each
+        through lrf_ingest_frame into a one-slot store whose pointers are the frame's rows."""
+        dev = self.device
+        w, h = self.img_wh
+        with torch.cuda.device(dev):
+            new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
+            self.all_rgbs = new(n, h, w, 3)
+            if self.load_depth:
+                self.all_invdepths = new(n, h, w)
+            if self.load_flow:
+                self.all_fwd_flow, self.all_fwd_mask = new(n, h, w, 2), new(n, h, w)
+                self.all_bwd_flow, self.all_bwd_mask = new(n, h, w, 2), new(n, h, w)
+            weight = new(w * h)                        # the loss weight, computed and discarded as in the reference
+            slot_frame = torch.full((1,), -1, dtype=torch.int64, device=dev)
+            for k in range(n):
+                s = _lib.LrfFrameStore()
+                s.n_px, s.capacity = w * h, 1
+                s.slot_frame, s.loss_weight = _ptr(slot_frame).value, _ptr(weight).value
+                for field, attr in (("rgb", "all_rgbs"), ("invdepth", "all_invdepths"), ("fwd_flow", "all_fwd_flow"),
+                                    ("fwd_mask", "all_fwd_mask"), ("bwd_flow", "all_bwd_flow"),
+                                    ("bwd_mask", "all_bwd_mask")):
+                    t = getattr(self, attr)
+                    setattr(s, field, _ptr(t[k]).value if t is not None else None)
+                self.ingest_frame(lo + k, s, 0, dev)
+            self._scratch.pop(dev, None)   # freed blocks are reused on this stream only, after the queued launches
 
     def ingest_frame(self, f, store, slot, device):
         """Uploads frame f's raw planes and enqueues lrf_ingest_frame into `slot` of `store` (an LrfFrameStore) on

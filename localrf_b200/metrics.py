@@ -8,6 +8,8 @@ arithmetic: fp32 squares and cross products, an fp64 separable Gaussian filter a
     rgb_ssim(img0, img1, max_val)   -> the reference's function (numpy in, float / numpy map out), on the GPU
     test_panels(depth, directions, ...) -> the flow and depth comparison panels of renderer.py:79-124
                                        (lrf_test_panels), device tensors, no host synchronisation
+    resize_linear(src, W, H)        -> cv2.resize(src, (W, H)) of a held-out frame's ground truth (renderer.py:157)
+                                       as OpenCV computes it without IPP (lrf_resize_linear), no synchronisation
 
 `renderer.rgb_ssim = localrf_b200.metrics.rgb_ssim` puts it into the reference's renderer.  There is no CPU
 fallback: without a CUDA device these raise RuntimeError.
@@ -67,6 +69,40 @@ def _enqueue(img, gt, out, ssim_map=None, W=None, max_val=1.0, filter_size=11, f
         _lib.check(L.lrf_image_metrics(_ptr(img), s_img, _ptr(gt), s_gt, H, W_, float(max_val), int(filter_size),
                                        float(filter_sigma), float(k1), float(k2), _ptr(out), _ptr(ssim_map),
                                        _ptr(scratch), int(nbytes), _stream(dev)))
+
+
+def resize_linear(src, W, H, out=None):
+    """cv2.resize(src, (W, H)) as OpenCV computes it without IPP (INTER_LINEAR, exact 2x as INTER_AREA; rules and the
+    documented difference from an IPP build in include/localrf_b200.h, lrf_resize_linear), bit for bit: the ground
+    truth renderer.py:157 resizes for every held-out frame.  src: float32 [h0,w0,3] on a CUDA device or pinned
+    (rows may be further apart than 3 w0 floats).  -> [H,W,3] float32 on src's device (the current CUDA device for a
+    pinned src), or `out` (a CUDA float32 [H,W,3] tensor with 3-float pixels), enqueued without synchronising."""
+    W, H = int(W), int(H)
+    if not isinstance(src, torch.Tensor):
+        raise TypeError(f"src must be a torch tensor, got {type(src).__name__}")
+    if src.dtype != torch.float32:
+        raise TypeError(f"src must be float32, got {src.dtype}")
+    if not (src.is_cuda or src.is_pinned()):
+        raise ValueError("src must be a CUDA tensor or a pinned host tensor")
+    if src.dim() != 3 or src.shape[2] != 3:
+        raise ValueError(f"src must be [h0,w0,3], got {tuple(src.shape)}")
+    h0, w0 = int(src.shape[0]), int(src.shape[1])
+    if not (src.stride(2) == 1 and src.stride(1) == 3 and (h0 == 1 or src.stride(0) >= 3 * w0)):
+        src = src.contiguous() if src.is_cuda else src.contiguous().pin_memory()
+    s_src = src.stride(0) if h0 > 1 else 3 * w0
+    dev = _device_of(src, *(() if out is None else (out,)))
+    if out is None:
+        out = torch.empty(H, W, 3, dtype=torch.float32, device=dev)
+    elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.dtype == torch.float32 and
+              tuple(out.shape) == (H, W, 3) and out.stride(2) == 1 and out.stride(1) == 3 and
+              (H == 1 or out.stride(0) >= 3 * W)):
+        raise ValueError(f"out must be a CUDA float32 [{H},{W},3] tensor with 3-float pixels")
+    elif out.device != dev:
+        raise ValueError(f"out is on {out.device} but src is on {dev}")
+    s_out = out.stride(0) if H > 1 else 3 * W
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().lrf_resize_linear(_ptr(src), w0, h0, s_src, _ptr(out), W, H, s_out, _stream(dev)))
+    return out
 
 
 def _device_of(*ts):
