@@ -487,7 +487,9 @@ int lrf_gather_rays(const LrfFrameStore *store, const LrfRayGather *g, lrf_strea
  * block in a fixed order (k = 2: ((a + b) + c) + d in row-major order; k = 4: each row in order, then the rows in
  * order), times 1 / k^2, as cv2 does for 3-channel float32 images; an enlargement (source <= w x h on both axes) is
  * cv2's separable area-weighted linear rule in fp32, horizontal then vertical, rounded to nearest even and saturated
- * for uint16.  Any other ratio is LRF_ERR_UNSUPPORTED. */
+ * for uint16; its weights are formed in double as cv2 forms them, the product and the difference each rounded once
+ * (never fused), so a weight that is exactly 0 there is exactly 0 here.  An enlargement by an integer factor has
+ * only such weights: it repeats the source pixel.  Any other ratio is LRF_ERR_UNSUPPORTED. */
 typedef struct LrfIngestFrame {
   int64_t slot;                /* 0 <= slot < store->capacity; the caller tags slot_frame */
   int32_t w, h;                /* the frame's size: w h == store->n_px */
@@ -508,8 +510,12 @@ typedef struct LrfIngestFrame {
   int64_t mask_stride;         /* >= wm */
 } LrfIngestFrame;
 
-/* Device scratch bytes of one frame of n_px pixels (8-byte aligned); 0 if n_px < 1 or the frame is too large (the
- * variance's summation tree is built for up to 2^16 leaves of 128 pixels, a little over 8.3 M pixels). */
+/* Device scratch bytes of one frame of n_px pixels (8-byte aligned); 0 if n_px < 1 or the frame is too large: the
+ * variance's summation tree is built for 16 halvings of numpy's recursion, which splits a run at half its length
+ * rounded down to a multiple of 8.  2^16 leaves of 128 pixels (8 388 608) is the largest frame taken; an uneven split
+ * leaves the longer half up to 7 values more at each level, so some smaller frames need a 17th halving and are
+ * refused as well (4096 x 2048 - 1 is one; 3840 x 2160 is taken; every frame up to 7 864 328 pixels is, 7 864 329
+ * is the smallest refused). */
 size_t lrf_ingest_scratch_bytes(int64_t n_px);
 /* Writes rgb, loss_weight and, when the store has them, invdepth, the flows and the flow masks of slot `slot`
  * (through the store's pointers, which must be writable here).  loss_weight = the variance of the 4-neighbour
@@ -520,7 +526,9 @@ size_t lrf_ingest_scratch_bytes(int64_t n_px);
  * without slot_frame, rgb or loss_weight, a partly given flow group, a slot outside [0, capacity), w h != n_px, a
  * plane sized below 1 or with a short stride, a NULL plane of a group the store has or a plane of a group it lacks,
  * and scratch not 8-byte aligned or smaller than lrf_ingest_scratch_bytes(n_px); LRF_ERR_UNSUPPORTED for the
- * ratios above and frames too large for the scratch. */
+ * ratios above and frames too large for the scratch.  Rows may be further apart than their width and planes need
+ * not start their allocation; only the slot's rows of the store and the first lrf_ingest_scratch_bytes(n_px) bytes
+ * of the scratch are written, and a scratch last used for another frame or size gives the same bits as a fresh one. */
 int lrf_ingest_frame(const LrfFrameStore *store, const LrfIngestFrame *frame, void *scratch, size_t scratch_bytes,
                      lrf_stream_t stream);
 

@@ -39,12 +39,14 @@ int resize_mode(int ws, int hs, int w, int h) {
   return (ws <= w && hs <= h) ? 0 : -1;
 }
 
-// cv2's INTER_AREA enlargement weights along one axis: source index and the next index's weight.
+// cv2's INTER_AREA enlargement weights along one axis: source index and the next index's weight.  The product and
+// the difference each round once in double, as the host computes them: a DFMA would leave a residue of a few 1e-16
+// where the weight is exactly 0 (6 -> 8 at d = 3), which a zero sample next to a large one shows in fp32.
 __device__ __forceinline__ void area_weight(int d, int dst, int src, int& s, float& f) {
   const double inv_scale = (double)dst / src;
   const double scale = 1.0 / inv_scale;
-  s = (int)floor(d * scale);
-  f = (float)((d + 1) - (s + 1) * inv_scale);
+  s = (int)floor(__dmul_rn((double)d, scale));
+  f = __double2float_rn(__dsub_rn((double)(d + 1), __dmul_rn((double)(s + 1), inv_scale)));
   f = f <= 0.f ? 0.f : __fsub_rn(f, floorf(f));
   if (s >= src - 1) s = src - 1, f = 0.f;
 }

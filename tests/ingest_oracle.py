@@ -147,20 +147,22 @@ def variance(x):
     return F32(pairwise_sum((d * d).astype(F32)) / n)
 
 
-def loss_weight(img, mask=None):
-    """float32 [h][w]: the Laplacian variance of the frame, zero where a motion mask is off."""
-    v = variance(laplacian(gray(img)))
+def loss_weight(img, mask=None, numpy_var=False):
+    """float32 [h][w]: the Laplacian variance of the frame, zero where a motion mask is off.  numpy_var takes the
+    variance from numpy's own .var() (which `variance` restates in Python, too slowly for large frames)."""
+    lap = laplacian(gray(img))
+    v = lap.var() if numpy_var else variance(lap)
     w = np.full(img.shape[:2], v, F32)
     return w if mask is None else (w * mask).astype(F32)
 
 
-def frame(bgr, k=1, depth=None, fwd=None, bwd=None, mask=None):
+def frame(bgr, k=1, depth=None, fwd=None, bwd=None, mask=None, numpy_var=False):
     """Every array read_meta builds for one frame, as a dict of float32 [n_px](w) arrays keyed as in a blob."""
     img = image(bgr, k)
     h, w = img.shape[:2]
     out = {"rgbs": img.reshape(-1, 3)}
     m = motion(mask, h, w) if mask is not None else None
-    out["loss_weights"] = loss_weight(img, m).reshape(-1, 1)
+    out["loss_weights"] = loss_weight(img, m, numpy_var).reshape(-1, 1)
     if depth is not None:
         out["invdepths"] = invdepth(depth, h, w).reshape(-1, 1)
     if fwd is not None:

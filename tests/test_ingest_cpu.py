@@ -53,27 +53,88 @@ def test_gray_is_the_15_bit_conversion():
         assert np.array_equal(io.gray(img), cv2.cvtColor((img * 255).astype(np.uint8), cv2.COLOR_RGB2GRAY))
 
 
-@pytest.mark.parametrize("hs,ws,h,w", [(15, 20, 30, 40), (135, 240, 270, 480), (13, 17, 41, 37), (20, 20, 20, 20),
-                                       (11, 9, 11, 31), (1, 1, 5, 3), (7, 5, 8, 6)])
-def test_flow(hs, ws, h, w):
-    rng = np.random.default_rng(hs * 100 + ws)
+# (hs, ws, h, w) enlargements: by 2 and by 3 (every area weight is 0: the source pixel is repeated), odd ratios, one
+# axis only, a 1 x 1 source, by 5 / 4 and 3 / 2 (weights .25, .5, .75: exact .5 ties for uint16), and the ratios
+# 6 -> 8, 9 -> 12, 10 -> 14 and 14 -> 16 on each axis and 720 x 405 -> 960 x 540, where some area weight is exactly 0
+# in double arithmetic (a fused multiply-add would leave about 1e-16 in its place).
+ENLARGEMENTS = [(15, 20, 30, 40), (10, 10, 30, 30), (13, 17, 41, 37), (11, 9, 11, 31), (1, 1, 5, 3), (7, 5, 8, 6),
+                (12, 16, 15, 20), (10, 14, 15, 21), (6, 6, 8, 8), (9, 6, 12, 8), (10, 9, 14, 12), (14, 10, 16, 14),
+                (6, 14, 8, 16), (405, 720, 540, 960)]
+
+
+def extreme_planes(hs, ws, seed):
+    """uint16 [hs][ws] planes of zeros next to 65535: alternating columns, alternating rows (each in both phases)
+    and a seeded mixture -- where a weight that should be exactly 0 or 1 shows in the result."""
+    cols, rows = np.zeros((hs, ws), np.uint16), np.zeros((hs, ws), np.uint16)
+    cols[:, 1::2] = rows[1::2] = 65535
+    mix = (np.random.default_rng(seed).integers(0, 2, (hs, ws)) * 65535).astype(np.uint16)
+    return {"cols": cols, "cols'": 65535 - cols, "rows": rows, "rows'": 65535 - rows, "mix": mix}
+
+
+def flow_planes(hs, ws, seed):
+    """uint16 [hs][ws][3] encoded flows: random codes with the saturating and mask-boundary codes in the corners,
+    the zero / 65535 planes, and codes around 32768 whose neighbours differ by 1, 2, 3 and 6, so that the weights of
+    an enlargement by 5 / 4 (.25, .5, .75) land on exact .5 ties next to even and to odd codes, and on the mask's
+    32768 / 32769 threshold."""
+    rng = np.random.default_rng(seed)
     e = rng.integers(0, 65536, (hs, ws, 3), dtype=np.uint16)
-    e[0, 0], e[0, -1], e[-1, 0] = 65535, 0, 32768                         # saturating and boundary codes
+    e[0, 0], e[0, -1], e[-1, 0] = 65535, 0, 32768
     e[-1, -1] = (32768, 32769, 32769)
+    x = extreme_planes(hs, ws, seed)
+    near = rng.choice(np.array([32762, 32764, 32765, 32767, 32768, 32769, 32770, 32771, 32773, 32776], np.uint16),
+                      (hs, ws, 3))
+    near[0, 0], near[0, -1] = (0, 65535, 32768), (65535, 0, 32769)
+    return {"random": e, "extreme": np.stack([x["cols"], x["rows'"], x["mix"]], -1), "near": near}
+
+
+@pytest.mark.parametrize("hs,ws,h,w", ENLARGEMENTS + [(135, 240, 270, 480), (20, 20, 20, 20)])
+def test_flow(hs, ws, h, w):
     scale = h / hs
-    f, m = io.flow(e, h, w, scale)
-    rf, rm = ref_flow(e, h, w, scale)
-    assert bits_equal(f, rf) and bits_equal(m, rm)
-    assert bits_equal(io.resize(e, h, w), cv2.resize(e, (w, h), interpolation=cv2.INTER_AREA))
+    for name, e in flow_planes(hs, ws, hs * 100 + ws).items():
+        f, m = io.flow(e, h, w, scale)
+        rf, rm = ref_flow(e, h, w, scale)
+        assert bits_equal(f, rf) and bits_equal(m, rm), name
+        assert bits_equal(io.resize(e, h, w), cv2.resize(e, (w, h), interpolation=cv2.INTER_AREA)), name
 
 
-@pytest.mark.parametrize("hs,ws,h,w", [(30, 40, 30, 40), (60, 80, 30, 40), (120, 160, 30, 40), (15, 20, 30, 40),
-                                       (13, 17, 41, 37)])
+def test_flow_planes_hold_ties_and_threshold_codes():
+    """What flow_planes promises, so that the rounding and the mask threshold are really exercised: at 12 x 16 ->
+    15 x 20 the "near" plane's blends land on exact .5 ties below even and below odd codes, some of them between
+    32768 and 32769 in the mask's channel, which also resizes to 32768 and to 32769 themselves."""
+    e = flow_planes(12, 16, 7)["near"]
+    sx, fx = io.area_weights(20, 16)
+    sy, fy = io.area_weights(15, 12)
+    assert {0.25, 0.5, 0.75} <= set(fx.tolist()) and {0.25, 0.5, 0.75} <= set(fy.tolist())
+    x = e.astype(np.float64)
+    hor = x[:, sx] * (1 - fx)[None, :, None] + x[:, np.minimum(sx + 1, 15)] * fx[None, :, None]
+    out = hor[sy] * (1 - fy)[:, None, None] + hor[np.minimum(sy + 1, 11)] * fy[:, None, None]   # exact in double
+    ties = out[out % 1 == 0.5]
+    assert (np.floor(ties) % 2 == 0).sum() > 10 and (np.floor(ties) % 2 == 1).sum() > 10
+    assert (out[..., 2] == 32768.5).any()
+    third = io.resize(e, 15, 20)[..., 2]
+    assert (third == 32768).sum() > 10 and (third == 32769).sum() > 10
+
+
+@pytest.mark.parametrize("hs,ws,h,w", ENLARGEMENTS + [(30, 40, 30, 40), (60, 80, 30, 40), (120, 160, 30, 40),
+                                                      (24, 32, 6, 8)])
 def test_invdepth(hs, ws, h, w):
     d = np.random.default_rng(hs + ws).integers(0, 65536, (hs, ws), dtype=np.uint16)
     d[0, 0] = 65535
-    want = cv2.resize(d.astype(np.float32), (w, h), interpolation=cv2.INTER_AREA)
-    assert bits_equal(io.invdepth(d, h, w), want)
+    for name, d in dict(extreme_planes(hs, ws, hs + ws), random=d).items():
+        want = cv2.resize(d.astype(np.float32), (w, h), interpolation=cv2.INTER_AREA)
+        assert bits_equal(io.invdepth(d, h, w), want), name
+
+
+def test_exact_zero_weight_at_6_to_8():
+    """The case a fused multiply-add gets wrong: output 3 of 6 -> 8 has weight 4 - 3 * (8 / 6) = 0 exactly when the
+    product rounds first, so a zero sample next to 65535 stays 0.0 (fused, it would be 65535 * 2.2e-16)."""
+    s, f = io.area_weights(8, 6)
+    assert s[3] == 2 and f[3] == 0
+    d = np.zeros((6, 6), np.uint16)
+    d[:, 3] = 65535
+    got = io.invdepth(d, 8, 8)
+    assert bits_equal(got, cv2.resize(d.astype(np.float32), (8, 8), interpolation=cv2.INTER_AREA))
+    assert np.all(got[:, 3].view(np.uint32) == 0)
 
 
 def test_unsupported_ratios():
@@ -104,6 +165,26 @@ def test_tree_depth_matches_the_library():
         D = io.tree_depth(n)
         assert L.lrf_ingest_scratch_bytes(n) == (16 + 4 * n + 5 * (1 << D) + n + 7) // 8 * 8
     assert L.lrf_ingest_scratch_bytes(0) == 0 and L.lrf_ingest_scratch_bytes(9_000_000) == 0
+
+
+def test_scratch_bytes_boundary():
+    """The deepest tree the library builds has 16 levels: 2^16 leaves of 128 values is the largest frame it takes,
+    one more pixel is refused; 3840 x 2160 needs all 16.  The split at half the length rounded down to a multiple of
+    8 leaves the right half up to 7 longer, so some smaller frames need a 17th level too: the library refuses
+    exactly those the recursion says it must."""
+    from localrf_b200 import _lib
+    L = _lib.lib()
+    top = 128 << 16
+    assert io.tree_depth(top) == 16 and io.tree_depth(top + 1) == 17 and io.tree_depth(3840 * 2160) == 16
+    assert L.lrf_ingest_scratch_bytes(top) == (16 + 4 * top + 5 * (1 << 16) + top + 7) // 8 * 8
+    for n in (top + 1, top + 8, 2 * top, 1 << 40):
+        assert io.tree_depth(n) > 16 and L.lrf_ingest_scratch_bytes(n) == 0, n
+    assert io.tree_depth(7864328) == 16 and io.tree_depth(7864329) == 17       # the smallest frame refused
+    for n in list(range(top - 70, top)) + [3840 * 2160, 3840 * 2160 + 1, 4096 * 2048 - 1, 2896 * 2896, 7864328,
+                                           7864329]:
+        D = io.tree_depth(n)
+        want = (16 + 4 * n + 5 * (1 << D) + n + 7) // 8 * 8 if D <= 16 else 0
+        assert L.lrf_ingest_scratch_bytes(n) == want, (n, D)
 
 
 def test_golden_scenes():
