@@ -1,6 +1,7 @@
 // lrf_abi.cu -- the C ABI declared in include/localrf_b200.h (validation + launches).
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <climits>
 #include <cstdio>
 #include <cstring>
@@ -8,6 +9,7 @@
 
 #include "../../include/localrf_b200.h"
 #include "lrf_common.cuh"
+#include "lrf_launch.cuh"
 
 namespace lrf {
 size_t render_smem_bytes(int S, bool floater, int max_smem, bool pe);
@@ -112,13 +114,14 @@ struct DevInfo {
   int max_smem = 0;
   bool ok = false;
   unsigned long long* sched = nullptr;   // ring of per-launch ray counters (device memory)
-  unsigned int next = 0;
+  unsigned int next = 0;                 // the ring's slot lrf_render took last
 };
 constexpr unsigned int SCHED_RING = 256;
 
 // per-device launch resources, process-global (one ring of launch counters per device, allocated on first
-// use by whichever host thread gets there first; the autograd engine's worker threads share it)
-int device_info(DevInfo& d) {
+// use by whichever host thread gets there first; the autograd engine's worker threads share it).  take_slot:
+// advance the ring for the render launch that asks (d.next is then its slot).
+int device_info(DevInfo& d, bool take_slot = false) {
   static DevInfo cache[64];
   static std::mutex mu;
   std::lock_guard<std::mutex> lock(mu);
@@ -136,10 +139,43 @@ int device_info(DevInfo& d) {
     if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc(ray counters)");
     cache[dev].ok = true;
   }
-  cache[dev].next = (cache[dev].next + 1) % SCHED_RING;
+  if (take_slot) cache[dev].next = (cache[dev].next + 1) % SCHED_RING;
   d = cache[dev];
   return LRF_OK;
 }
+
+}  // namespace
+
+// The dynamic shared memory each kernel may use, per device, for the kernels that raise it (a handful).  An entry's
+// kernel is set once and never changes, so a reader that finds its kernel configured needs no lock.
+cudaError_t lrf::set_max_dynamic_smem(const void* kernel, int bytes) {
+  struct OptIn {
+    std::atomic<const void*> kernel{nullptr};
+    std::atomic<int> bytes[64] = {};
+  };
+  static OptIn table[16];
+  static std::mutex mu;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64) return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  for (const OptIn& t : table)
+    if (t.kernel.load(std::memory_order_acquire) == kernel && t.bytes[dev].load(std::memory_order_acquire) >= bytes)
+      return cudaSuccess;
+  std::lock_guard<std::mutex> lock(mu);
+  for (OptIn& t : table) {
+    const void* k = t.kernel.load(std::memory_order_relaxed);
+    if (k && k != kernel) continue;
+    if (!k) t.kernel.store(kernel, std::memory_order_release);
+    if (t.bytes[dev].load(std::memory_order_relaxed) >= bytes) return cudaSuccess;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) t.bytes[dev].store(bytes, std::memory_order_release);
+    return e;
+  }
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);   // the table is full
+}
+
+namespace {
 
 // validates the parts of a field every entry point needs and fills the device-side view
 int make_field(const LrfField* f, bool need_mlp, bool need_table, const void* prepared,
@@ -251,6 +287,46 @@ int check_field_grads(const LrfGradients* g, bool need_d_rays) {
   return LRF_OK;
 }
 
+// the MLP block lrf_field_prepare (allow_pe: fea_pe / view_pe up to 8) and lrf_field_prepare_backward (none) fold
+int check_mlp_block(const LrfField* f, bool allow_pe) {
+  if (f->app_dim != lrf::APP_DIM || f->featureC != lrf::FC || f->n_acomp != lrf::CA)
+    return fail(LRF_ERR_UNSUPPORTED, "only app_dim=27 / featureC=128 / appearance_n_comp=24 are built");
+  if (allow_pe && (f->fea_pe < 0 || f->view_pe < 0 || f->fea_pe > lrf::PE_MAX_FEA || f->view_pe > lrf::PE_MAX_VIEW))
+    return fail(LRF_ERR_UNSUPPORTED, "fea_pe / view_pe must be in [0, 8]");
+  if (!allow_pe && (f->fea_pe != 0 || f->view_pe != 0))
+    return fail(LRF_ERR_UNSUPPORTED, "positional encodings (fea_pe/view_pe > 0) are not built yet");
+  if (!f->basis || !f->w1 || !f->b1 || !f->w2 || !f->b2 || !f->w3 || !f->b3)
+    return fail(LRF_ERR_INVALID, "MLP / basis pointer is NULL");
+  return LRF_OK;
+}
+
+// a caller's scratch block: non-NULL, `align`-byte aligned (8 or 16) and at least `need` bytes
+int check_scratch(const void* scratch, size_t bytes, size_t need, int align, const char* too_small) {
+  if (!scratch || ((uintptr_t)scratch & (align - 1)))
+    return fail(LRF_ERR_INVALID, "scratch is NULL or not %s-byte aligned", align == 16 ? "16" : "8");
+  if (bytes < need) return fail(LRF_ERR_INVALID, "%s", too_small);
+  return LRF_OK;
+}
+
+// how many of the flow group's four pointers (fwd_flow, fwd_mask, bwd_flow, bwd_mask) are set
+template <typename T>
+int flow_count(const T& x) {
+  return !!x.fwd_flow + !!x.fwd_mask + !!x.bwd_flow + !!x.bwd_mask;
+}
+
+// the frame store of lrf_gather_rays and lrf_ingest_frame; n_flow: 4 when it holds the flow group, else 0
+int check_store(const LrfFrameStore* s, int& n_flow) {
+  if (s->n_px < 1) return fail(LRF_ERR_INVALID, "n_px must be >= 1");
+  if (s->capacity < 1) return fail(LRF_ERR_INVALID, "capacity must be >= 1");
+  if (!s->slot_frame || !s->rgb || !s->loss_weight)
+    return fail(LRF_ERR_INVALID, "slot_frame / rgb / loss_weight of the store is NULL");
+  n_flow = flow_count(*s);
+  if (n_flow != 0 && n_flow != 4)
+    return fail(LRF_ERR_INVALID, "the store's flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, "
+                                 "bwd_mask or none");
+  return LRF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -288,12 +364,8 @@ size_t lrf_prepared_bytes_for(const LrfField* f) {
 int lrf_field_prepare(const LrfField* f, void* prepared, lrf_stream_t stream) {
   if (!f || !prepared) return fail(LRF_ERR_INVALID, "field or prepared is NULL");
   if ((uintptr_t)prepared & 15) return fail(LRF_ERR_INVALID, "prepared must be 16-byte aligned");
-  if (f->app_dim != lrf::APP_DIM || f->featureC != lrf::FC || f->n_acomp != lrf::CA)
-    return fail(LRF_ERR_UNSUPPORTED, "only app_dim=27 / featureC=128 / appearance_n_comp=24 are built");
-  if (f->fea_pe < 0 || f->view_pe < 0 || f->fea_pe > lrf::PE_MAX_FEA || f->view_pe > lrf::PE_MAX_VIEW)
-    return fail(LRF_ERR_UNSUPPORTED, "fea_pe / view_pe must be in [0, 8]");
-  if (!f->basis || !f->w1 || !f->b1 || !f->w2 || !f->b2 || !f->w3 || !f->b3)
-    return fail(LRF_ERR_INVALID, "MLP / basis pointer is NULL");
+  const int rc = check_mlp_block(f, /*allow_pe=*/true);
+  if (rc != LRF_OK) return rc;
   if (f->fea_pe != 0 || f->view_pe != 0) {
     if ((uintptr_t)prepared & 1023) return fail(LRF_ERR_INVALID, "the prepared block of a field with positional encodings must be 1024-byte aligned");
     return cuda_status(lrf::launch_prepare_pe(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3, f->fea_pe, f->view_pe,
@@ -373,7 +445,7 @@ int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const
     B.signal_seq = o->signal_seq; B.wait_seq = o->wait_seq; B.rank = o->rank;
   }
   DevInfo d;
-  rc = device_info(d);
+  rc = device_info(d, /*take_slot=*/true);
   if (rc != LRF_OK) return rc;
   const size_t smem = lrf::render_smem_bytes(F.S, B.floater_thresh > 0.0f, d.max_smem, F.fea_pe > 0 || F.view_pe > 0);
   if ((long long)smem > d.max_smem)
@@ -464,12 +536,8 @@ size_t lrf_backward_scratch_bytes(int64_t n_rays, int32_t n_samples) {
 int lrf_field_prepare_backward(const LrfField* f, void* prepared_bwd, lrf_stream_t stream) {
   if (!f || !prepared_bwd) return fail(LRF_ERR_INVALID, "field or prepared_bwd is NULL");
   if ((uintptr_t)prepared_bwd & 15) return fail(LRF_ERR_INVALID, "prepared_bwd must be 16-byte aligned");
-  if (f->app_dim != lrf::APP_DIM || f->featureC != lrf::FC || f->n_acomp != lrf::CA)
-    return fail(LRF_ERR_UNSUPPORTED, "only app_dim=27 / featureC=128 / appearance_n_comp=24 are built");
-  if (f->fea_pe != 0 || f->view_pe != 0)
-    return fail(LRF_ERR_UNSUPPORTED, "positional encodings (fea_pe/view_pe > 0) are not built yet");
-  if (!f->basis || !f->w1 || !f->b1 || !f->w2 || !f->b2 || !f->w3 || !f->b3)
-    return fail(LRF_ERR_INVALID, "MLP / basis pointer is NULL");
+  const int rc = check_mlp_block(f, /*allow_pe=*/false);
+  if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_prepare_backward(f->basis, f->w1, f->b1, f->w2, f->b2, f->w3, f->b3,
                                                   static_cast<float*>(prepared_bwd),
                                                   (cudaStream_t)stream), "prepare_backward_kernel");
@@ -488,9 +556,9 @@ int lrf_render_backward(const LrfField* f, const void* prepared_bwd, const float
   if (n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
   if (!rays || !grad_rgb || !grad_depth || !g) return fail(LRF_ERR_INVALID, "rays / grad_rgb / grad_depth / grads is NULL");
   if ((rc = check_field_grads(g, true)) != LRF_OK) return rc;
-  if (!scratch || ((uintptr_t)scratch & 15)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 16-byte aligned");
-  if (scratch_bytes < lrf::backward_scratch_bytes(n_rays, F.S))
-    return fail(LRF_ERR_INVALID, "scratch is smaller than lrf_backward_scratch_bytes(n_rays, n_samples)");
+  if ((rc = check_scratch(scratch, scratch_bytes, lrf::backward_scratch_bytes(n_rays, F.S), 16,
+                          "scratch is smaller than lrf_backward_scratch_bytes(n_rays, n_samples)")) != LRF_OK)
+    return rc;
   DevInfo d;
   rc = device_info(d);
   if (rc != LRF_OK) return rc;
@@ -532,9 +600,9 @@ int lrf_render_backward_batch(const LrfField* f, const void* prepared_bwd, const
   if ((rc = make_batch(b, true, 2147483647LL, B)) != LRF_OK) return rc;
   if (!x || !grad_rgb || !grad_depth) return fail(LRF_ERR_INVALID, "rgb_linear / grad_rgb / grad_depth is NULL");
   if ((rc = check_field_grads(g, false)) != LRF_OK) return rc;
-  if (!scratch || ((uintptr_t)scratch & 15)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 16-byte aligned");
-  if (scratch_bytes < lrf::train_backward_scratch_bytes(b->n_rays, F.S, b->n_views))
-    return fail(LRF_ERR_INVALID, "scratch is smaller than lrf_backward_batch_scratch_bytes(n_rays, n_samples, n_views)");
+  rc = check_scratch(scratch, scratch_bytes, lrf::train_backward_scratch_bytes(b->n_rays, F.S, b->n_views), 16,
+                     "scratch is smaller than lrf_backward_batch_scratch_bytes(n_rays, n_samples, n_views)");
+  if (rc != LRF_OK) return rc;
   if (b->floater_thresh > 0.0f) return fail(LRF_ERR_UNSUPPORTED, "the backward is built for floater_thresh = 0");
   DevInfo d;
   if ((rc = device_info(d)) != LRF_OK) return rc;
@@ -649,9 +717,9 @@ int lrf_image_metrics(const float* img, int32_t img_stride, const float* gt, int
   if (filter_size < 1 || filter_size > 16) return fail(LRF_ERR_UNSUPPORTED, "filter_size must be in [1, 16]");
   if (H < filter_size || W < filter_size)
     return fail(LRF_ERR_INVALID, "H and W must be >= filter_size (the reference's SSIM map would be empty)");
-  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
-  if (scratch_bytes < lrf::metrics_scratch_bytes(H, W))
-    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_image_metrics_scratch_bytes(H, W, filter_size)");
+  const int rc = check_scratch(scratch, scratch_bytes, lrf::metrics_scratch_bytes(H, W), 8,
+                               "scratch_bytes is smaller than lrf_image_metrics_scratch_bytes(H, W, filter_size)");
+  if (rc != LRF_OK) return rc;
   const double c1 = (k1 * max_val) * (k1 * max_val), c2 = (k2 * max_val) * (k2 * max_val);
   return cuda_status(lrf::launch_image_metrics(img, img_stride, gt, gt_stride, H, W, filter_size, filter_sigma, c1, c2,
                                                out, ssim_map, scratch, (cudaStream_t)stream), "metrics_tile_kernel");
@@ -670,10 +738,8 @@ static int check_loss_batch(const LrfLossBatch* b, const void* scratch, size_t s
   if (b->use_depth && (!b->depth_map || !b->invdepths))
     return fail(LRF_ERR_INVALID, "a pointer of the depth term is NULL");
   if (b->n_rays / b->n_views > 4096) return fail(LRF_ERR_UNSUPPORTED, "more than 4096 rays per view");
-  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
-  if (scratch_bytes < lrf::losses_scratch_bytes(b->n_rays, b->n_views))
-    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_supervision_scratch_bytes(n_rays, n_views, n_cams)");
-  return LRF_OK;
+  return check_scratch(scratch, scratch_bytes, lrf::losses_scratch_bytes(b->n_rays, b->n_views), 8,
+                       "scratch_bytes is smaller than lrf_supervision_scratch_bytes(n_rays, n_views, n_cams)");
 }
 
 size_t lrf_supervision_scratch_bytes(int64_t n_rays, int64_t n_views, int64_t n_cams) {
@@ -710,14 +776,9 @@ int lrf_adam_step(const LrfAdamTensor* t, int64_t n, lrf_stream_t stream) {
 
 int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t stream) {
   if (!s || !g) return fail(LRF_ERR_INVALID, "store / gather is NULL");
-  if (s->n_px < 1) return fail(LRF_ERR_INVALID, "n_px must be >= 1");
-  if (s->capacity < 1) return fail(LRF_ERR_INVALID, "capacity must be >= 1");
-  if (!s->slot_frame || !s->rgb || !s->loss_weight)
-    return fail(LRF_ERR_INVALID, "slot_frame / rgb / loss_weight of the store is NULL");
-  const int n_flow = !!s->fwd_flow + !!s->fwd_mask + !!s->bwd_flow + !!s->bwd_mask;
-  if (n_flow != 0 && n_flow != 4)
-    return fail(LRF_ERR_INVALID, "the store's flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, "
-                                 "bwd_mask or none");
+  int n_flow = 0;
+  const int rc = check_store(s, n_flow);
+  if (rc != LRF_OK) return rc;
   if (g->n_rays < 0 || g->n_views < 1 || g->n_rays % g->n_views != 0)
     return fail(LRF_ERR_INVALID, "n_rays must be a multiple of n_views >= 1");
   if (g->n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
@@ -725,8 +786,7 @@ int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t 
     return fail(LRF_ERR_INVALID, "ids / idx / rgb / loss_weight of the gather is NULL");
   if (!s->invdepth != !g->invdepth)
     return fail(LRF_ERR_INVALID, "the invdepth output must be set exactly when the store has invdepth");
-  const int n_flow_out = !!g->fwd_flow + !!g->fwd_mask + !!g->bwd_flow + !!g->bwd_mask;
-  if (n_flow_out != n_flow)
+  if (flow_count(*g) != n_flow)
     return fail(LRF_ERR_INVALID, "the flow outputs must be set exactly when the store has the flow group");
   return cuda_status(lrf::launch_gather_rays(*s, *g, (cudaStream_t)stream), "gather_rays_kernel");
 }
@@ -746,7 +806,7 @@ int lrf_test_panels(const LrfPanelFrame* f, void* scratch, size_t scratch_bytes,
   if (f->n_cams < 1) return fail(LRF_ERR_INVALID, "n_cams must be >= 1");
   if (f->idx < 0 || f->idx >= f->n_cams) return fail(LRF_ERR_INVALID, "idx must lie in [0, n_cams)");
   if (!f->depth) return fail(LRF_ERR_INVALID, "depth is NULL");
-  const int n_flow = !!f->fwd_flow + !!f->fwd_mask + !!f->bwd_flow + !!f->bwd_mask;
+  const int n_flow = flow_count(*f);
   if (n_flow != 0 && n_flow != 4)
     return fail(LRF_ERR_INVALID, "the flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, bwd_mask "
                                  "or none");
@@ -754,11 +814,11 @@ int lrf_test_panels(const LrfPanelFrame* f, void* scratch, size_t scratch_bytes,
     return fail(LRF_ERR_INVALID, "the flow panels need directions, cam2world and intrinsics");
   if (n_flow && (!f->fwd_panel || !f->bwd_panel)) return fail(LRF_ERR_INVALID, "fwd_panel / bwd_panel is NULL");
   if (f->invdepth && !f->depth_panel) return fail(LRF_ERR_INVALID, "depth_panel is NULL");
-  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
-  if (scratch_bytes < lrf_test_panels_scratch_bytes(f->W, f->H))
-    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_test_panels_scratch_bytes(W, H)");
+  int rc = check_scratch(scratch, scratch_bytes, lrf_test_panels_scratch_bytes(f->W, f->H), 8,
+                         "scratch_bytes is smaller than lrf_test_panels_scratch_bytes(W, H)");
+  if (rc != LRF_OK) return rc;
   DevInfo d;
-  int rc = device_info(d);
+  rc = device_info(d);
   if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_test_panels(*f, scratch, d.n_sms, (cudaStream_t)stream), "test_panels");
 }
@@ -776,19 +836,13 @@ static int check_plane(const void* p, int32_t ws, int32_t hs, int64_t stride, in
 int lrf_ingest_frame(const LrfFrameStore* s, const LrfIngestFrame* f, void* scratch, size_t scratch_bytes,
                      lrf_stream_t stream) {
   if (!s || !f) return fail(LRF_ERR_INVALID, "store / frame is NULL");
-  if (s->n_px < 1) return fail(LRF_ERR_INVALID, "n_px must be >= 1");
-  if (s->capacity < 1) return fail(LRF_ERR_INVALID, "capacity must be >= 1");
-  if (!s->slot_frame || !s->rgb || !s->loss_weight)
-    return fail(LRF_ERR_INVALID, "slot_frame / rgb / loss_weight of the store is NULL");
-  const int n_flow = !!s->fwd_flow + !!s->fwd_mask + !!s->bwd_flow + !!s->bwd_mask;
-  if (n_flow != 0 && n_flow != 4)
-    return fail(LRF_ERR_INVALID, "the store's flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, "
-                                 "bwd_mask or none");
+  int n_flow = 0;
+  int rc = check_store(s, n_flow);
+  if (rc != LRF_OK) return rc;
   if (f->slot < 0 || f->slot >= s->capacity) return fail(LRF_ERR_INVALID, "slot must lie in [0, capacity)");
   if (f->w < 1 || f->h < 1 || (int64_t)f->w * f->h != s->n_px)
     return fail(LRF_ERR_INVALID, "w and h must be >= 1 with w h == the store's n_px");
-  int rc = check_plane(f->image, f->w0, f->h0, f->image_stride, 3, "image");
-  if (rc != LRF_OK) return rc;
+  if ((rc = check_plane(f->image, f->w0, f->h0, f->image_stride, 3, "image")) != LRF_OK) return rc;
   if (!s->invdepth != !f->invdepth)
     return fail(LRF_ERR_INVALID, "invdepth must be set exactly when the store has invdepth");
   if (f->invdepth && (rc = check_plane(f->invdepth, f->wd, f->hd, f->invdepth_stride, 1, "invdepth")) != LRF_OK)
@@ -799,11 +853,11 @@ int lrf_ingest_frame(const LrfFrameStore* s, const LrfIngestFrame* f, void* scra
                  (rc = check_plane(f->bwd_flow, f->wf, f->hf, f->flow_stride, 3, "bwd_flow")) != LRF_OK))
     return rc;
   if (f->mask && (rc = check_plane(f->mask, f->wm, f->hm, f->mask_stride, 1, "mask")) != LRF_OK) return rc;
-  if (!scratch || ((uintptr_t)scratch & 7)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 8-byte aligned");
-  const size_t need = lrf_ingest_scratch_bytes(s->n_px);
+  const size_t need = lrf_ingest_scratch_bytes(s->n_px);   // 0: too large, refused after the scratch checks
+  if ((rc = check_scratch(scratch, scratch_bytes, need, 8,
+                          "scratch_bytes is smaller than lrf_ingest_scratch_bytes(n_px)")) != LRF_OK)
+    return rc;
   if (need == 0) return fail(LRF_ERR_UNSUPPORTED, "frames above 2^16 leaves of 128 pixels are not built");
-  if (scratch_bytes < need)
-    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_ingest_scratch_bytes(n_px)");
   const int image_mode = lrf::ingest_resize_mode(f->w0, f->h0, f->w, f->h);
   if (image_mode < 1)
     return fail(LRF_ERR_UNSUPPORTED, "the image must be w x h or a reduction by 2 or 4 of it (k w x k h)");

@@ -1,6 +1,7 @@
 // lrf_aux.cu -- the small kernels around the render kernel: the synchronous tensor-core MLP on
 // explicit features (lrf_mlp_forward), weight preparation, stand-alone feature lookups, repack.
 #include "lrf_device.cuh"
+#include "lrf_launch.cuh"
 
 namespace lrf {
 
@@ -213,19 +214,9 @@ cudaError_t launch_mlp(const float* prep, const float* feats, const float* viewd
                        float* rgb, int n_sms, cudaStream_t stream) {
   if (M == 0) return cudaSuccess;
   const size_t smem = (size_t)mlp_smem().total;
-  static bool configured[64] = {false};   // per device
-  int dev = 0;
-  cudaError_t e0 = cudaGetDevice(&dev);
-  if (e0 != cudaSuccess) return e0;
-  if (dev >= 0 && dev < 64 && !configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(mlp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[dev] = true;
-  }
-  long long n_tiles = (M + TM - 1) / TM;
-  int grid = (int)(n_tiles < n_sms ? n_tiles : n_sms);
-  mlp_kernel<<<grid, THREADS, smem, stream>>>(prep, feats, viewdirs, M, rgb);
+  const cudaError_t e = set_max_dynamic_smem((const void*)mlp_kernel, (int)smem);
+  if (e != cudaSuccess) return e;
+  mlp_kernel<<<cta_count(M, TM, n_sms, 1), THREADS, smem, stream>>>(prep, feats, viewdirs, M, rgb);
   return cudaGetLastError();
 }
 
@@ -275,9 +266,7 @@ __global__ void pack_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* _
 
 cudaError_t launch_pack_bf16(const float* src, void* dst, long long n, int n_sms, cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
-  long long blocks = (n + 255) / 256;
-  const long long cap = (long long)n_sms * 8;
-  pack_bf16_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, stream>>>(
+  pack_bf16_kernel<<<cta_count(n, 256, n_sms, 8), 256, 0, stream>>>(
       src, static_cast<__nv_bfloat16*>(dst), n);
   return cudaGetLastError();
 }

@@ -26,6 +26,7 @@
 #include <cstdlib>
 
 #include "lrf_device.cuh"
+#include "lrf_launch.cuh"
 
 namespace lrf {
 
@@ -59,36 +60,22 @@ struct BwdArgs {
   BwdScratch s;
 };
 
-__host__ __device__ inline size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
-
-__host__ inline size_t bwd_scratch_layout(long long n, int S, BwdScratch* out, unsigned char* base,
-                                          size_t* zero_bytes) {
+// each array 16-byte aligned; *zero_bytes: the leading bytes that hold count and d_ovd
+inline BwdScratch carve(ScratchCarver& c, long long n, int S, size_t* zero_bytes = nullptr) {
   const size_t ns = (size_t)n * (size_t)S;
-  size_t off = 0;
-  const size_t o_count = off; off += 16;
-  const size_t o_ovd = off;   off = align16(off + (size_t)n * 6 * sizeof(float));
-  if (zero_bytes) *zero_bytes = off;
-  const size_t o_alpha = off; off = align16(off + ns * 4);
-  const size_t o_T = off;     off = align16(off + ns * 4);
-  const size_t o_w = off;     off = align16(off + ns * 4);
-  const size_t o_fe = off;    off = align16(off + ns * 4);
-  const size_t o_gw = off;    off = align16(off + ns * 4);
-  const size_t o_ray = off;   off = align16(off + ns * 4);
-  const size_t o_k = off;     off = align16(off + ns * 4);
-  const size_t o_valid = off; off = align16(off + ns);
-  if (out && base) {
-    out->count = reinterpret_cast<unsigned long long*>(base + o_count);
-    out->d_ovd = reinterpret_cast<float*>(base + o_ovd);
-    out->alpha = reinterpret_cast<float*>(base + o_alpha);
-    out->T = reinterpret_cast<float*>(base + o_T);
-    out->w = reinterpret_cast<float*>(base + o_w);
-    out->fe = reinterpret_cast<float*>(base + o_fe);
-    out->gw = reinterpret_cast<float*>(base + o_gw);
-    out->app_ray = reinterpret_cast<int*>(base + o_ray);
-    out->app_k = reinterpret_cast<int*>(base + o_k);
-    out->valid = base + o_valid;
-  }
-  return off;
+  BwdScratch s;
+  s.count = c.take<unsigned long long>(16, 16);
+  s.d_ovd = c.take<float>((size_t)n * 6 * sizeof(float), 16);
+  if (zero_bytes) *zero_bytes = c.size(16);
+  s.alpha = c.take<float>(ns * 4, 16);
+  s.T = c.take<float>(ns * 4, 16);
+  s.w = c.take<float>(ns * 4, 16);
+  s.fe = c.take<float>(ns * 4, 16);
+  s.gw = c.take<float>(ns * 4, 16);
+  s.app_ray = c.take<int>(ns * 4, 16);
+  s.app_k = c.take<int>(ns * 4, 16);
+  s.valid = c.take(ns, 16);
+  return s;
 }
 
 // ====================================================================================================
@@ -736,7 +723,9 @@ cudaError_t launch_prepare(const float* basis, const float* w1, const float* b1,
                            const float* b2, const float* w3, const float* b3, unsigned char* prep,
                            cudaStream_t stream);
 size_t backward_scratch_bytes(long long n_rays, int S) {
-  return bwd_scratch_layout(n_rays, S, nullptr, nullptr, nullptr);
+  ScratchCarver c(nullptr);
+  carve(c, n_rays, S);
+  return c.size(16);
 }
 size_t backward_shade_smem_bytes(bool tc) { return (size_t)(tc ? ShadeSmemT<true>::total : ShadeSmem::total) * sizeof(float); }
 
@@ -751,8 +740,9 @@ cudaError_t launch_prepare_backward(const float* basis, const float* w1, const f
 
 cudaError_t launch_render_backward(const FieldDev& F, BwdArgs A, void* scratch, float* dpos, int n_sms,
                                    cudaStream_t stream) {
+  ScratchCarver c(scratch);
   size_t zero_bytes = 0;
-  bwd_scratch_layout(A.n_rays, F.S, &A.s, static_cast<unsigned char*>(scratch), &zero_bytes);
+  A.s = carve(c, A.n_rays, F.S, &zero_bytes);
   A.s.dpos = dpos;
   cudaError_t e = cudaMemsetAsync(scratch, 0, zero_bytes, stream);
   if (e != cudaSuccess) return e;
@@ -761,21 +751,10 @@ cudaError_t launch_render_backward(const FieldDev& F, BwdArgs A, void* scratch, 
   const char* tc_env = getenv("LRF_BWD_TC");
   const bool use_tc = !(tc_env && tc_env[0] == '0');
   const size_t smem = backward_shade_smem_bytes(use_tc);
-  static bool configured[2][64] = {{false}, {false}};
-  int dev = 0;
-  e = cudaGetDevice(&dev);
+  e = set_max_dynamic_smem(use_tc ? (const void*)bwd_shade_kernel<true> : (const void*)bwd_shade_kernel<false>,
+                           (int)smem);
   if (e != cudaSuccess) return e;
-  if (dev >= 0 && dev < 64 && !configured[use_tc][dev]) {
-    e = use_tc ? cudaFuncSetAttribute(bwd_shade_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-               : cudaFuncSetAttribute(bwd_shade_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[use_tc][dev] = true;
-  }
-  const long long warps_per_cta = MARCH_THREADS / 32;
-  long long want = (A.n_rays + warps_per_cta - 1) / warps_per_cta;
-  const long long cap = (long long)n_sms * 8;
-  int grid = (int)(want < cap ? want : cap);
-  if (grid < 1) grid = 1;
+  const unsigned int grid = cta_count(A.n_rays, MARCH_THREADS / 32, n_sms, 8);   // a warp per ray
   bwd_march_kernel<<<grid, MARCH_THREADS, 0, stream>>>(F, A);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;

@@ -21,6 +21,7 @@
 #include <initializer_list>
 
 #include "../../include/localrf_b200.h"
+#include "lrf_launch.cuh"
 
 namespace lrf {
 
@@ -298,24 +299,16 @@ struct Scratch {
   float* sums;
   uint8_t* flags;
   uint8_t* gray;
-  size_t bytes;
 };
 
-Scratch carve(void* base, long long n, int depth) {
-  char* b = (char*)base;
+Scratch carve(ScratchCarver& c, long long n, int depth) {
+  const size_t S = (size_t)1 << depth;
   Scratch s;
-  const long long S = 1LL << depth;
-  size_t o = 16;
-  s.stats = (float*)b;
-  s.lap = (float*)(b + o);
-  o += 4 * (size_t)n;
-  s.sums = (float*)(b + o);
-  o += 4 * (size_t)S;
-  s.flags = (uint8_t*)(b + o);
-  o += (size_t)S;
-  s.gray = (uint8_t*)(b + o);
-  o += (size_t)n;
-  s.bytes = (o + 7) & ~(size_t)7;
+  s.stats = c.take<float>(16, 4);
+  s.lap = c.take<float>(4 * (size_t)n, 4);
+  s.sums = c.take<float>(4 * S, 4);
+  s.flags = c.take<uint8_t>(S, 1);
+  s.gray = c.take<uint8_t>((size_t)n, 1);
   return s;
 }
 
@@ -351,7 +344,10 @@ int ingest_tree_depth(long long n) {
 
 size_t ingest_scratch_bytes(long long n_px) {
   const int depth = ingest_tree_depth(n_px);
-  return depth < 0 ? 0 : carve(nullptr, n_px, depth).bytes;
+  if (depth < 0) return 0;
+  ScratchCarver c(nullptr);
+  carve(c, n_px, depth);
+  return c.size(8);
 }
 
 int ingest_resize_mode(int ws, int hs, int w, int h) { return resize_mode(ws, hs, w, h); }
@@ -360,7 +356,8 @@ cudaError_t launch_ingest_frame(const LrfFrameStore& st, const LrfIngestFrame& f
                                 cudaStream_t stream) {
   const long long n = (long long)f.w * f.h;
   const int depth = ingest_tree_depth(n);
-  const Scratch s = carve(scratch, n, depth);
+  ScratchCarver c(scratch);
+  const Scratch s = carve(c, n, depth);
   const unsigned blocks = (unsigned)((n + INGEST_THREADS - 1) / INGEST_THREADS);
   const unsigned slot_blocks = (unsigned)(((1LL << depth) + INGEST_THREADS - 1) / INGEST_THREADS);
   const long long at = f.slot * n;

@@ -18,6 +18,7 @@
 #include <stdint.h>
 
 #include "../../include/localrf_b200.h"
+#include "lrf_launch.cuh"
 #include "lrf_reproject.cuh"
 #define LRF_SELECT_KEYS_ONLY
 #include "lrf_select.cuh"
@@ -30,42 +31,23 @@ constexpr float LOSS_Q_FLOW = 0.9f, LOSS_Q_DEPTH = 0.8f;
 // 8..19 d(Rcc, tcc) of the backward direction, 20..31 of the forward direction (row-major 3x4)
 constexpr int P_RGB = 0, P_W = 1, P_FLOW = 2, P_DEPTH = 3, P_INTR = 4, P_CAM = 8;
 
-struct LossLayout {
-  size_t e, d, tau, med, mad, glob, part, total;
-};
-
-// The leading part is documented in the header (lrf_supervision_losses): e [N], d [N], tau [2][V], med [V][2].
-inline LossLayout loss_layout(long long N, long long V) {
-  LossLayout L;
-  L.e = 0;
-  L.d = 4 * (size_t)N;
-  L.tau = 8 * (size_t)N;
-  L.med = L.tau + 8 * (size_t)V;
-  L.mad = L.med + 8 * (size_t)V;
-  L.glob = (L.mad + 8 * (size_t)V + 7) & ~(size_t)7;
-  L.part = L.glob + 16;
-  L.total = L.part + (size_t)LOSS_NPART * 8 * (size_t)V;
-  return L;
-}
-
 struct LossPtrs {                     // scratch, carved
   float *e, *d, *tau_f, *tau_d, *mad;
   int* med;
   double *glob, *part;
 };
 
-static LossPtrs carve(void* scratch, long long N, long long V) {
-  const LossLayout L = loss_layout(N, V);
-  unsigned char* s = static_cast<unsigned char*>(scratch);
+// The leading part is documented in the header (lrf_supervision_losses): e [N], d [N], tau [2][V], med [V][2].
+static LossPtrs carve(ScratchCarver& c, long long N, long long V) {
   LossPtrs p;
-  p.e = reinterpret_cast<float*>(s + L.e);
-  p.d = reinterpret_cast<float*>(s + L.d);
-  p.tau_f = reinterpret_cast<float*>(s + L.tau);
-  p.tau_d = p.tau_f + V;
-  p.med = reinterpret_cast<int*>(s + L.med);
-  p.mad = reinterpret_cast<float*>(s + L.mad);
-  p.glob = reinterpret_cast<double*>(s + L.glob);
-  p.part = reinterpret_cast<double*>(s + L.part);
+  p.e = c.take<float>(4 * (size_t)N, 4);
+  p.d = c.take<float>(4 * (size_t)N, 4);
+  p.tau_f = c.take<float>(4 * (size_t)V, 4);
+  p.tau_d = c.take<float>(4 * (size_t)V, 4);
+  p.med = c.take<int>(8 * (size_t)V, 4);
+  p.mad = c.take<float>(8 * (size_t)V, 4);
+  p.glob = c.take<double>(16, 8);
+  p.part = c.take<double>((size_t)LOSS_NPART * 8 * (size_t)V, 8);
   return p;
 }
 
@@ -116,20 +98,9 @@ __device__ inline unsigned long long sorted_median(const unsigned long long* k, 
   return k[lo];
 }
 
-__device__ inline double block_sum_d(double v, double* red) {      // result valid in thread 0
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[warp] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < nw; ++w) s += red[w];
-  return s;
-}
-// the same, broadcast to every thread
+// block_sum_fp64, broadcast to every thread
 __device__ inline double block_sum_all(double v, double* red) {
-  const double s = block_sum_d(v, red);
+  const double s = block_sum_fp64(v, red);
   __syncthreads();
   if (threadIdx.x == 0) red[0] = s;
   __syncthreads();
@@ -185,8 +156,8 @@ __global__ void __launch_bounds__(LOSS_THREADS) losses_view_kernel(LrfLossBatch 
     srgb += (double)a + (double)c + (double)d;
     sw += (double)w;
   }
-  srgb = block_sum_d(srgb, red);
-  sw = block_sum_d(sw, red);
+  srgb = block_sum_fp64(srgb, red);
+  sw = block_sum_fp64(sw, red);
   if (threadIdx.x == 0) {
     part[P_RGB] = srgb;
     part[P_W] = sw;
@@ -222,7 +193,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) losses_view_kernel(LrfLossBatch 
       const float e = key2f(keys[i]);
       if (!(e > tau)) sf += (double)e;
     }
-    sf = block_sum_d(sf, red);
+    sf = block_sum_fp64(sf, red);
     if (threadIdx.x == 0) {
       s.tau_f[v] = tau;
       part[P_FLOW] = sf;
@@ -282,7 +253,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) losses_view_kernel(LrfLossBatch 
       const float d = key2f(keys[i]);
       if (!(d > tau)) sd += (double)d;
     }
-    sd = block_sum_d(sd, red);
+    sd = block_sum_fp64(sd, red);
     if (threadIdx.x == 0) {
       s.tau_d[v] = tau;
       part[P_DEPTH] = sd;
@@ -295,7 +266,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) losses_final_kernel(LrfLossBatch
   double acc[4] = {0.0, 0.0, 0.0, 0.0};
   for (long long v = threadIdx.x; v < b.n_views; v += blockDim.x)
     for (int j = 0; j < 4; ++j) acc[j] += s.part[LOSS_NPART * v + j];
-  for (int j = 0; j < 4; ++j) acc[j] = block_sum_d(acc[j], red);
+  for (int j = 0; j < 4; ++j) acc[j] = block_sum_fp64(acc[j], red);
   if (threadIdx.x == 0) {
     const double N = (double)b.n_rays;
     const double mean_w = acc[P_W] / N;
@@ -479,7 +450,11 @@ __global__ void __launch_bounds__(LOSS_THREADS) losses_final_backward_kernel(Lrf
 }
 
 // ---- host side --------------------------------------------------------------------------------------------
-size_t losses_scratch_bytes(long long N, long long V) { return loss_layout(N, V).total; }
+size_t losses_scratch_bytes(long long N, long long V) {
+  ScratchCarver c(nullptr);
+  carve(c, N, V);
+  return c.size();
+}
 
 static int pow2_at_least(int R) {
   int P = 1;
@@ -488,18 +463,11 @@ static int pow2_at_least(int R) {
 }
 
 cudaError_t launch_supervision_losses(const LrfLossBatch& b, float* losses, void* scratch, cudaStream_t stream) {
-  static bool configured[64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_max_dynamic_smem((const void*)losses_view_kernel, LOSS_MAX_R * (8 + 4));
   if (e != cudaSuccess) return e;
-  const size_t max_smem = (size_t)LOSS_MAX_R * (8 + 4);
-  if (dev >= 0 && dev < 64 && !configured[dev]) {
-    e = cudaFuncSetAttribute(losses_view_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem);
-    if (e != cudaSuccess) return e;
-    configured[dev] = true;
-  }
   const int R = (int)(b.n_rays / b.n_views), P = pow2_at_least(R);
-  const LossPtrs s = carve(scratch, b.n_rays, b.n_views);
+  ScratchCarver c(scratch);
+  const LossPtrs s = carve(c, b.n_rays, b.n_views);
   losses_view_kernel<<<(unsigned)b.n_views, LOSS_THREADS, (size_t)P * 8 + (size_t)R * 4, stream>>>(b, R, P, s);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
@@ -510,7 +478,8 @@ cudaError_t launch_supervision_losses(const LrfLossBatch& b, float* losses, void
 cudaError_t launch_supervision_losses_backward(const LrfLossBatch& b, const float* grad_losses, const LrfLossGrads& g,
                                                void* scratch, cudaStream_t stream) {
   const int R = (int)(b.n_rays / b.n_views);
-  const LossPtrs s = carve(scratch, b.n_rays, b.n_views);
+  ScratchCarver c(scratch);
+  const LossPtrs s = carve(c, b.n_rays, b.n_views);
   losses_view_backward_kernel<<<(unsigned)b.n_views, LOSS_THREADS, 0, stream>>>(b, R, s, grad_losses, g);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

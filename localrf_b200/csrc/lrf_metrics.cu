@@ -15,6 +15,8 @@
 // deterministic, with no atomics.
 #include <cuda_runtime.h>
 
+#include "lrf_launch.cuh"
+
 namespace lrf {
 
 constexpr int MET_TH = 16, MET_TW = 32, MET_THREADS = 256, MET_MAX_FS = 16;
@@ -26,18 +28,6 @@ struct MetricTaps {
 __host__ __device__ inline size_t metrics_smem_bytes(int fs) {
   const int rows = MET_TH + fs - 1, cols = MET_TW + fs - 1;
   return (size_t)5 * MET_TH * cols * sizeof(double) + (size_t)2 * 3 * rows * cols * sizeof(float);
-}
-
-__device__ inline double block_sum(double v, double* red) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();                                   // red may still be read by a previous call
-  if ((threadIdx.x & 31) == 0) red[warp] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < nw; ++w) s += red[w];
-  return s;                                          // valid in thread 0
 }
 
 __global__ void __launch_bounds__(MET_THREADS) metrics_tile_kernel(
@@ -131,8 +121,8 @@ __global__ void __launch_bounds__(MET_THREADS) metrics_tile_kernel(
     __syncthreads();                                 // V is rewritten by the next channel
   }
 
-  const double mse_cta = block_sum(mse, red);
-  const double ssim_cta = block_sum(ssim, red);
+  const double mse_cta = block_sum_fp64(mse, red);
+  const double ssim_cta = block_sum_fp64(ssim, red);
   if (threadIdx.x == 0) {
     const int cta = blockIdx.y * gridDim.x + blockIdx.x;
     partial[2 * cta] = mse_cta;
@@ -148,8 +138,8 @@ __global__ void __launch_bounds__(1024) metrics_final_kernel(const double* __res
     mse += partial[2 * i];
     ssim += partial[2 * i + 1];
   }
-  mse = block_sum(mse, red);
-  ssim = block_sum(ssim, red);
+  mse = block_sum_fp64(mse, red);
+  ssim = block_sum_fp64(ssim, red);
   if (threadIdx.x == 0) {
     out[0] = mse / n_pix;
     out[1] = ssim / n_map;
@@ -181,16 +171,8 @@ static MetricTaps gaussian_taps(int fs, double sigma) {
 cudaError_t launch_image_metrics(const float* img, int img_stride, const float* gt, int gt_stride, int H, int W,
                                  int fs, double sigma, double c1, double c2, double* out, double* ssim_map,
                                  void* scratch, cudaStream_t stream) {
-  static bool configured[64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_max_dynamic_smem((const void*)metrics_tile_kernel, (int)metrics_smem_bytes(MET_MAX_FS));
   if (e != cudaSuccess) return e;
-  if (dev >= 0 && dev < 64 && !configured[dev]) {
-    e = cudaFuncSetAttribute(metrics_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)metrics_smem_bytes(MET_MAX_FS));
-    if (e != cudaSuccess) return e;
-    configured[dev] = true;
-  }
   const MetricTaps t = gaussian_taps(fs, sigma);
   const dim3 grid((W + MET_TW - 1) / MET_TW, (H + MET_TH - 1) / MET_TH);
   double* partial = static_cast<double*>(scratch);

@@ -19,6 +19,7 @@
 #include <stdint.h>
 
 #include "../../include/localrf_b200.h"
+#include "lrf_launch.cuh"
 #include "lrf_reproject.cuh"
 #include "lrf_select.cuh"
 
@@ -29,21 +30,6 @@ constexpr int PAN_THREADS = 256, PAN_MAD_BLOCKS = 1024, PAN_NSTATS = 8;
 // upper neighbour is the next rank, that one too; the medians of x and g follow (or come first without the flow
 // branch).  Only above 2^24 values can numpy's float32 index put the upper neighbour two ranks up: it then gets a job
 // of its own after the medians.
-
-struct PanelLayout {
-  size_t state, stats, mad, cmp, xg, total;
-};
-
-inline PanelLayout panel_layout(long long n_px) {
-  PanelLayout L;
-  L.state = 0;
-  L.stats = L.state + (size_t)SEL_MAX_JOBS * sizeof(SelectState);
-  L.mad = L.stats + 64;
-  L.cmp = L.mad + (size_t)2 * PAN_MAD_BLOCKS * sizeof(double);
-  L.xg = L.cmp + (size_t)4 * 2 * n_px * sizeof(float);
-  L.total = L.xg + (size_t)2 * n_px * sizeof(float);
-  return L;
-}
 
 // what the host folds for the device: np.quantile's rank and weight for n = 2 W H values
 struct QuantRule {
@@ -67,6 +53,15 @@ struct PanelArgs {
   float* cmp;                  // [4][2 n]: pred_c rows, then gt_c rows
   float* xg;                   // [2][n]: x, g
 };
+
+// the scratch: the selection states, the statistics, the MAD partials, cmp, xg
+static void carve(ScratchCarver& c, PanelArgs& a) {
+  a.st = c.take<SelectState>((size_t)SEL_MAX_JOBS * sizeof(SelectState), 8);
+  a.stats = c.take<float>(64, 8);
+  a.mad = c.take<double>((size_t)2 * PAN_MAD_BLOCKS * sizeof(double), 8);
+  a.cmp = c.take<float>((size_t)4 * 2 * a.n * sizeof(float), 8);
+  a.xg = c.take<float>((size_t)2 * a.n * sizeof(float), 8);
+}
 
 // clamp(0, 1) as torch's and numpy's: NaN and -0 pass through (only values strictly outside are replaced)
 __device__ inline float clamp01(float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); }
@@ -128,18 +123,6 @@ __device__ inline float selected(const SelectState& S) {
   return S.n_nan ? __int_as_float(0x7fffffff) : select_value(S);
 }
 
-__device__ inline double block_sum_fixed(double v, double* red) {   // result valid in thread 0
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[warp] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < nw; ++w) s += red[w];
-  return s;
-}
-
 // blockIdx.y: 0 x, 1 g.  Every block sums a fixed slice of the pixels, so the order depends on n alone.
 __global__ void __launch_bounds__(PAN_THREADS) panels_mad_kernel(PanelArgs a) {
   __shared__ double red[PAN_THREADS / 32];
@@ -149,7 +132,7 @@ __global__ void __launch_bounds__(PAN_THREADS) panels_mad_kernel(PanelArgs a) {
   double s = 0.0;
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < a.n; p += (long long)gridDim.x * blockDim.x)
     s += (double)fabsf(__fsub_rn(v[p], t));
-  s = block_sum_fixed(s, red);
+  s = block_sum_fp64(s, red);
   if (threadIdx.x == 0) a.mad[which * PAN_MAD_BLOCKS + blockIdx.x] = s;
 }
 
@@ -174,7 +157,7 @@ __global__ void __launch_bounds__(PAN_THREADS) panels_stats_kernel(PanelArgs a) 
     double s = 0.0;
     if (a.depth)
       for (int b = threadIdx.x; b < a.mad_blocks; b += blockDim.x) s += a.mad[which * PAN_MAD_BLOCKS + b];
-    s = block_sum_fixed(s, red);
+    s = block_sum_fp64(s, red);
     if (threadIdx.x == 0) {
       a.stats[4 + 2 * which] = a.depth ? selected(a.st[a.job_x + which]) : nan;
       a.stats[5 + 2 * which] = a.depth ? (float)(s / (double)a.n) : nan;
@@ -214,7 +197,13 @@ __global__ void __launch_bounds__(PAN_THREADS) panels_finish_kernel(PanelArgs a)
 }
 
 // ---- host side --------------------------------------------------------------------------------------------
-size_t panels_scratch_bytes(long long n_px) { return panel_layout(n_px).total; }
+size_t panels_scratch_bytes(long long n_px) {
+  PanelArgs a;
+  a.n = n_px;
+  ScratchCarver c(nullptr);
+  carve(c, a);
+  return c.size();
+}
 
 // numpy 2.x, method="linear", float32 input: q is float32(0.9); the virtual index (n - 1) * q is float32 (the Python
 // int n - 1 is cast to float32 first), floor() and + 1 stay float32, and gamma = index - floor(index) is float32.
@@ -244,13 +233,8 @@ cudaError_t launch_test_panels(const LrfPanelFrame& f, void* scratch, int n_sms,
   a.job_x = a.flow ? 4 : 0;
   a.hi_mode = a.q.hi == a.q.lo ? 0 : (a.q.hi == a.q.lo + 1 ? 1 : 2);
   a.job_hi = a.job_x + (a.depth ? 2 : 0);
-  const PanelLayout L = panel_layout(a.n);
-  unsigned char* s = static_cast<unsigned char*>(scratch);
-  a.st = reinterpret_cast<SelectState*>(s + L.state);
-  a.stats = reinterpret_cast<float*>(s + L.stats);
-  a.mad = reinterpret_cast<double*>(s + L.mad);
-  a.cmp = reinterpret_cast<float*>(s + L.cmp);
-  a.xg = reinterpret_cast<float*>(s + L.xg);
+  ScratchCarver c(scratch);
+  carve(c, a);
   const long long mb = (a.n + 4095) / 4096;
   a.mad_blocks = (int)(mb < PAN_MAD_BLOCKS ? mb : PAN_MAD_BLOCKS);
 
@@ -267,8 +251,7 @@ cudaError_t launch_test_panels(const LrfPanelFrame& f, void* scratch, int n_sms,
 
   cudaError_t e = cudaMemsetAsync(a.st, 0, (size_t)n_jobs * sizeof(SelectState), stream);
   if (e != cudaSuccess) return e;
-  const long long want = (a.n + PAN_THREADS - 1) / PAN_THREADS, cap = (long long)(n_sms > 0 ? n_sms : 132) * 16;
-  const unsigned int grid = (unsigned int)(want < cap ? want : cap);
+  const unsigned int grid = cta_count(a.n, PAN_THREADS, n_sms, 16);
   panels_prep_kernel<<<grid, PAN_THREADS, 0, stream>>>(a);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   e = launch_select(jobs, a.st, n_jobs, (unsigned int)(a.flow ? 2 * a.n : a.n), n_sms, stream);

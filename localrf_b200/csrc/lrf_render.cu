@@ -34,6 +34,7 @@
 // smallest step that holds the CTA: the default build's folded-MLP layout fits the 196 KB step, which leaves
 // the L1 60 KB for the texel gathers.
 #include "lrf_device.cuh"
+#include "lrf_launch.cuh"
 
 namespace lrf {
 
@@ -662,17 +663,13 @@ cudaError_t launch_render(const FieldDev& F, const BatchDev& B, int n_sms, int m
   if (nprod < 1) return cudaErrorInvalidConfiguration;
   const size_t smem = (size_t)smem_v3(F.S, floater, nprod, pe).total;
   const int variant = pe ? 1 : (F.grid16 ? 2 : 0);   // (bf16 grids with positional encodings are refused by the ABI)
-  static size_t configured[3][64] = {{0}, {0}, {0}};   // per kernel, per device: the attribute belongs to the device's context
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
   const void* kern = variant == 1 ? (const void*)render_kernel_t<true, false>
                    : variant == 2 ? (const void*)render_kernel_t<false, true> : (const void*)render_kernel_t<false, false>;
-  if (dev >= 0 && dev < 64 && smem > configured[variant][dev]) {
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[variant][dev] = smem;
-  }
+  cudaError_t e = set_max_dynamic_smem(kern, (int)smem);
+  if (e != cudaSuccess) return e;
+  int dev = 0;
+  e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
   // The shared-memory carveout is the smallest step that holds this launch's CTA, so the L1 gets the rest;
   // it is the code's choice, not the driver's.  A percentage that is not a step rounds up to the next step.
   static size_t carved[3][64] = {{0}, {0}, {0}};       // per kernel, per device: the CTA size the carveout was set for
@@ -692,9 +689,7 @@ cudaError_t launch_render(const FieldDev& F, const BatchDev& B, int n_sms, int m
   e = cudaMemsetAsync(B.sched, 0, 2 * sizeof(unsigned long long), stream);   // ray counter + finished-CTA counter
   if (e != cudaSuccess) return e;
   // a CTA per SM, but never more CTAs than there are groups of 8 rays
-  long long want = (B.n_rays + 7) / 8;
-  int grid = (int)(want < n_sms ? want : n_sms);
-  if (grid < 1) grid = 1;
+  const unsigned int grid = cta_count(B.n_rays, 8, n_sms, 1);
   if (variant == 1) render_kernel_t<true, false><<<grid, THREADS, smem, stream>>>(F, B, nprod);
   else if (variant == 2) render_kernel_t<false, true><<<grid, THREADS, smem, stream>>>(F, B, nprod);
   else render_kernel_t<false, false><<<grid, THREADS, smem, stream>>>(F, B, nprod);

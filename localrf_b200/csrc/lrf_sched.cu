@@ -7,6 +7,7 @@
 //   TV loss on planes / lines      TVLoss                              utils/utils.py:293-312
 //   sample_ray                     ray-AABB intersection sampler       models/tensorBase.py:396-417
 #include "lrf_device.cuh"
+#include "lrf_launch.cuh"
 
 namespace lrf {
 
@@ -346,31 +347,23 @@ cudaError_t launch_frame_u8(const float* rgb, int rgb_stride, const float* depth
                             double d_lo, double d_hi, const unsigned char* lut, unsigned char* rgb8,
                             unsigned char* depth8, int n_sms, cudaStream_t stream) {
   if (N == 0) return cudaSuccess;
-  long long b = (N + 255) / 256;
-  if (b > (long long)n_sms * 16) b = (long long)n_sms * 16;
-  frame_u8_kernel<<<(unsigned)b, 256, 0, stream>>>(rgb, rgb_stride, depth, depth_stride, N, (float)d_lo,
-                                                  (float)(d_hi - d_lo + 1e-8), lut, rgb8, depth8);
+  frame_u8_kernel<<<cta_count(N, 256, n_sms, 16), 256, 0, stream>>>(rgb, rgb_stride, depth, depth_stride, N,
+                                                                    (float)d_lo, (float)(d_hi - d_lo + 1e-8), lut,
+                                                                    rgb8, depth8);
   return cudaGetLastError();
 }
 
 // ---- launchers -------------------------------------------------------------------------------------------
-static inline unsigned blocks_for(long long n, int threads, int n_sms) {
-  long long b = (n + threads - 1) / threads;
-  const long long cap = (long long)n_sms * 16;
-  if (b > cap) b = cap;
-  return (unsigned)(b < 1 ? 1 : b);
-}
-
 cudaError_t launch_alpha_mask_build(const FieldDev& F, const float* aabb_max, const int* dims, float length,
                                     float thres, float* alpha_scratch, float* mask,
                                     unsigned long long* kept, int n_sms, cudaStream_t stream) {
   const long long n = (long long)dims[0] * dims[1] * dims[2];
   if (n == 0) return cudaSuccess;
-  dense_alpha_kernel<<<blocks_for(n, 256, n_sms), 256, 0, stream>>>(
+  dense_alpha_kernel<<<cta_count(n, 256, n_sms, 16), 256, 0, stream>>>(
       F, make_float3(aabb_max[0], aabb_max[1], aabb_max[2]), dims[0], dims[1], dims[2], length, alpha_scratch);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || !mask) return e;
-  alpha_pool_kernel<<<blocks_for(n, 256, n_sms), 256, 0, stream>>>(alpha_scratch, dims[0], dims[1], dims[2],
+  alpha_pool_kernel<<<cta_count(n, 256, n_sms, 16), 256, 0, stream>>>(alpha_scratch, dims[0], dims[1], dims[2],
                                                                    thres, mask, kept);
   return cudaGetLastError();
 }
@@ -379,13 +372,13 @@ cudaError_t launch_upsample(const float* src, int H, int W, float* dst, int H2, 
                             cudaStream_t stream) {
   const long long n = (long long)H2 * W2 * (C / 4);
   if (n == 0) return cudaSuccess;
-  upsample_kernel<<<blocks_for(n, 256, n_sms), 256, 0, stream>>>(src, H, W, dst, H2, W2, C / 4);
+  upsample_kernel<<<cta_count(n, 256, n_sms, 16), 256, 0, stream>>>(src, H, W, dst, H2, W2, C / 4);
   return cudaGetLastError();
 }
 
 cudaError_t launch_density_l1(const FieldDev& F, double* sum, int n_sms, cudaStream_t stream) {
   const long long N = (long long)F.g[0] * F.g[1] * F.g[2];
-  density_l1_fwd_kernel<<<blocks_for(N, 256, n_sms), 256, 0, stream>>>(F, N, sum);
+  density_l1_fwd_kernel<<<cta_count(N, 256, n_sms, 16), 256, 0, stream>>>(F, N, sum);
   return cudaGetLastError();
 }
 
@@ -406,7 +399,7 @@ cudaError_t launch_density_l1_backward(const FieldDev& F, const float* gout, flo
 cudaError_t launch_tv(const float* x, int H, int W, int C, double* sums, int n_sms, cudaStream_t stream) {
   const long long n = (long long)H * W * C;
   if (n == 0) return cudaSuccess;
-  tv_fwd_kernel<<<blocks_for(n, 256, n_sms), 256, 0, stream>>>(x, H, W, C, sums);
+  tv_fwd_kernel<<<cta_count(n, 256, n_sms, 16), 256, 0, stream>>>(x, H, W, C, sums);
   return cudaGetLastError();
 }
 
@@ -414,7 +407,7 @@ cudaError_t launch_tv_backward(const float* x, int H, int W, int C, const float*
                                float* dx, int n_sms, cudaStream_t stream) {
   const long long n = (long long)H * W * C;
   if (n == 0) return cudaSuccess;
-  tv_bwd_kernel<<<blocks_for(n, 256, n_sms), 256, 0, stream>>>(x, H, W, C, gout, kh, kw, dx);
+  tv_bwd_kernel<<<cta_count(n, 256, n_sms, 16), 256, 0, stream>>>(x, H, W, C, gout, kh, kw, dx);
   return cudaGetLastError();
 }
 
@@ -422,7 +415,7 @@ cudaError_t launch_sample_ray(const float* rays, const float* jitter, long long 
                               float near, float far, float step, float* pts, float* z,
                               unsigned char* inside, int n_sms, cudaStream_t stream) {
   if (N * S == 0) return cudaSuccess;
-  sample_ray_kernel<<<blocks_for(N * S, 256, n_sms), 256, 0, stream>>>(
+  sample_ray_kernel<<<cta_count(N * S, 256, n_sms, 16), 256, 0, stream>>>(
       rays, jitter, N, S, make_float3(aabb[0], aabb[1], aabb[2]), make_float3(aabb[3], aabb[4], aabb[5]),
       near, far, step, pts, z, inside);
   return cudaGetLastError();

@@ -18,6 +18,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "lrf_launch.cuh"
+
 namespace lrf {
 
 // order-preserving; every NaN becomes the canonical +NaN first, so that NaNs of either sign sort after +inf and
@@ -133,17 +135,11 @@ static __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const S
 __device__ inline float select_value(const SelectState& S) { return key32_to_f(S.prefix); }
 __device__ inline float select_next_value(const SelectState& S) { return key32_to_f(S.need_next ? S.next : S.prefix); }
 
-inline unsigned int select_grid_x(unsigned int n_max, int n_sms) {
-  const unsigned int want = (n_max + SEL_THREADS * 8 - 1) / (SEL_THREADS * 8);   // about 8 keys per thread
-  const unsigned int cap = (unsigned int)(n_sms > 0 ? n_sms : 132) * 8;
-  return want < 1 ? 1 : (want > cap ? cap : want);
-}
-
 // Enqueues the four passes over n_jobs <= SEL_MAX_JOBS jobs (states zeroed by the caller), and the successor pass
 // when a job asks for rank k + 1.
 inline cudaError_t launch_select(const SelectJobs& jobs, SelectState* st, int n_jobs, unsigned int n_max, int n_sms,
                                  cudaStream_t stream) {
-  const dim3 grid(select_grid_x(n_max, n_sms), (unsigned)n_jobs);
+  const dim3 grid(cta_count(n_max, SEL_THREADS * 8, n_sms, 8), (unsigned)n_jobs);   // about 8 keys per thread
   for (int pass = 0; pass < SEL_PASSES; ++pass) {
     select_hist_kernel<<<grid, SEL_THREADS, 0, stream>>>(jobs, st, pass);
     cudaError_t e = cudaGetLastError();

@@ -14,6 +14,7 @@
 // views in order) and no atomics, so the camera gradients are bitwise repeatable.
 #include "../../include/localrf_b200.h"
 #include "lrf_device.cuh"
+#include "lrf_launch.cuh"
 
 namespace lrf {
 
@@ -29,41 +30,24 @@ constexpr int PART = 8;            // per-view fp64 partials: d_world2rf [3], d_
 constexpr int CAM_THREADS = 256;
 constexpr int CAM_ACC = 24;        // d_cam2world [12], d_exposure [9], d_intrinsics [3]
 
-inline size_t al16(size_t x) { return (x + 15) & ~(size_t)15; }
-
 struct TrainScratch {
   float *rays, *dirs, *g_lin, *g_clip, *d_rays, *dpos;
   double* part;
   void* field;                     // the field backward's own block
 };
 
-// byte offsets in the order of the header's description; returns the total
-size_t train_scratch_layout(long long n, int S, long long V, unsigned char* base, TrainScratch* s) {
-  size_t off = 0;
-  const size_t o_rays = off;  off = al16(off + (size_t)n * 6 * 4);
-  const size_t o_dirs = off;  off = al16(off + (size_t)n * 3 * 4);
-  const size_t o_glin = off;  off = al16(off + (size_t)n * 3 * 4);
-  const size_t o_gclip = off; off = al16(off + (size_t)n * 3 * 4);
-  const size_t o_drays = off; off = al16(off + (size_t)n * 6 * 4);
-  const size_t o_part = off;  off = al16(off + (size_t)V * PART * 8);
-  const size_t o_dpos = off;  off = al16(off + (size_t)n * S * 3 * 4);
-  const size_t o_field = off; off = al16(off + backward_scratch_bytes(n, S));
-  if (base && s) {
-    s->rays = reinterpret_cast<float*>(base + o_rays);
-    s->dirs = reinterpret_cast<float*>(base + o_dirs);
-    s->g_lin = reinterpret_cast<float*>(base + o_glin);
-    s->g_clip = reinterpret_cast<float*>(base + o_gclip);
-    s->d_rays = reinterpret_cast<float*>(base + o_drays);
-    s->part = reinterpret_cast<double*>(base + o_part);
-    s->dpos = reinterpret_cast<float*>(base + o_dpos);
-    s->field = base + o_field;
-  }
-  return off;
-}
-
-int grid_for(long long n, int threads, int n_sms) {
-  const long long want = (n + threads - 1) / threads, cap = (long long)n_sms * 8;
-  return (int)(want < 1 ? 1 : (want < cap ? want : cap));
+// in the order of the header's description, each array 16-byte aligned
+TrainScratch carve(ScratchCarver& c, long long n, int S, long long V) {
+  TrainScratch s;
+  s.rays = c.take<float>((size_t)n * 6 * 4, 16);
+  s.dirs = c.take<float>((size_t)n * 3 * 4, 16);
+  s.g_lin = c.take<float>((size_t)n * 3 * 4, 16);
+  s.g_clip = c.take<float>((size_t)n * 3 * 4, 16);
+  s.d_rays = c.take<float>((size_t)n * 6 * 4, 16);
+  s.part = c.take<double>((size_t)V * PART * 8, 16);
+  s.dpos = c.take<float>((size_t)n * S * 3 * 4, 16);
+  s.field = c.take(backward_scratch_bytes(n, S), 16);
+  return s;
 }
 
 }  // namespace
@@ -182,13 +166,15 @@ __global__ void cam_final_kernel(const TrainScratch s, long long V, int fov360, 
 
 // ---- host-side launchers --------------------------------------------------------------------------
 size_t train_backward_scratch_bytes(long long n, int S, long long V) {
-  return train_scratch_layout(n, S, V, nullptr, nullptr);
+  ScratchCarver c(nullptr);
+  carve(c, n, S, V);
+  return c.size(16);
 }
 
 cudaError_t launch_exposure_clamp(const float* x, const float* E, long long n, long long V, float* rgb, int n_sms,
                                   cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
-  exposure_clamp_kernel<<<grid_for(n, 256, n_sms), 256, 0, stream>>>(x, E, n, n / V, rgb);
+  exposure_clamp_kernel<<<cta_count(n, 256, n_sms, 8), 256, 0, stream>>>(x, E, n, n / V, rgb);
   return cudaGetLastError();
 }
 
@@ -196,11 +182,11 @@ cudaError_t launch_render_backward_batch(const FieldDev& F, const BatchDev& B, c
                                          const float* g_rgb, const float* g_depth, const float* g_dirs,
                                          const LrfGradients& G, const LrfCameraGrads& CG, void* scratch,
                                          long long n_views, int n_sms, cudaStream_t stream) {
-  TrainScratch s;
-  train_scratch_layout(B.n_rays, F.S, n_views, static_cast<unsigned char*>(scratch), &s);
+  ScratchCarver c(scratch);
+  const TrainScratch s = carve(c, B.n_rays, F.S, n_views);
   cudaError_t e = cudaMemsetAsync(s.dpos, 0, (size_t)B.n_rays * F.S * 3 * 4, stream);
   if (e != cudaSuccess) return e;
-  ray_prologue_kernel<<<grid_for(B.n_rays, 256, n_sms), 256, 0, stream>>>(B, x, g_rgb, s);
+  ray_prologue_kernel<<<cta_count(B.n_rays, 256, n_sms, 8), 256, 0, stream>>>(B, x, g_rgb, s);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   LrfGradients G2 = G;

@@ -20,7 +20,7 @@ from gpu_helpers import oracle_field
 pytestmark = pytest.mark.gpu
 
 U = so.U32
-THREADS_PER_SM = 16 * 256          # blocks_for() in lrf_sched.cu: at most 16 blocks of 256 threads per SM
+THREADS_PER_SM = 16 * 256          # cta_count(..., 16) in lrf_sched.cu: at most 16 blocks of 256 threads per SM
 
 
 class TVLoss(torch.nn.Module):
