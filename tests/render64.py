@@ -1,14 +1,20 @@
 """float64 restatement of the training call, differentiated by torch autograd, with each ray's decision margins.
 
-What is restated (floater_thresh = 0, no positional encodings):
+What is restated:
   - TensorBase.forward (models/tensorBase.py:567-636): sample points o + (d / |d|) z, contract (utils/ray_utils.py:
     9-12), the alpha mask (trilinear, zero padding) on the contracted points, normalise_coord, the VM lookups with
     F.grid_sample(align_corners=True, padding_mode="border") (tensoRF.py:112-196), softplus(f + shift) or relu(f),
     alpha = 1 - exp(-sigma dist scale) with alpha[:, -1] = 1, T = cumprod(1 - alpha + 1e-10), w = alpha T, depth =
-    sum(w z) / |d|, the shading switch w > rayMarch_weight_thres, MLPRender_Fea_late_view (viewdirs detached) with
-    sigmoid, and the white background.
-  - The camera side of LocalTensorfs.forward (local_tensorfs.py:397-499, one field): pixel directions (lean or 360),
-    rays (t + world2rf, R dir), exposure E x and clamp(0, 1), whose backward passes the gradient at both bounds.
+    sum(w z) / |d|, the floater filter (tensorBase.py:617-620: idx = sum_k w_k k, alpha[k < idx thresh] = 0, the
+    weights again; acc and depth keep the pre-filter weights), the shading switch w > rayMarch_weight_thres,
+    MLPRender_Fea_late_view (viewdirs detached) with positional encodings fea_pe / view_pe 0..8 (the 27 features, then
+    sin (d-major, f-minor), then cos; zeros for the feature encoding when `refine` is 0) and sigmoid, and the white
+    background (the pre-filter acc).  field_forward's extras also give what the render kernel's early termination
+    leaves: the samples before the end of the 32-sample block in which T first falls below 1e-10 (`k_end`), the
+    valid samples marched and the samples shaded there (`n_march`, `n_shade`, what its `stats` counts).
+  - The camera side of LocalTensorfs.forward (local_tensorfs.py:397-499): pixel directions (lean or 360), rays (t +
+    world2rf, R dir), per-view blend and accumulation over several fields (render_views), exposure E x and clamp(0,
+    1), whose backward passes the gradient at both bounds.
 
 Every hard switch of that function is evaluated on the float64 values, and for each ray `margins` gives how close its
 float64 forward comes to each switch.  Where an fp32 implementation's error in the switched quantity grows along the
@@ -24,13 +30,24 @@ computation, the margin is in units of a propagated bound on that error (EPS = 2
   mlp       each of the 2 x featureC MLP pre-activations against 0 on each shaded sample, over its error: 8 EPS of
             the layer-1 sum of |terms| (folded W1 basis on the 72 products; a sum of independently rounded terms
             grows as the square root of its length) plus the position error through the products' slope; 8 EPS of
-            layer 2's plus layer 1's error through |W2|;
+            layer 2's plus layer 1's error through |W2|.  With positional encodings the 27 features are their own
+            sum (8 EPS of it plus the slope), and their error reaches layer 1 through the encoding: 2^f times it in
+            sin / cos of frequency f, plus 4 EPS for sin / cos themselves;
+  floater   |idx thresh - k| for the integer k nearest to idx thresh (the floater cut), over a bound on the fp32 idx
+            times thresh: sum_k w_err_k k, plus the rounding of a per-lane sequential sum of ceil(S / 32) terms and a
+            5-level warp tree (ceil(S / 32) + 6 EPS of sum_k w_k k), plus the product's rounding.  inf where the
+            filter is off, k is the last sample (its alpha is 1 either way) or alpha_k = 0 (the cut changes nothing).
+            With the filter, `thres` is measured on the filtered weights, whose product restarts at 1 and carries
+            only the errors of the alphas it keeps;
 and in units of EPS times the quantity's size where the rounding does not accumulate:
   contract  max|p| - 1 (p = o + vd z carries (|o| + |z|) EPS), and, where the point is contracted, the gap between
             the largest and second-largest |p_a| (the contraction's argmax, which routes the norm's gradient);
   mask      the alpha-mask value against 0 (its fp32 value is a sum of non-negative terms: only an exact 0 in one
             implementation and not the other flips it, which happens at a mask-cell boundary: the margin is the
             distance of the mask-lattice coordinate to the nearest integer, in units of (dim) EPS).
+Not a decision of the colour, but of what the kernel counts (`term`): |T_b - 1e-10| over T_b's propagated error,
+for the transmittance T_b at the end of each 32-sample block up to the one where the march stops (the kernel's
+early termination; inf with the floater filter, which marches every sample).
 The texel floors (`texel`): the distance of every un-clipped pixel coordinate ((q + 1) / 2) (size - 1) of the twelve
 lookups to the nearest integer in [0, size - 1] (unit: size EPS).  floor() chooses the cell, and the clip at 0 and
 size - 1 zeroes the position gradient, so only the position gradients (d_rays and what the cameras derive from it)
@@ -51,8 +68,9 @@ GRID_KEYS = [f"{n}.{i}" for n in ("density_plane", "density_line", "app_plane", 
 MLP_KEYS = ["basis_mat.weight", "renderModule.mlp.0.weight", "renderModule.mlp.0.bias", "renderModule.mlp.2.weight",
             "renderModule.mlp.2.bias", "renderModule.mlp_view.0.weight", "renderModule.mlp_view.0.bias"]
 PARAM_KEYS = GRID_KEYS + MLP_KEYS
-MARGIN_KEYS = ("thres", "contract", "mask", "relu_f", "softplus", "mlp")
-BOUND_KEYS = ("thres", "relu_f", "softplus", "mlp")     # margins in units of a propagated error bound
+MARGIN_KEYS = ("thres", "contract", "mask", "relu_f", "softplus", "mlp", "floater")
+BOUND_KEYS = ("thres", "relu_f", "softplus", "mlp", "floater")     # margins in units of a propagated error bound
+T_TERM = float(np.float32(1e-10))                       # the render kernel's early-termination transmittance (fp32)
 
 
 class Field64:
@@ -73,6 +91,8 @@ class Field64:
         self.scale = float(fd.get("distance_scale", 25.0))
         self.thres = float(fd.get("rayMarch_weight_thres", 1e-3))
         self.act = str(fd.get("fea2denseAct", "softplus"))
+        self.fea_pe = int(fd.get("fea_pe", 0))
+        self.view_pe = int(fd.get("view_pe", 0))
         self.device = device
 
     @staticmethod
@@ -83,20 +103,22 @@ class Field64:
         fd["distance_scale"] = float(m.distance_scale)
         fd["rayMarch_weight_thres"] = float(m.rayMarch_weight_thres if thres is None else thres)
         fd["fea2denseAct"] = m.fea2denseAct
+        fd["fea_pe"], fd["view_pe"] = int(m.fea_pe), int(m.view_pe)
         if m.alphaMask is None:
             fd.pop("alphaMask.alpha_volume", None)
         return Field64(fd, device)
 
 
 def random_field(grid=(9, 11, 13), act="softplus", shift=-2.0, thres=1e-3, seed=0, mask=None, aabb=2.0,
-                 safe_mlp=False, coarse=None):
+                 safe_mlp=False, coarse=None, fea_pe=0, view_pe=0):
     """A field dict (reference layout, float64 numpy, with the scalars module_from_golden reads) with random grids:
     density features of spread ~1.5, so softplus(f + shift) spans several decades.  `mask`: an alpha volume
     [1, 1, D, H, W] over the same aabb.  safe_mlp: both hidden layers' units biased +-1 alternately with weights
     small enough that no pre-activation comes near 0 (check it with the `mlp` margin); the MLP is then smooth on
     every sample, at any number of samples.  coarse: draw the grids at that resolution per axis and upsample them
     bilinearly (align_corners, as up_sampling_VM does) to `grid` -- a field as training leaves it after an upsample,
-    whose slope per unit length does not grow with the grid size."""
+    whose slope per unit length does not grow with the grid size.  fea_pe / view_pe: the MLP's positional
+    encodings (layer 1 then reads 27 (1 + 2 fea_pe) inputs, the view layer 128 + 3 (1 + 2 view_pe))."""
     rng = np.random.default_rng(seed)
     gx, gy, gz = grid
     hw, L = [(gy, gx), (gz, gx), (gz, gy)], [gz, gy, gx]
@@ -114,11 +136,12 @@ def random_field(grid=(9, 11, 13), act="softplus", shift=-2.0, thres=1e-3, seed=
         fd[f"app_plane.{i}"] = draw(0.3, 24, hw[i])
         fd[f"app_line.{i}"] = draw(1.0, 24, (L[i], 1))
     fd["basis_mat.weight"] = 0.2 * rng.standard_normal((27, 72))
-    fd["renderModule.mlp.0.weight"] = 0.2 * rng.standard_normal((128, 27))
+    n_in, n_view = 27 * (1 + 2 * fea_pe), 3 * (1 + 2 * view_pe)
+    fd["renderModule.mlp.0.weight"] = 0.2 * rng.standard_normal((128, n_in)) / math.sqrt(1 + 2 * fea_pe)
     fd["renderModule.mlp.0.bias"] = 0.1 * rng.standard_normal(128)
     fd["renderModule.mlp.2.weight"] = 0.1 * rng.standard_normal((128, 128))
     fd["renderModule.mlp.2.bias"] = 0.1 * rng.standard_normal(128)
-    fd["renderModule.mlp_view.0.weight"] = 0.3 * rng.standard_normal((3, 131))
+    fd["renderModule.mlp_view.0.weight"] = 0.3 * rng.standard_normal((3, 128 + n_view))
     fd["renderModule.mlp_view.0.bias"] = 0.1 * rng.standard_normal(3)
     if safe_mlp:
         sign = np.where(np.arange(128) % 2 == 0, 1.0, -1.0)
@@ -127,8 +150,8 @@ def random_field(grid=(9, 11, 13), act="softplus", shift=-2.0, thres=1e-3, seed=
         fd["renderModule.mlp.2.weight"] *= 0.05
         fd["renderModule.mlp.2.bias"] = sign
         fd["renderModule.mlp_view.0.weight"] *= 0.2         # keeps the sigmoid away from saturation
-    scal = dict(density_shift=shift, distance_scale=25.0, rayMarch_weight_thres=thres, fea2denseAct=act, fea_pe=0,
-                view_pe=0, featureC=128, app_dim=27, step_ratio=0.5, gridSize=list(grid))
+    scal = dict(density_shift=shift, distance_scale=25.0, rayMarch_weight_thres=thres, fea2denseAct=act,
+                fea_pe=fea_pe, view_pe=view_pe, featureC=128, app_dim=27, step_ratio=0.5, gridSize=list(grid))
     fd.update({k: np.asarray(v) for k, v in scal.items()})
     if mask is not None:
         fd["alphaMask.alpha_volume"] = np.asarray(mask, np.float64)
@@ -213,18 +236,31 @@ def _mask_value(F, p):
     return v, marg
 
 
-def _mlp(F, feats, vd, want_margin, qa=None, dqa=None):
-    """MLPRender_Fea_late_view (pe 0) on products feats [M, 72] -> rgb [M, 3], per-sample MLP margin [M] (in units
-    of the pre-activations' fp32 error bound; qa / dqa: the shaded points and their position error)."""
+def _pe(x, n_freq):
+    """[sin(x_d 2^f), cos(x_d 2^f)] with d-major, f-minor order (tensorBase.py:14-21)."""
+    bands = 2.0 ** torch.arange(n_freq, dtype=x.dtype, device=x.device)
+    ang = (x[..., None] * bands).reshape(*x.shape[:-1], -1)
+    return torch.cat([ang.sin(), ang.cos()], -1)
+
+
+def _mlp(F, feats, vd, want_margin, qa=None, dqa=None, refine=True):
+    """MLPRender_Fea_late_view on products feats [M, 72] -> rgb [M, 3], per-sample MLP margin [M] (in units of the
+    pre-activations' fp32 error bound; qa / dqa: the shaded points and their position error).  fea_pe / view_pe:
+    the 27 features, then sin, then cos of each feature times 2^f (zeros when refine is off); the view term
+    likewise (always encoded)."""
     p = F.p
     x = feats @ p["basis_mat.weight"].t()
+    enc = x
+    if F.fea_pe:
+        enc = torch.cat([x, _pe(x, F.fea_pe) if refine else x.new_zeros(x.shape[0], 2 * x.shape[1] * F.fea_pe)], -1)
     w1, b1, w2, b2 = p["renderModule.mlp.0.weight"], p["renderModule.mlp.0.bias"], p["renderModule.mlp.2.weight"], \
         p["renderModule.mlp.2.bias"]
-    a1 = x @ w1.t() + b1
+    a1 = enc @ w1.t() + b1
     h1 = torch.relu(a1)
     a2 = h1 @ w2.t() + b2
     h2 = torch.relu(a2)
-    s = torch.cat([h2, vd], -1) @ p["renderModule.mlp_view.0.weight"].t() + p["renderModule.mlp_view.0.bias"]
+    v = vd if not F.view_pe else torch.cat([vd, _pe(vd, F.view_pe)], -1)
+    s = torch.cat([h2, v], -1) @ p["renderModule.mlp_view.0.weight"].t() + p["renderModule.mlp_view.0.bias"]
     marg = None
     if want_margin:
         with torch.no_grad():
@@ -232,20 +268,35 @@ def _mlp(F, feats, vd, want_margin, qa=None, dqa=None):
             # rounded terms grows as its square root (8 EPS of the sum of |terms| covers 72 and 128 terms), plus the
             # position error through the features' slope; layer 2: plus layer 1's error through |W2| on the units
             # that are on.  The tensor-core path's 16-bit products need a 2^8 larger margin (the tests' bound).
-            w1b = (w1 @ p["basis_mat.weight"]).detach()
             keys = [(f"app_plane.{i}", f"app_line.{i}") for i in range(3)]
             fabs = torch.cat(_abs_sum(keys, qa, F), -1)
-            pre1 = lambda qq: torch.cat([_lookup(p[a].detach(), p[b].detach(), qq, i)
-                                         for i, (a, b) in enumerate(keys)], -1) @ w1b.t()
-            e1 = 8 * EPS * (fabs @ w1b.abs().t() + b1.abs()) + _slope(pre1, qa, dqa)
+            prods = lambda qq: torch.cat([_lookup(p[a].detach(), p[b].detach(), qq, i)
+                                          for i, (a, b) in enumerate(keys)], -1)
+            w1d = w1.detach()
+            if not (F.fea_pe or F.view_pe):
+                w1b = w1d @ p["basis_mat.weight"].detach()
+                e1 = 8 * EPS * (fabs @ w1b.abs().t() + b1.abs()) + _slope(lambda qq: prods(qq) @ w1b.t(), qa, dqa)
+            else:
+                # the 27 features are a sum of their own (layer 0); their error reaches layer 1 through the encoding:
+                # 2^f times it in sin / cos of frequency f (x 2^f is exact), plus 4 EPS for sin / cos themselves
+                basis = p["basis_mat.weight"].detach()
+                e0 = 8 * EPS * (fabs @ basis.abs().t()) + _slope(lambda qq: prods(qq) @ basis.t(), qa, dqa)
+                e_enc = e0
+                if F.fea_pe:
+                    bands = 2.0 ** torch.arange(F.fea_pe, dtype=e0.dtype, device=e0.device)
+                    e_f = (e0[..., None] * bands).reshape(e0.shape[0], -1) + 4 * EPS
+                    e_enc = torch.cat([e0, e_f, e_f] if refine else [e0, torch.zeros_like(e_f), torch.zeros_like(e_f)],
+                                      -1)
+                e1 = 8 * EPS * (enc.detach().abs() @ w1d.abs().t() + b1.abs()) + e_enc @ w1d.abs().t()
             e2 = 8 * EPS * (h1.abs() @ w2.abs().t() + b2.abs()) + (e1 * (a1 > 0)) @ w2.abs().t()
             marg = torch.minimum((a1.abs() / e1).amin(-1), (a2.abs() / e2).amin(-1))
     return torch.sigmoid(s), marg
 
 
-def field_forward(F, rays, z, white_bg, want_margins=False):
+def field_forward(F, rays, z, white_bg, want_margins=False, floater=0.0, refine=True):
     """TensorBase.forward on rays [n, 6] (float64, may require grad) with the distance table z [S] ->
-    (rgb [n, 3], depth [n], extras dict: w [n, S] and, with want_margins, the margins and `texel` [n])."""
+    (rgb [n, 3], depth [n], extras dict: w [n, S] (after the floater filter) and, with want_margins, the margins,
+    `texel` [n], `term` [n], and the early termination's `k_end`, `n_march` and `n_shade` [n])."""
     n, S = rays.shape[0], z.shape[0]
     dev, f64 = rays.device, torch.float64
     o, d = rays[:, :3], rays[:, 3:]
@@ -293,21 +344,29 @@ def field_forward(F, rays, z, white_bg, want_margins=False):
     w = alpha * T
     acc = w.sum(-1)
     depth = (w * zz[None]).sum(-1) / nrm[:, 0]
-    app = w > F.thres
+    wf, af, Tf = w, alpha, T
+    if floater > 0:                         # tensorBase.py:617-620; acc and depth keep the pre-filter weights
+        ks = torch.arange(S, dtype=f64, device=dev)
+        idx = (w * ks).sum(-1, keepdim=True)
+        af = torch.where(ks[None] < idx * floater, torch.zeros_like(alpha), alpha)
+        af = torch.cat([af[:, :-1], torch.ones_like(af[:, -1:])], -1)
+        Tf = torch.cumprod(torch.cat([torch.ones_like(af[:, :1]), 1.0 - af + 1e-10], -1), -1)[:, :-1]
+        wf = af * Tf
+    app = wf > F.thres
     rgb_s = torch.zeros(n, S, 3, dtype=f64, device=dev)
     mlp_m = torch.full((n, S), math.inf, dtype=f64, device=dev)
     if app.any():
         qa = q[app]
         feats = torch.cat([_lookup(F.p[f"app_plane.{i}"], F.p[f"app_line.{i}"], qa, i) for i in range(3)], -1)
         vda = vd[:, None, :].expand(n, S, 3)[app].detach()
-        col, mm = _mlp(F, feats, vda, want_margins, qa.detach(), dq[app] if want_margins else None)
+        col, mm = _mlp(F, feats, vda, want_margins, qa.detach(), dq[app] if want_margins else None, refine)
         rgb_s = rgb_s.index_put((app,), col)
         if want_margins:
             mlp_m[app] = mm
-    rgb = (w[..., None] * rgb_s).sum(-2)
+    rgb = (wf[..., None] * rgb_s).sum(-2)
     if white_bg:
         rgb = rgb + (1.0 - acc)[:, None]
-    ex = {"w": w.detach()}
+    ex = {"w": wf.detach()}
     if not want_margins:
         return rgb, depth, ex
     with torch.no_grad():
@@ -342,10 +401,46 @@ def field_forward(F, rays, z, white_bg, want_margins=False):
         relT = torch.cumsum(rel, -1) - rel
         # below 2^-126 fp32 is subnormal: its rounding there is absolute (and products flush to 0)
         ex["w_err"] = Td * dalpha + wd * (relT + EPS) + 2.0 ** -126
-        mk["thres"] = (wd - F.thres).abs() / ex["w_err"]
+        ks = torch.arange(S, dtype=f64, device=dev)
+        ta, tT, tw, terr = a, Td, wd, ex["w_err"]
+        if floater > 0:
+            # the cut k < idx thresh against the nearest integer; idx = sum_k w_k k carries each weight's error times
+            # k and the rounding of the kernel's sum (per lane ceil(S / 32) terms in sequence, then a warp tree)
+            idx = (wd * ks).sum(-1)
+            lim = idx * floater
+            kr = torch.round(lim)
+            idx_err = (ex["w_err"] * ks).sum(-1) + ((S + 31) // 32 + 6) * EPS * idx
+            fm = (lim - kr).abs() / (idx_err * floater + EPS * lim + 1e-300)
+            a_at = a.gather(1, kr.long().clamp(0, S - 1)[:, None])[:, 0]
+            mk["floater"] = torch.where((kr >= S - 1) | (a_at == 0), torch.full_like(fm, math.inf), fm)[:, None]
+            # the filtered product restarts at 1 and carries the errors of the alphas it keeps
+            ta, tT, tw = af.detach(), Tf.detach(), wf.detach()
+            daf = torch.where(ta == a, dalpha, torch.zeros_like(dalpha))
+            relf = daf / ((1 - ta) + 1e-10) + 3 * EPS
+            terr = tT * daf + tw * (torch.cumsum(relf, -1) - relf + EPS) + 2.0 ** -126
+            ex["w_err"] = terr
+        mk["thres"] = (tw - F.thres).abs() / terr
         if F.thres <= 0:      # an fp32 T below ~2^-126 is 0, and its w then fails w > 0 where float64's passes
-            mk["thres"] = torch.where(Td < 2.0 ** -100, torch.zeros_like(wd), mk["thres"])
-        mk["thres"] = torch.where(a == 0, inf, mk["thres"])    # sigma exactly 0: w = 0 on both sides
+            mk["thres"] = torch.where(tT < 2.0 ** -100, torch.zeros_like(tw), mk["thres"])
+        mk["thres"] = torch.where(ta == 0, inf, mk["thres"])    # sigma exactly 0 (or cut): w = 0 on both sides
+        # early termination (floater 0): the march stops after the 32-sample block whose end leaves T < 1e-10
+        nb = (S + 31) // 32
+        ends = torch.clamp(torch.arange(nb, device=dev) * 32 + 31, max=S - 1)
+        Tb = torch.cumprod(fac, -1)[:, ends]
+        eb = torch.cumsum(rel, -1)[:, ends]
+        hit = Tb < T_TERM                  # (an empty ray's last factor, (1 + 1e-10)^S 1e-10, can end above 1e-10f)
+        b_term = torch.where(hit.any(-1), hit.to(torch.int64).argmax(-1), nb - 1)
+        tm = (Tb - T_TERM).abs() / (Tb * eb + T_TERM * EPS)
+        reached = torch.arange(nb, device=dev)[None] <= b_term[:, None]
+        tm = torch.where(reached & (torch.arange(nb, device=dev)[None] < nb - 1), tm, torch.full_like(tm, math.inf))
+        k_end = torch.clamp((b_term + 1) * 32, max=S)
+        if floater > 0:                                         # the filter marches every sample
+            k_end, tm = torch.full_like(k_end, S), torch.full_like(tm, math.inf)
+        before = ks[None] < k_end[:, None]
+        ex["k_end"] = k_end
+        ex["term"] = tm.amin(-1)
+        ex["n_march"] = (valid & before).sum(-1)
+        ex["n_shade"] = (app & before).sum(-1)
         if F.act == "softplus":
             mk["softplus"] = torch.where(valid, (x - 20).abs() / (df + 20 * EPS), inf)
         else:
@@ -394,6 +489,22 @@ def field_backward(F, rays, z, white_bg, g_rgb, g_depth, want_margins=True, chun
     return grads, {k: torch.cat(v) for k, v in fwd.items()}
 
 
+def forward_chunked(F, rays, z, white_bg, floater=0.0, refine=True, chunk_samples=CHUNK_SAMPLES):
+    """field_forward with margins, without autograd, in chunks of rays -> dict: rgb, depth, w and the extras."""
+    dev = F.device
+    rays = torch.as_tensor(rays).to(dev, torch.float64)
+    z = torch.as_tensor(z).to(dev, torch.float64)
+    step = max(1, chunk_samples // z.shape[0])
+    out = {}
+    with torch.no_grad():
+        for r0 in range(0, rays.shape[0], step):
+            rgb, depth, ex = field_forward(F, rays[r0:r0 + step], z, white_bg, True, floater, refine)
+            ex["rgb"], ex["depth"] = rgb, depth
+            for k, v in ex.items():
+                out.setdefault(k, []).append(v)
+    return {k: torch.cat(v) for k, v in out.items()}
+
+
 def clear(fwd, bound=2.0, margin=64.0, mlp_bound=None):
     """Per ray: True where every decision margin clears its bound -- `bound` for the margins in units of a propagated
     error bound (BOUND_KEYS; `mlp_bound` for the MLP when given), `margin` for the others (EPS units)."""
@@ -420,6 +531,45 @@ def directions(ray_ids, W, H, intr, fov360):
         theta = i * 2 * math.pi / W + math.pi
         return torch.stack([torch.cos(phi) * torch.sin(theta), torch.sin(phi), torch.cos(phi) * torch.cos(theta)], -1)
     return torch.stack([(i - intr[1]) / intr[0], -(j - intr[2]) / intr[0], -torch.ones_like(i)], -1)
+
+
+def render_views(fields, z, ray_ids, W, H, fov360, intr, c2w, w2rf, blend, E, white_bg, floater=0.0, refine=True,
+                 finalize=True):
+    """The eval call of LocalTensorfs.forward in float64 (local_tensorfs.py:397-499): each ray's camera-space
+    direction and pixel from its id, its view r // (n / V), then for every field f the rays t_v + world2rf_f and
+    R_v dir, rendered and blended: rgb = sum_f blend[v, f] rgb_f (likewise depth); with `finalize`, clamp(E_v rgb, 0,
+    1) (E None: clamp only).  fields: Field64 list; w2rf: one [3] per field (or None); blend [V, n_fields] or None
+    (weight 1).  -> dict: rgb, depth, dirs [n, 3], ij [n, 2], per-field forward dicts `fwd` (forward_chunked), and
+    every margin and count of forward_chunked combined over the fields (smallest margin, summed counts)."""
+    dev, f64 = fields[0].device, torch.float64
+    T = lambda a: torch.as_tensor(a).to(dev, f64)
+    ray_ids = torch.as_tensor(ray_ids).to(dev)
+    n, V = ray_ids.shape[0], c2w.shape[0]
+    view = torch.arange(n, device=dev) // (n // V)
+    c2w, intr = T(c2w), T(intr)
+    dirs = directions(ray_ids, W, H, intr, fov360)
+    rays_d = (c2w[view, :, :3] @ dirs[:, :, None])[..., 0]
+    rgb = torch.zeros(n, 3, dtype=f64, device=dev)
+    depth = torch.zeros(n, dtype=f64, device=dev)
+    out = {"fwd": []}
+    for f, F in enumerate(fields):
+        o = c2w[view, :, 3] + (T(w2rf[f]) if w2rf is not None and w2rf[f] is not None else 0.0)
+        fw = forward_chunked(F, torch.cat([o, rays_d], -1), z, white_bg, floater, refine)
+        b = T(blend)[view, f] if blend is not None else torch.ones(n, dtype=f64, device=dev)
+        rgb = rgb + b[:, None] * fw["rgb"]
+        depth = depth + b * fw["depth"]
+        out["fwd"].append(fw)
+        for k in MARGIN_KEYS + ("texel", "term"):
+            out[k] = torch.minimum(out[k], fw[k]) if k in out else fw[k]
+        for k in ("n_march", "n_shade"):
+            out[k] = out[k] + fw[k] if k in out else fw[k]
+    if finalize:
+        if E is not None:
+            rgb = torch.einsum("nab,nb->na", T(E)[view], rgb)
+        rgb = rgb.clamp(0, 1)
+    ids = ray_ids.to(torch.int64)
+    out.update(rgb=rgb, depth=depth, dirs=dirs, ij=torch.stack([ids % W, (ids // W) % H], -1))
+    return out
 
 
 def train_backward(F, z, ray_ids, W, H, fov360, intr, c2w, w2rf, E, x, white_bg, g_rgb, g_depth, g_dirs,

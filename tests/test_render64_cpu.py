@@ -209,3 +209,119 @@ def test_clamp_margin_and_exact_bounds():
     # g' = g on both bounds: the identity exposure's gradient is the sum of x over the rays that pass
     dE = grads["d_exposure"][0]
     assert torch.allclose(dE[0], x[[0, 1, 3]].sum(0)) and torch.allclose(dE[1], x.sum(0))
+
+
+# ---- the floater filter and the positional encodings against the reference's goldens --------------------------------
+@pytest.mark.parametrize("name,case,floater,refine", [("cfg1_64", "eval_floater", 0.5, True),
+                                                      ("opaque_32", "eval_floater", 0.5, True),
+                                                      ("aniso_pe", "refine", 0.5, True),
+                                                      ("aniso_pe", "norefine", 0.0, False)])
+def test_forward_vs_reference_golden(name, case, floater, refine):
+    """The reference's own fp32 forward (floater_thresh 0.5; fea_pe = view_pe = 2 with refine on and off): rgb and
+    depth within 1e-5 of their scale and weights within 1e-6, on the rays clear of every decision (measured <= 3.3e-7
+    and 1.1e-7; the excluded rays are the MLP's near-zero pre-activations of these random MLPs).  The filter cuts
+    samples on many rays, so the pin is not that of the unfiltered forward."""
+    g = load_golden(name)
+    F = R.Field64(full_field_dict(g))
+    out = R.forward_chunked(F, g["rays"], g[case + ".z"], True, floater, refine)
+    keep = R.clear(out).numpy()
+    print(name, case, "rays excluded:", int((~keep).sum()), "of", keep.size)
+    assert keep.mean() > 0.6
+    errs = (scale_err(out["rgb"].numpy()[keep], g[case + ".rgb"][keep]),
+            scale_err(out["depth"].numpy()[keep], g[case + ".depth"][keep]),
+            float(np.abs(out["w"].numpy()[keep] - g[case + ".weights"][keep]).max()))
+    print(f"{name} {case}: rgb {errs[0]:.1e} depth {errs[1]:.1e} weights {errs[2]:.1e}")
+    assert errs[0] < 1e-5 and errs[1] < 1e-5 and errs[2] < 1e-6
+    if floater:
+        plain = R.forward_chunked(F, g["rays"], g[case + ".z"], True, 0.0, refine)
+        moved = (plain["w"] - out["w"]).abs().amax(-1) > 1e-3
+        assert int(moved.sum()) >= 0.2 * keep.size
+        assert torch.equal(plain["depth"], out["depth"])            # depth keeps the pre-filter weights
+
+
+def _floater_setup():
+    fd = _field(shift=0.0)
+    rays = _rays()
+    ex = _margins(fd, rays)
+    ks = torch.arange(Z.shape[0], dtype=torch.float64)
+    idx = (ex["w"] * ks).sum(-1)
+    return fd, rays, idx
+
+
+def test_margin_floater():
+    """floater_thresh that puts ray 2's cut idx thresh exactly on an integer: its margin is 0; half way between two
+    integers the margin is large."""
+    fd, rays, idx = _floater_setup()
+    k = math.floor(float(idx[2])) - 1
+    assert 1 <= k < Z.shape[0] - 1
+    F = R.Field64(fd)
+    on = R.forward_chunked(F, rays, Z, True, floater=k / float(idx[2]))
+    assert float(on["floater"][2]) < 1.0 and float(on["floater"].max()) > 1.0
+    off = R.forward_chunked(F, rays, Z, True, floater=(k + 0.5) / float(idx[2]))
+    assert float(off["floater"][2]) > 1e3
+    assert math.isinf(float(R.forward_chunked(F, rays, Z, True)["floater"].min()))     # no filter: no decision
+
+
+def test_margin_thres_after_floater():
+    """With the filter, `thres` is measured on the filtered weights: a threshold equal to a filtered weight that
+    differs from the unfiltered one sits on the switch."""
+    fd, rays, idx = _floater_setup()
+    fl = 0.5
+    F = R.Field64(fd)
+    out = R.forward_chunked(F, rays, Z, True, floater=fl)
+    plain = _margins(fd, rays)
+    r, k = [int(v) for v in torch.nonzero((out["w"] - plain["w"]).abs() > 1e-3)[-1]]
+    fd["rayMarch_weight_thres"] = float(out["w"][r, k])
+    out2 = R.forward_chunked(R.Field64(fd), rays, Z, True, floater=fl)
+    assert float(out2["thres"][r]) == 0.0 and float(out2["thres"].max()) > 1.0
+
+
+def test_margin_mlp_positional_encodings():
+    """fea_pe = 3, view_pe = 2: a layer-1 unit whose pre-activation (encoded input, refine on) is 0 on one sample is
+    flagged; with refine off the encoded inputs are zeros, and the same unit's pre-activation moves off 0."""
+    fd = _field(thres=0.0, fea_pe=3, view_pe=2, safe_mlp=True)
+    rays = _rays()
+    F = R.Field64(fd)
+    with torch.no_grad():
+        rc = torch.as_tensor(rays[4:5], dtype=torch.float64)
+        o, d = rc[:, :3], rc[:, 3:] / rc[:, 3:].norm()
+        p = o + d * Z[3]
+        am = p.abs().amax(-1, keepdim=True)
+        pc = torch.where(am <= 1, p, (2 * am - 1) / am ** 2 * p)
+        feats = torch.cat([R._lookup(F.p[f"app_plane.{i}"], F.p[f"app_line.{i}"], pc / 2, i) for i in range(3)], -1)
+        x = feats @ F.p["basis_mat.weight"].t()
+        enc = torch.cat([x, R._pe(x, 3)], -1)
+        a = float((enc @ F.p["renderModule.mlp.0.weight"].t())[0, 17])
+    fd["renderModule.mlp.0.bias"][17] = -a
+    on = R.forward_chunked(R.Field64(fd), rays, Z, True)
+    assert float(on["mlp"][4]) < 1.0 and float(on["mlp"].max()) > 1.0
+    off = R.forward_chunked(R.Field64(fd), rays, Z, True, refine=False)
+    assert float(off["mlp"][4]) > float(on["mlp"][4])
+
+
+def test_margin_term_and_counts():
+    """A distance scale that puts ray 1's transmittance at the end of the first 32-sample block on 1e-10 (fp32) is
+    flagged by `term`; below it the march stops after that block (k_end = 32: the marched and shaded counts only
+    reach the first block), above it the ray marches all 40 samples."""
+    fd, rays = _field(), _rays()
+
+    def tb(scale):
+        fd["distance_scale"] = scale
+        return R.forward_chunked(R.Field64(fd), rays, Z, True)
+
+    lo, hi = math.log(1.0), math.log(1e5)
+    for _ in range(70):                       # T at the block end falls as the scale grows
+        mid = 0.5 * (lo + hi)
+        out = tb(math.exp(mid))
+        if int(out["k_end"][1]) == 32:
+            hi = mid
+        else:
+            lo = mid
+    on = tb(math.exp(hi))
+    assert int(on["k_end"][1]) == 32 and float(on["term"][1]) < 1.0
+    above = tb(math.exp(lo) * 0.5)
+    assert int(above["k_end"][1]) == 40 and float(above["term"][1]) > 1.0
+    below = tb(math.exp(hi) * 2)
+    assert int(below["k_end"][1]) == 32 and float(below["term"][1]) > 1.0
+    assert int(below["n_march"][1]) == 32 and int(above["n_march"][1]) == 39
+    assert int(below["n_shade"][1]) == int((below["w"][1, :32] > float(fd["rayMarch_weight_thres"])).sum())
