@@ -175,10 +175,17 @@ int lrf_render(const LrfField *field, const void *prepared, const LrfBatch *batc
 
 /* basis_mat + MLPRender_Fea_late_view.forward (tensoRF.py:196 + tensorBase.py:115-135, pe = 0) on
  * explicit inputs: feats [M][72] = the plane x line products (tensoRF.py:192-194 order: plane-major,
- * channel-minor), viewdirs [M][3] normalised -> rgb [M][3].  Same tensor-core code as lrf_render. */
+ * channel-minor), viewdirs [M][3] normalised -> rgb [M][3].  Same tensor-core code as lrf_render.
+ * `prepared` must be 16-byte aligned (it is staged by TMA bulk copies); feats / viewdirs / rgb may be NULL
+ * when M = 0, which enqueues nothing.  M < 0 is LRF_ERR_INVALID. */
 int lrf_mlp_forward(const void *prepared, const float *feats, const float *viewdirs, int64_t M,
                     float *rgb, lrf_stream_t stream);
 
+/* The lookups below and their backward read F.grid_sample(align_corners=True, padding_mode="border") at
+ * xyz_norm: a coordinate outside [-1, 1], +-inf included, clips to the border texel.  NaN reads texel 0 of
+ * that axis (no NaN reaches the output) and, like a clipped coordinate, gets a zero position gradient.
+ * xyz_norm / out / grad_out / d_xyz need only float alignment and may be NULL when M = 0 (nothing is
+ * enqueued); M < 0 is LRF_ERR_INVALID. */
 /* compute_densityfeature (tensoRF.py:112-151): xyz_norm [M][3] in [-1,1]^3 -> out [M] */
 int lrf_density_feature(const LrfField *field, const float *xyz_norm, int64_t M, float *out,
                         lrf_stream_t stream);
@@ -188,12 +195,12 @@ int lrf_app_feature(const LrfField *field, const float *xyz_norm, int64_t M, flo
 
 /* ---- differentiable lookups (the composed training path; SURVEY.md §8f rank 1) -------------------
  * The 72 plane x line products of compute_appfeature BEFORE basis_mat (tensoRF.py:174-194 order):
- * xyz_norm [M][3] -> out [M][3*n_acomp]. */
+ * xyz_norm [M][3] -> out [M][3*n_acomp].  `out` must be 16-byte aligned (float4 stores). */
 int lrf_app_products(const LrfField *field, const float *xyz_norm, int64_t M, float *out,
                      lrf_stream_t stream);
 /* Backward of lrf_density_feature (autograd of F.grid_sample x6 + product-sum, tensoRF.py:112-151):
- * grad_out [M]; d_plane[i] / d_line[i] have the layout of the parameters and are ACCUMULATED into
- * (atomic adds; zero them first); d_xyz [M][3] is overwritten (may be NULL). */
+ * grad_out [M]; d_plane[i] / d_line[i] have the layout of the parameters, must be 16-byte aligned (float4
+ * atomic adds) and are ACCUMULATED into (zero them first); d_xyz [M][3] is overwritten (may be NULL). */
 int lrf_density_feature_backward(const LrfField *field, const float *xyz_norm,
                                  const float *grad_out, int64_t M, float *const d_plane[3],
                                  float *const d_line[3], float *d_xyz, lrf_stream_t stream);
@@ -604,7 +611,7 @@ int lrf_test_panels(const LrfPanelFrame *frame, void *scratch, size_t scratch_by
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */
 int lrf_pack_bf16(const float *src, void *dst, int64_t n, lrf_stream_t stream);
 
-/* [C][H][W] (contiguous NCHW parameter of the reference) -> [H][W][C] */
+/* [C][H][W] (contiguous NCHW parameter of the reference) -> [H][W][C]; float alignment suffices */
 int lrf_repack_nchw_to_nhwc(const float *src, float *dst, int32_t C, int32_t H, int32_t W,
                             lrf_stream_t stream);
 

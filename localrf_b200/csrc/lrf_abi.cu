@@ -458,7 +458,9 @@ int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const
 int lrf_mlp_forward(const void* prepared, const float* feats, const float* viewdirs, int64_t M,
                     float* rgb, lrf_stream_t stream) {
   if (!prepared) return fail(LRF_ERR_INVALID, "prepared is NULL (call lrf_field_prepare first)");
+  if ((uintptr_t)prepared & 15) return fail(LRF_ERR_INVALID, "prepared must be 16-byte aligned");
   if (M < 0 || (M > 0 && (!feats || !viewdirs || !rgb))) return fail(LRF_ERR_INVALID, "bad feats/viewdirs/rgb/M");
+  if (M == 0) return LRF_OK;
   DevInfo d;
   int rc = device_info(d);
   if (rc != LRF_OK) return rc;
@@ -492,13 +494,19 @@ int lrf_app_products(const LrfField* f, const float* xyz, int64_t M, float* out,
   int rc = make_field(f, false, false, nullptr, F);
   if (rc != LRF_OK) return rc;
   if (M < 0 || (M > 0 && (!xyz || !out))) return fail(LRF_ERR_INVALID, "bad xyz/out/M");
+  if ((uintptr_t)out & 15) return fail(LRF_ERR_INVALID, "out must be 16-byte aligned");
   return cuda_status(lrf::launch_app_products(F, xyz, M, out, (cudaStream_t)stream), "app_products_kernel");
 }
 
-static int check_grads(float* const d_plane[3], float* const d_line[3]) {
+// the plane / line gradient buffers of the lookups' backward and lrf_density_l1_backward; `aligned16`: the lookups'
+// backward adds into them with 16-byte vector atomics (lrf_density_l1_backward's scalar adds need float alignment only)
+static int check_grads(float* const d_plane[3], float* const d_line[3], bool aligned16) {
   if (!d_plane || !d_line) return fail(LRF_ERR_INVALID, "gradient pointer arrays are NULL");
-  for (int i = 0; i < 3; ++i)
+  for (int i = 0; i < 3; ++i) {
     if (!d_plane[i] || !d_line[i]) return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
+    if (aligned16 && (((uintptr_t)d_plane[i] | (uintptr_t)d_line[i]) & 15))
+      return fail(LRF_ERR_INVALID, "plane/line gradient buffers must be 16-byte aligned");
+  }
   return LRF_OK;
 }
 
@@ -508,7 +516,7 @@ int lrf_density_feature_backward(const LrfField* f, const float* xyz, const floa
   lrf::FieldDev F;
   int rc = make_field(f, false, false, nullptr, F);
   if (rc != LRF_OK) return rc;
-  if ((rc = check_grads(d_plane, d_line)) != LRF_OK) return rc;
+  if ((rc = check_grads(d_plane, d_line, true)) != LRF_OK) return rc;
   if (M < 0 || (M > 0 && (!xyz || !gout))) return fail(LRF_ERR_INVALID, "bad xyz/grad_out/M");
   return cuda_status(lrf::launch_density_backward(F, d_plane, d_line, xyz, gout, M, d_xyz,
                                                   (cudaStream_t)stream), "density_backward_kernel");
@@ -520,7 +528,7 @@ int lrf_app_products_backward(const LrfField* f, const float* xyz, const float* 
   lrf::FieldDev F;
   int rc = make_field(f, false, false, nullptr, F);
   if (rc != LRF_OK) return rc;
-  if ((rc = check_grads(d_plane, d_line)) != LRF_OK) return rc;
+  if ((rc = check_grads(d_plane, d_line, true)) != LRF_OK) return rc;
   if (M < 0 || (M > 0 && (!xyz || !gout))) return fail(LRF_ERR_INVALID, "bad xyz/grad_out/M");
   return cuda_status(lrf::launch_app_products_backward(F, d_plane, d_line, xyz, gout, M, d_xyz,
                                                        (cudaStream_t)stream), "app_products_backward_kernel");
@@ -653,7 +661,7 @@ int lrf_density_l1_backward(const LrfField* f, const float* grad_out, float* con
   int rc = make_field(f, false, false, nullptr, F);
   if (rc != LRF_OK) return rc;
   if (!grad_out) return fail(LRF_ERR_INVALID, "grad_out is NULL");
-  if ((rc = check_grads(d_plane, d_line)) != LRF_OK) return rc;
+  if ((rc = check_grads(d_plane, d_line, false)) != LRF_OK) return rc;
   return cuda_status(lrf::launch_density_l1_backward(F, grad_out, d_plane, d_line,
                                                      (cudaStream_t)stream), "density_l1_bwd_kernel");
 }

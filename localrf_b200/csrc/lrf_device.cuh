@@ -483,11 +483,12 @@ __device__ __forceinline__ float sample_alpha(const FieldDev& F, const RaySm& R,
 }
 
 // ---- backward of the VM lookup (F.grid_sample align_corners=True, padding_mode="border") ----------------
-// pixel coordinate, its two taps and d(pixel)/d(normalised coordinate) (0 when clipped: ATen clip_coordinates_set_grad)
+// pixel coordinate, its two taps and d(pixel)/d(normalised coordinate) (0 when clipped: ATen clip_coordinates_set_grad;
+// 0 for NaN too, which the clamp below reads as texel 0)
 __device__ __forceinline__ void grid_coord_grad(float c, int size, int& i0, int& i1, float& t,
                                                 float& dcoord) {
   float x = ((c + 1.0f) * 0.5f) * (float)(size - 1);
-  dcoord = (x <= 0.0f || x >= (float)(size - 1)) ? 0.0f : 0.5f * (float)(size - 1);
+  dcoord = (x > 0.0f && x < (float)(size - 1)) ? 0.5f * (float)(size - 1) : 0.0f;
   x = fminf((float)(size - 1), fmaxf(x, 0.0f));
   const float f = floorf(x);
   i0 = (int)f;

@@ -148,7 +148,7 @@ def random_field(grid=(9, 11, 13), act="softplus", shift=-2.0, thres=1e-3, seed=
         fd["renderModule.mlp.0.weight"] *= 0.05
         fd["renderModule.mlp.0.bias"] = sign
         fd["renderModule.mlp.2.weight"] *= 0.05
-        fd["renderModule.mlp.2.bias"] = sign
+        fd["renderModule.mlp.2.bias"] = sign.copy()        # its own array: Field64's two leaves would share storage
         fd["renderModule.mlp_view.0.weight"] *= 0.2         # keeps the sigmoid away from saturation
     scal = dict(density_shift=shift, distance_scale=25.0, rayMarch_weight_thres=thres, fea2denseAct=act,
                 fea_pe=fea_pe, view_pe=view_pe, featureC=128, app_dim=27, step_ratio=0.5, gridSize=list(grid))
@@ -458,9 +458,11 @@ def field_forward(F, rays, z, white_bg, want_margins=False, floater=0.0, refine=
     return rgb, depth, ex
 
 
-def field_backward(F, rays, z, white_bg, g_rgb, g_depth, want_margins=True, chunk_samples=CHUNK_SAMPLES):
+def field_backward(F, rays, z, white_bg, g_rgb, g_depth, want_margins=True, chunk_samples=CHUNK_SAMPLES,
+                   floater=0.0, refine=True):
     """Chunked forward + autograd: -> (grads dict keyed like PARAM_KEYS plus "rays" [n, 6], forward dict with
-    rgb, depth, w and the per-ray margins).  Cotangents may be zero on any ray: that ray then adds exactly nothing."""
+    rgb, depth, w and the per-ray margins).  Cotangents may be zero on any ray: that ray then adds exactly nothing.
+    floater / refine as in field_forward (the floater cut is a hard switch: no gradient flows through idx)."""
     dev = F.device
     rays = torch.as_tensor(rays).to(dev, torch.float64)
     g_rgb = torch.as_tensor(g_rgb).to(dev, torch.float64)
@@ -474,7 +476,7 @@ def field_backward(F, rays, z, white_bg, g_rgb, g_depth, want_margins=True, chun
     for r0 in range(0, n, step):
         r1 = min(n, r0 + step)
         rc = rays[r0:r1].clone().requires_grad_(True)
-        rgb, depth, ex = field_forward(F, rc, z, white_bg, want_margins)
+        rgb, depth, ex = field_forward(F, rc, z, white_bg, want_margins, floater, refine)
         loss = (rgb * g_rgb[r0:r1]).sum() + (depth * g_depth[r0:r1]).sum()
         keys = list(F.p)
         gs = torch.autograd.grad(loss, [rc] + [F.p[k] for k in keys], allow_unused=True)

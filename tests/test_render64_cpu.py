@@ -325,3 +325,49 @@ def test_margin_term_and_counts():
     assert int(below["k_end"][1]) == 32 and float(below["term"][1]) > 1.0
     assert int(below["n_march"][1]) == 32 and int(above["n_march"][1]) == 39
     assert int(below["n_shade"][1]) == int((below["w"][1, :32] > float(fd["rayMarch_weight_thres"])).sum())
+
+
+# ---- field_backward with the floater filter and refine: against central differences -------------------------------
+def _directional(F, rays, z, g_rgb, g_depth, floater, refine, v, v_rays, h):
+    """(L(theta + h v) - L(theta - h v)) / 2h, L = sum(rgb g_rgb) + sum(depth g_depth), and the hard decisions (the
+    filtered alphas' zeros and the shading switch) at both ends."""
+    vals, cuts = [], []
+    with torch.no_grad():
+        for s in (1.0, -1.0):
+            for k in R.PARAM_KEYS:
+                F.p[k].add_(s * h * v[k])
+            rgb, depth, ex = R.field_forward(F, rays + s * h * v_rays, z, True, False, floater, refine)
+            for k in R.PARAM_KEYS:
+                F.p[k].sub_(s * h * v[k])
+            vals.append(float((rgb * g_rgb).sum() + (depth * g_depth).sum()))
+            cuts.append(((ex["w"] == 0), ex["w"] > F.thres))
+    return (vals[0] - vals[1]) / (2 * h), cuts
+
+
+@pytest.mark.parametrize("floater,refine,pe", [(0.5, True, (0, 0)), (0.5, True, (2, 1)), (0.0, False, (3, 0)),
+                                               (0.3, False, (2, 2))])
+def test_field_backward_floater_refine_vs_central_differences(floater, refine, pe):
+    """field_backward(floater, refine) on a small field: the gradient's projection on random directions (every
+    parameter and the ray origins at once) equals a float64 central difference within 1e-6 relative, on rays whose every
+    decision clears its margin (render64.clear) and whose filter cut and shading switch stay put across +-h."""
+    fd = R.random_field((9, 11, 13), shift=0.0, seed=5, fea_pe=pe[0], view_pe=pe[1], safe_mlp=True)
+    F = R.Field64(fd)
+    rays = torch.as_tensor(_rays(16, seed=3), dtype=torch.float64)
+    fw = R.forward_chunked(F, rays, Z, True, floater=floater, refine=refine)
+    keep = R.clear(fw, bound=4.0, margin=256.0) & (fw["texel"] >= 4.0)
+    assert int(keep.sum()) >= 8, int(keep.sum())
+    g_rgb, g_depth = (torch.as_tensor(c, dtype=torch.float64) for c in _cot(16, seed=7))
+    g_rgb, g_depth = g_rgb * keep[:, None], g_depth * keep
+    grads, _ = R.field_backward(F, rays, Z, True, g_rgb, g_depth, want_margins=False, floater=floater, refine=refine)
+    gen = torch.Generator().manual_seed(9)
+    for trial in range(3):
+        v = {k: torch.randn(F.p[k].shape, generator=gen, dtype=torch.float64) for k in R.PARAM_KEYS}
+        # origins only: the MLP reads the view direction detached (as the reference does), so d's gradient is partial
+        v_rays = torch.randn(rays.shape, generator=gen, dtype=torch.float64) * keep[:, None]
+        v_rays[:, 3:] = 0
+        proj = sum(float((grads[k] * v[k]).sum()) for k in R.PARAM_KEYS) + float((grads["rays"] * v_rays).sum())
+        fd_, cuts = _directional(F, rays, Z, g_rgb, g_depth, floater, refine, v, v_rays, 1e-6)
+        for a, b in zip(cuts[0], cuts[1]):
+            assert torch.equal(a[keep], b[keep]), "a decision moved within +-h"
+        print(f"floater {floater} refine {refine} pe {pe}: projection {proj:.6e}, central difference {fd_:.6e}")
+        assert abs(proj - fd_) <= 1e-6 * max(abs(proj), 1.0), (trial, proj, fd_)
