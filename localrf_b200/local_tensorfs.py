@@ -23,7 +23,7 @@ import torch
 from . import _lib
 from .optim import adam_step, zero_grad
 from .tensorf import (AlphaGridMask, TensorVMSplit, _check_field_state, _field_grad_buffers, _field_grads,
-                      _field_state, _ptr, _require_cuda, _stream)
+                      _field_state, _key, _memo, _ptr, _require_cuda, _stream)
 from .utils import N_to_reso, mtx_to_sixD, sixD_to_mtx
 
 
@@ -553,17 +553,6 @@ class LocalTensorfs(torch.nn.Module):
             return outs[0]
         return tuple(torch.cat([o[i] for o in outs]) for i in range(4))
 
-    def _cached(self, slot, key, build, refs=()):
-        """Small memo for tensors derived from parameters: rebuilt when the key changes.  Keys are made
-        of ids + version counters of the source tensors; `refs` keeps those tensors alive while the
-        entry exists, so a freed tensor's id can never be reused by a different one."""
-        c = self.__dict__.setdefault("_memo", {})
-        hit = c.get(slot)
-        if hit is None or hit[0] != key:
-            hit = (key, build(), tuple(refs))
-            c[slot] = hit
-        return hit[1]
-
     def _train_node_covers(self, k, floater_thresh):
         """Whether a training call of field k runs as one _TrainRenderFn node: the fields _RenderFn covers
         (pe = 0, no floater filter) unless LRF_TRAIN_PATH=composed selects the torch-op path."""
@@ -573,7 +562,7 @@ class LocalTensorfs(torch.nn.Module):
 
     def _blend_host(self):
         bw = self.blending_weights
-        return self._cached("bw_host", (id(bw), bw._version), lambda: bw.detach().cpu(), refs=[bw])
+        return _memo(self, "bw_host", _key((bw,)), lambda _: bw.detach().cpu(), (bw,))
 
     def forward(self, ray_ids, view_ids, W, H, white_bg=True, is_train=True, cam2world=None,
                 world2rf=None, blending_weights=None, chunk=16384, test_id=False,
@@ -713,18 +702,16 @@ class LocalTensorfs(torch.nn.Module):
             guards.append((P, "blending_weights", self.blending_weights, self.blending_weights._version))
         if cam2world is None:
             src = [self.r_c2w[i] for i in ids] + [self.t_c2w[i] for i in ids]
-            key = (tuple(ids), tuple((id(t), t._version) for t in src), str(dev))
-            cam2world = self._cached("c2w", key, lambda: self.get_cam2world(ids).detach()
-                                     .to(dev, torch.float32).contiguous(), refs=src)
+            cam2world = _memo(self, "c2w", (tuple(ids), _key(src), str(dev)),
+                              lambda _: self.get_cam2world(ids).detach().to(dev, torch.float32).contiguous(), src)
             for i in set(ids):     # (guards index the lists' _parameters dicts: ~10x cheaper than __getitem__)
                 guards.append((self.r_c2w._parameters, str(i), self.r_c2w[i], self.r_c2w[i]._version))
                 guards.append((self.t_c2w._parameters, str(i), self.t_c2w[i], self.t_c2w[i]._version))
         else:
             cam2world = cam2world.detach().to(dev, torch.float32).contiguous()
         src = [self.init_focal, self.focal_offset, self.center_rel]
-        key = (W, H, self.W, tuple((id(t), t._version) for t in src), str(dev))
-        intr = self._cached("intr", key, lambda: self._intrinsics(W, H).detach().to(dev, torch.float32).contiguous(),
-                            refs=src)
+        intr = _memo(self, "intr", (W, H, self.W, _key(src), str(dev)),
+                     lambda _: self._intrinsics(W, H).detach().to(dev, torch.float32).contiguous(), src)
         for name in ("init_focal", "focal_offset", "center_rel"):
             guards.append((P, name, P[name], P[name]._version))
         exposure = None
@@ -733,8 +720,8 @@ class LocalTensorfs(torch.nn.Module):
             used = sorted(set(ids + ([max(v - 1, 0) for v in ids] + [min(v + 1, n_e - 1) for v in ids]
                                      + [min(1, n_e - 1), max(n_e - 2, 0)] if test_id else [])))
             src = [self.exposure[i] for i in used]
-            key = (tuple(ids), bool(test_id), n_e, tuple((id(t), t._version) for t in src), str(dev))
-            exposure = self._cached("expo", key, lambda: self._exposure_for(ids, test_id, dev).detach(), refs=src)
+            exposure = _memo(self, "expo", (tuple(ids), bool(test_id), n_e, _key(src), str(dev)),
+                             lambda _: self._exposure_for(ids, test_id, dev).detach(), src)
             for i, t in zip(used, src):
                 guards.append((self.exposure._parameters, str(i), t, t._version))
 

@@ -19,6 +19,7 @@ physically [H][W][C] / [L][C] -- one texel's components are one 32-byte (density
 (appearance) contiguous run, which is what the kernel gathers.
 """
 import ctypes as C
+import operator
 import os
 
 import torch
@@ -28,6 +29,38 @@ from . import _lib
 
 MAT_MODE = ((0, 1), (0, 2), (1, 2))   # models/tensorBase.py:274
 VEC_MODE = (2, 1, 0)                  # models/tensorBase.py:275
+
+# The field's 19 tensors in _grad_params order: (LrfField slot, index in the slot's array of three or None, module
+# attribute).  TensorBase._tensors reads them in this order; the gradient of slot s is LrfGradients.d_<s>, except
+# that basis and w1 share d_w1b (the kernels read their product w1 @ basis).
+_FIELD_TENSORS = (
+    *((slot, i, f"{attr}.{i}") for slot, attr in (("dplane", "density_plane"), ("dline", "density_line"),
+                                                  ("aplane", "app_plane"), ("aline", "app_line")) for i in range(3)),
+    ("basis", None, "basis_mat.weight"), ("w1", None, "renderModule.mlp.0.weight"),
+    ("b1", None, "renderModule.mlp.0.bias"), ("w2", None, "renderModule.mlp.2.weight"),
+    ("b2", None, "renderModule.mlp.2.bias"), ("w3", None, "renderModule.mlp_view.0.weight"),
+    ("b3", None, "renderModule.mlp_view.0.bias"))
+
+# _memo slots of a field's LrfFields, [bf16][without a distance table]
+_FIELD_SLOTS = (("field", "field without table"), ("field16", "field16 without table"))
+
+_data_ptr, _version = torch.Tensor.data_ptr, operator.attrgetter("_version")
+
+
+def _key(tensors):
+    """Memo key of tensors: their addresses and version counters (an in-place update bumps the counter)."""
+    return tuple(map(_data_ptr, tensors)), tuple(map(_version, tensors))
+
+
+def _memo(owner, slot, key, build, refs=()):
+    """The object `owner` derives under `slot`: build(previous object or None) when the slot is empty or was built
+    under another key.  The entry holds `refs` (the tensors the key was made from), so none of them can be freed
+    and its address reused by another tensor while the entry exists."""
+    memo = owner.__dict__.setdefault("_memo", {})
+    hit = memo.get(slot)
+    if hit is None or hit[0] != key:
+        hit = memo[slot] = (key, build(None if hit is None else hit[1]), refs)
+    return hit[1]
 
 
 def _ptr(t):
@@ -50,6 +83,14 @@ def _require_cuda(t, what):
             "(there is no CPU fallback)")
 
 
+def _grid_grads(grids):
+    """Zeroed gradient buffers of three planes and three lines, laid out like them (channel-last), and the two
+    `void* [3]` arrays of their addresses -> (buffers, planes, lines)."""
+    bufs = [torch.zeros_like(t, memory_format=torch.channels_last) for t in grids]
+    return (bufs, (C.c_void_p * 3)(*[t.data_ptr() for t in bufs[:3]]),
+            (C.c_void_p * 3)(*[t.data_ptr() for t in bufs[3:]]))
+
+
 class _VMLookup(torch.autograd.Function):
     """Differentiable VM lookups of the training path: forward and backward are CUDA kernels behind
     the C ABI (lrf_density_feature / lrf_app_products and their *_backward); gradients reach the
@@ -69,29 +110,23 @@ class _VMLookup(torch.autograd.Function):
     def backward(ctx, grad_out):
         (xyz,) = ctx.saved_tensors
         m, dev = ctx.module, xyz.device
-        planes, lines = (m.density_plane, m.density_line) if ctx.kind == "density" else \
-            (m.app_plane, m.app_line)
-        d_planes = [torch.zeros_like(p, memory_format=torch.channels_last) for p in planes]
-        d_lines = [torch.zeros_like(l, memory_format=torch.channels_last) for l in lines]
+        grids = m._tensors()[0]
+        d_grids, planes, lines = _grid_grads(grids[:6] if ctx.kind == "density" else grids[6:])
         d_xyz = torch.empty_like(xyz) if ctx.needs_input_grad[2] else None
         g = grad_out.detach().to(torch.float32).contiguous()
         fn = getattr(_lib.lib(), "lrf_density_feature_backward" if ctx.kind == "density"
                      else "lrf_app_products_backward")
         with torch.cuda.device(dev):
-            fs, keep = m._field_struct(None, need_mlp=False)
-            pp = (C.c_void_p * 3)(*[t.data_ptr() for t in d_planes])
-            lp = (C.c_void_p * 3)(*[t.data_ptr() for t in d_lines])
-            _lib.check(fn(C.byref(fs), _ptr(xyz), _ptr(g), xyz.shape[0], pp, lp, _ptr(d_xyz),
+            _lib.check(fn(C.byref(m._field()), _ptr(xyz), _ptr(g), xyz.shape[0], planes, lines, _ptr(d_xyz),
                           _stream(dev)))
-        return (None, None, d_xyz, *d_planes, *d_lines)
+        return (None, None, d_xyz, *d_grids)
 
 
 def _field_state(m, params):
     """What a fused backward recomputes from: the parameters' storage and versions, the grid size and the alpha
     mask.  The backward compares it with the forward's to catch in-place updates in between."""
     am = m.alphaMask
-    return (tuple((p.data_ptr(), p._version) for p in params), tuple(m._grid_host),
-            None if am is None else (am.alpha_volume.data_ptr(), am.alpha_volume._version))
+    return _key(params), tuple(m._grid_host), None if am is None else _key((am.alpha_volume,))
 
 
 def _check_field_state(m, seen):
@@ -103,34 +138,30 @@ def _check_field_state(m, seen):
 
 
 def _field_grad_buffers(m, dev):
-    """Zeroed gradient buffers laid out like the field's parameters (d_w1b = d(mlp[0].weight @ basis_mat.weight))
-    and the LrfGradients struct pointing at them (d_rays left NULL) -> (buffers, struct)."""
-    rm = m.renderModule
-    cl = torch.channels_last
-    d_dp = [torch.zeros_like(p, memory_format=cl) for p in m.density_plane]
-    d_dl = [torch.zeros_like(p, memory_format=cl) for p in m.density_line]
-    d_ap = [torch.zeros_like(p, memory_format=cl) for p in m.app_plane]
-    d_al = [torch.zeros_like(p, memory_format=cl) for p in m.app_line]
-    d_w1b = torch.zeros(rm.mlp[0].weight.shape[0], m.basis_mat.weight.shape[1], device=dev)
-    d_b1, d_w2, d_b2 = (torch.zeros_like(t) for t in (rm.mlp[0].bias, rm.mlp[2].weight, rm.mlp[2].bias))
-    d_w3, d_b3 = torch.zeros_like(rm.mlp_view[0].weight), torch.zeros_like(rm.mlp_view[0].bias)
+    """Zeroed gradient buffers laid out like the field's tensors, in _FIELD_TENSORS order with one d_w1b =
+    d(w1 @ basis) in place of basis and w1, and the LrfGradients struct pointing at them (d_rays left NULL)
+    -> ((d_dplane, d_dline, d_aplane, d_aline: lists of three), d_w1b, d_b1, d_w2, d_b2, d_w3, d_b3), struct."""
+    grids, mlp = m._tensors()
     g = _lib.LrfGradients()
-    for i in range(3):
-        g.d_dplane[i], g.d_dline[i] = d_dp[i].data_ptr(), d_dl[i].data_ptr()
-        g.d_aplane[i], g.d_aline[i] = d_ap[i].data_ptr(), d_al[i].data_ptr()
-    g.d_w1b, g.d_b1, g.d_w2 = d_w1b.data_ptr(), d_b1.data_ptr(), d_w2.data_ptr()
-    g.d_b2, g.d_w3, g.d_b3 = d_b2.data_ptr(), d_w3.data_ptr(), d_b3.data_ptr()
-    return (d_dp, d_dl, d_ap, d_al, d_w1b, d_b1, d_w2, d_b2, d_w3, d_b3), g
+    bufs = []
+    for k in (0, 6):                                   # the density, then the appearance planes and lines
+        d_grids, planes, lines = _grid_grads(grids[k:k + 6])
+        setattr(g, "d_" + _FIELD_TENSORS[k][0], planes)
+        setattr(g, "d_" + _FIELD_TENSORS[k + 3][0], lines)
+        bufs += [d_grids[:3], d_grids[3:]]
+    basis, w1 = mlp[:2]
+    bufs += [torch.zeros(w1.shape[0], basis.shape[1], device=dev)] + [torch.zeros_like(t) for t in mlp[2:]]
+    for (slot, _, _), t in zip(_FIELD_TENSORS[13:], bufs[4:]):
+        setattr(g, "d_w1b" if slot == "w1" else "d_" + slot, t.data_ptr())
+    return tuple(bufs), g
 
 
 def _field_grads(m, bufs):
-    """The buffers of _field_grad_buffers as gradients in _grad_params order.  W1B = mlp[0].weight @
-    basis_mat.weight was folded for the kernel: its gradient is unfolded here."""
-    d_dp, d_dl, d_ap, d_al, d_w1b, d_b1, d_w2, d_b2, d_w3, d_b3 = bufs
-    w1, basis = m.renderModule.mlp[0].weight, m.basis_mat.weight
-    d_w1 = d_w1b @ basis.detach().t()
-    d_basis = w1.detach().t() @ d_w1b
-    return (*d_dp, *d_dl, *d_ap, *d_al, d_basis, d_w1, d_b1, d_w2, d_b2, d_w3, d_b3)
+    """The buffers of _field_grad_buffers as gradients in _grad_params order: d_w1b, the gradient of the product
+    w1 @ basis the kernels read, is unfolded into those of basis and w1."""
+    basis, w1 = (t.detach() for t in m._tensors()[1][:2])
+    d_w1b = bufs[4]
+    return (*(t for d_grids in bufs[:4] for t in d_grids), w1.t() @ d_w1b, d_w1b @ basis.t(), *bufs[5:])
 
 
 class _RenderFn(torch.autograd.Function):
@@ -184,8 +215,7 @@ class _DensityL1Fn(torch.autograd.Function):
         dev = grids[0].device
         acc = torch.zeros(1, dtype=torch.float64, device=dev)
         with torch.cuda.device(dev):
-            fs, _ = module._field_struct(None, need_mlp=False)
-            _lib.check(_lib.lib().lrf_density_l1(C.byref(fs), _ptr(acc), _stream(dev)))
+            _lib.check(_lib.lib().lrf_density_l1(C.byref(module._field()), _ptr(acc), _stream(dev)))
         ctx.module = module
         n = 1
         for g in module._grid_host:
@@ -195,17 +225,14 @@ class _DensityL1Fn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         m = ctx.module
-        dev = m.density_plane[0].device
-        cl = torch.channels_last
-        d_planes = [torch.zeros_like(p, memory_format=cl) for p in m.density_plane]
-        d_lines = [torch.zeros_like(p, memory_format=cl) for p in m.density_line]
+        grids = m._tensors()[0][:6]
+        dev = grids[0].device
+        d_grids, planes, lines = _grid_grads(grids)
         gg = g.detach().to(torch.float32).reshape(1).contiguous()
         with torch.cuda.device(dev):
-            fs, _ = m._field_struct(None, need_mlp=False)
-            pp = (C.c_void_p * 3)(*[t.data_ptr() for t in d_planes])
-            lp = (C.c_void_p * 3)(*[t.data_ptr() for t in d_lines])
-            _lib.check(_lib.lib().lrf_density_l1_backward(C.byref(fs), _ptr(gg), pp, lp, _stream(dev)))
-        return (None, *d_planes, *d_lines)
+            _lib.check(_lib.lib().lrf_density_l1_backward(C.byref(m._field()), _ptr(gg), planes, lines,
+                                                          _stream(dev)))
+        return (None, *d_grids)
 
 
 class _TVFn(torch.autograd.Function):
@@ -350,7 +377,6 @@ class TensorBase(torch.nn.Module):
         self.shadingMode, self.pos_pe, self.view_pe, self.fea_pe, self.featureC = (
             shadingMode, pos_pe, view_pe, fea_pe, featureC)
         self.init_render_func(shadingMode, pos_pe, view_pe, fea_pe, featureC, device)
-        self._prepared = None
         self.last_weights = None     # set by forward(..., return_weights=True)
         self.grid_storage = "fp32"   # see set_grid_storage()
 
@@ -398,9 +424,7 @@ class TensorBase(torch.nn.Module):
         self.stepSize = self.stepSize.to(device)
         if self.alphaMask is not None:
             self.alphaMask = self.alphaMask.to(device)
-        self._prepared = None
-        for memo in ("_prep_memo", "_fs_memo", "_fs16_memo", "_g16_memo"):
-            self.__dict__.pop(memo, None)
+        self.__dict__.pop("_memo", None)
         return super().to(device)
 
     # -- the per-batch distance table (tensorBase.py:419-437) -------------------------------------
@@ -413,12 +437,7 @@ class TensorBase(torch.nn.Module):
         device = device if device is not None else self.aabb.device
         n = (N_samples if N_samples > 0 else self.nSamples) // 6
         if not is_train:   # deterministic: build once per (n, device)
-            key = (n, str(device))
-            cached = self.__dict__.get("_ztab")
-            if cached is None or cached[0] != key:
-                cached = (key, self._build_table(n, device, False))
-                self.__dict__["_ztab"] = cached
-            return cached[1]
+            return _memo(self, "z", (n, str(device)), lambda _: self._build_table(n, device, False))
         return self._build_table(n, device, True)
 
     @staticmethod
@@ -456,40 +475,62 @@ class TensorBase(torch.nn.Module):
         if kind == "bf16" and (self.fea_pe or self.view_pe):
             raise NotImplementedError("localrf_b200: bf16 grid storage is built for fields without positional encodings")
         self.grid_storage = kind
-        if kind == "fp32":
-            self.__dict__.pop("_g16_memo", None)
-            self.__dict__.pop("_fs16_memo", None)
+        self.__dict__.pop("_memo", None)
         return self
 
-    def _grids16(self):
-        """bfloat16 copies of the twelve grids (memory [H][W][C] / [L][C]), rebuilt when a parameter is
-        replaced or updated in place.  -> dict name -> [3 tensors]"""
-        names = (("dplane", self.density_plane), ("dline", self.density_line),
-                 ("aplane", self.app_plane), ("aline", self.app_line))
-        src = [p for _, plist in names for p in plist]
-        key = tuple((p.data_ptr(), p._version) for p in src)
-        memo = self.__dict__.get("_g16_memo")
-        if memo is None or memo[0] != key:
+    def _tensors(self):
+        """(grids, mlp): the field's tensors as two tuples in _FIELD_TENSORS order.  Read through the modules'
+        _parameters / _modules dicts: ParameterList / Sequential indexing costs ~1 us per access, and this runs on
+        every render call."""
+        mods = self._modules
+        rm = mods["renderModule"]._modules
+        l0, l2, l3 = rm["mlp"]._modules["0"]._parameters, rm["mlp"]._modules["2"]._parameters, \
+            rm["mlp_view"]._modules["0"]._parameters
+        return ((*mods["density_plane"]._parameters.values(), *mods["density_line"]._parameters.values(),
+                 *mods["app_plane"]._parameters.values(), *mods["app_line"]._parameters.values()),
+                (mods["basis_mat"]._parameters["weight"], l0["weight"], l0["bias"], l2["weight"], l2["bias"],
+                 l3["weight"], l3["bias"]))
+
+    def _grids16(self, grids):
+        """bfloat16 copies of the twelve grids (memory [H][W][C] / [L][C]), rebuilt when a grid is replaced or
+        updated in place."""
+        def build(_):
             lib = _lib.lib()
-            out = {}
-            for name, plist in names:
-                out[name] = []
-                for p in plist:
-                    dev = p.device
-                    dst = torch.empty(p.numel(), dtype=torch.bfloat16, device=dev)
-                    with torch.cuda.device(dev):
-                        _lib.check(lib.lrf_pack_bf16(_ptr(p.detach()), _ptr(dst), p.numel(), _stream(dev)))
-                    out[name].append(dst)
-            key = tuple((p.data_ptr(), p._version) for p in src)
-            memo = (key, out, src)
-            self.__dict__["_g16_memo"] = memo
-        return memo[1]
+            out = []
+            for p in grids:
+                dst = torch.empty(p.numel(), dtype=torch.bfloat16, device=p.device)
+                with torch.cuda.device(p.device):
+                    _lib.check(lib.lrf_pack_bf16(_ptr(p.detach()), _ptr(dst), p.numel(), _stream(p.device)))
+                out.append(dst)
+            return tuple(out)
+        return _memo(self, "grids16", _key(grids), build, grids)
+
+    def _field(self, z=None, bf16=False, prepared=False):
+        """This field's LrfField, memoised: rebuilt when a tensor it points at or copies from is replaced or
+        updated in place, or a scalar it holds changes.  `bf16`: the grids are their bfloat16 copies.  Without `z`
+        the table is NULL, for the entry points that read no table.  With `prepared`: (struct, forward prepared
+        block), the block rebuilt in place when the MLP / basis weights change."""
+        grids, mlp = self._tensors()
+        am = self.alphaMask
+        src = mlp + grids + (self._parameters["aabb"],) + (() if z is None else (z,)) + \
+            (() if am is None else (am._parameters["alpha_volume"], am._parameters["aabb"]))
+        k = _key(src)
+        key = (k, None if z is None else z.numel(), tuple(self._grid_host), float(self.density_shift),
+               float(self.distance_scale), float(self.rayMarch_weight_thres), self.fea2denseAct)
+        fs = _memo(self, _FIELD_SLOTS[bf16][z is None], key, lambda _: self._field_struct(z, grid16=bf16), src)[0]
+        if not prepared:
+            return fs
+        n = len(mlp)                   # src starts with the MLP tensors: the head of k is _key(mlp)
+        return fs, _memo(self, "prepared", (k[0][:n], k[1][:n]), lambda block: self.prepare(fs, block), mlp)
 
     def _field_struct(self, z=None, need_mlp=True, grid16=False):
+        """A new LrfField of this field and the bfloat16 copies it points at, if any -> (struct, copies).  The
+        builder of _field's memo, which is where callers take their struct from.  `need_mlp=False` leaves the MLP
+        pointers other than basis NULL, for the entry points that run no MLP."""
+        grids, mlp = self._tensors()
         s = _lib.LrfField()
-        keep = []
         g = self._grid_host
-        aabb = self._host_copy("_aabb_host", self.aabb)
+        aabb = self._host_copy("aabb", self.aabb)
         for i in range(3):
             s.grid[i] = int(g[i])
         for i in range(6):
@@ -497,36 +538,28 @@ class TensorBase(torch.nn.Module):
         if len(set(self.density_n_comp)) != 1 or len(set(self.app_n_comp)) != 1:
             raise NotImplementedError("per-plane component counts must be equal")
         s.n_dcomp, s.n_acomp = self.density_n_comp[0], self.app_n_comp[0]
-        for i in range(3):
-            for name, plist in (("dplane", self.density_plane), ("dline", self.density_line),
-                                ("aplane", self.app_plane), ("aline", self.app_line)):
-                p = plist[i]
-                _require_cuda(p, f"{name}[{i}]")
-                if p.dtype != torch.float32:
-                    raise TypeError(f"{name}[{i}] must be float32, got {p.dtype}")
-                if not p.is_contiguous(memory_format=torch.channels_last):
-                    # a parameter swapped in from outside in NCHW layout: re-lay it out IN PLACE, once,
-                    # so the struct always points at the live storage the optimiser updates (a
-                    # temporary copy would go stale on the next in-place update)
-                    p.data = _cl(p.data)
-                getattr(s, name)[i] = p.data_ptr()
+        for (slot, i, _), p in zip(_FIELD_TENSORS, grids):
+            _require_cuda(p, f"{slot}[{i}]")
+            if p.dtype != torch.float32:
+                raise TypeError(f"{slot}[{i}] must be float32, got {p.dtype}")
+            if not p.is_contiguous(memory_format=torch.channels_last):
+                # a parameter swapped in from outside in NCHW layout: re-lay it out IN PLACE, once,
+                # so the struct always points at the live storage the optimiser updates (a
+                # temporary copy would go stale on the next in-place update)
+                p.data = _cl(p.data)
+            getattr(s, slot)[i] = p.data_ptr()
         s.app_dim = self.app_dim
         s.featureC = self.featureC
         s.fea_pe, s.view_pe = self.fea_pe, self.view_pe
-        if need_mlp:
-            rm = self.renderModule
-            for name, t in (("basis", self.basis_mat.weight), ("w1", rm.mlp[0].weight),
-                            ("b1", rm.mlp[0].bias), ("w2", rm.mlp[2].weight),
-                            ("b2", rm.mlp[2].bias), ("w3", rm.mlp_view[0].weight),
-                            ("b3", rm.mlp_view[0].bias)):
-                _require_cuda(t, name)
-                if t.dtype != torch.float32:
-                    raise TypeError(f"{name} must be float32, got {t.dtype}")
-                if not t.is_contiguous():
-                    t.data = t.data.contiguous()       # in place, for the same reason as above
-                setattr(s, name, t.data_ptr())
-        else:
-            s.basis = self.basis_mat.weight.detach().data_ptr()
+        for (slot, _, _), t in zip(_FIELD_TENSORS[12:], mlp if need_mlp else ()):
+            _require_cuda(t, slot)
+            if t.dtype != torch.float32:
+                raise TypeError(f"{slot} must be float32, got {t.dtype}")
+            if not t.is_contiguous():
+                t.data = t.data.contiguous()       # in place, for the same reason as above
+            setattr(s, slot, t.data_ptr())
+        if not need_mlp:
+            s.basis = mlp[0].detach().data_ptr()
         if self.alphaMask is not None:
             vol = self.alphaMask.alpha_volume
             _require_cuda(vol, "alphaMask.alpha_volume")
@@ -535,7 +568,7 @@ class TensorBase(torch.nn.Module):
             s.alpha_vol = vol.data_ptr()
             for i in range(3):
                 s.alpha_dims[i] = vol.shape[-3 + i]
-            ab = self._host_copy("_alpha_aabb_host", self.alphaMask.aabb)
+            ab = self._host_copy("alpha_aabb", self.alphaMask.aabb)
             for i in range(6):
                 s.alpha_aabb[i] = ab[i]
         s.density_shift = float(self.density_shift)
@@ -545,81 +578,41 @@ class TensorBase(torch.nn.Module):
         if z is not None:
             s.z_vals = z.data_ptr()
             s.n_samples = z.numel()
+        copies = ()
         if grid16:
             # (after the loop above: the fp32 parameters are channel-last by now, so the copies are too)
-            g16 = self._grids16()
-            for name, tensors in g16.items():
-                for i, t in enumerate(tensors):
-                    getattr(s, name)[i] = t.data_ptr()
+            copies = self._grids16(grids)
+            for (slot, i, _), t in zip(_FIELD_TENSORS, copies):
+                getattr(s, slot)[i] = t.data_ptr()
             s.grid_dtype = _lib.GRID_BF16
-            keep.append(g16)
-        return s, keep
+        return s, copies
 
-    def _host_copy(self, slot, param):
-        """Host mirror of a small device tensor, refreshed only when the tensor object or its
-        version counter changes (load_state_dict / in-place edits) -- keeps the per-call path free
-        of device->host synchronisation."""
-        key = (id(param), param._version, param.device)
-        cached = self.__dict__.get(slot)
-        if cached is None or cached[0] != key:
-            # the entry keeps `param` alive, so its id cannot be recycled by another tensor
-            cached = (key, param.detach().reshape(-1).tolist(), param)
-            self.__dict__[slot] = cached
-        return cached[1]
+    def _host_copy(self, slot, t):
+        """Host list of a small device tensor (an aabb), memoised: the per-call path does no device-to-host
+        synchronisation."""
+        return _memo(self, slot, _key((t,)), lambda _: t.detach().reshape(-1).tolist(), (t,))
 
     def field_and_prepared(self, z, fp32=False):
-        """(LrfField struct, prepared block) for this field, memoised: the ctypes struct is rebuilt
-        only when a tensor it points at is replaced, the prepared block only when the MLP / basis
-        weights change (data pointer or version counter) -- every optimiser step while training,
-        never inside an eval loop.  With grid_storage == "bf16" the struct points at the bfloat16
-        copies of the grids (additionally keyed on the grids' version counters) unless `fp32` is set
-        (the autograd node: forward and backward read the live fp32 parameters)."""
-        # (read through the modules' _parameters / _modules dicts: ParameterList / Sequential indexing
-        #  costs ~1 us per access, and this runs on every render call)
-        mods = self._modules
-        rm = mods["renderModule"]._modules
-        l0, l2, l3 = rm["mlp"]._modules["0"]._parameters, rm["mlp"]._modules["2"]._parameters, \
-            rm["mlp_view"]._modules["0"]._parameters
-        mlp = (mods["basis_mat"]._parameters["weight"], l0["weight"], l0["bias"], l2["weight"], l2["bias"],
-               l3["weight"], l3["bias"])
-        grids = (*mods["density_plane"]._parameters.values(), *mods["density_line"]._parameters.values(),
-                 *mods["app_plane"]._parameters.values(), *mods["app_line"]._parameters.values())
-        am = self.alphaMask
-        use16 = self.grid_storage == "bf16" and not fp32
-        k_struct = (tuple(t.data_ptr() for t in grids + mlp), z.data_ptr(), z.numel(),
-                    None if am is None else (am.alpha_volume.data_ptr(), am.aabb._version),
-                    self.aabb._version, tuple(self._grid_host), float(self.density_shift),
-                    float(self.distance_scale), float(self.rayMarch_weight_thres), self.fea2denseAct,
-                    tuple(t._version for t in grids) if use16 else None)
-        slot = "_fs16_memo" if use16 else "_fs_memo"
-        memo = self.__dict__.get(slot)
-        if memo is None or memo[0] != k_struct:
-            fs, keep = self._field_struct(z, grid16=use16)
-            # hold every tensor whose address the struct stores: no recycled pointers while cached
-            memo = (k_struct, fs, keep, grids + mlp + (z,) + (() if am is None else (am.alpha_volume,)))
-            self.__dict__[slot] = memo
-        fs = memo[1]
-        k_prep = tuple((t.data_ptr(), t._version) for t in mlp)
-        pm = self.__dict__.get("_prep_memo")
-        if pm is None or pm[0] != k_prep or self._prepared is None:
-            self.prepare(fs)
-            self.__dict__["_prep_memo"] = (k_prep, mlp)
-        return fs, self._prepared
+        """(LrfField struct, prepared block) for this field, memoised (_field): rebuilt every optimiser step
+        while training, never inside an eval loop.  With grid_storage == "bf16" the struct points at the bfloat16
+        copies of the grids unless `fp32` is set (the autograd node: forward and backward read the live fp32
+        parameters)."""
+        return self._field(z, self.grid_storage == "bf16" and not fp32, prepared=True)
 
-    def prepare(self, field_struct):
-        """(Re)builds the folded / re-laid-out MLP block the kernel stages into shared memory (for a field with
-        positional encodings: the separate basis / layer-1 operand images, 1024-byte aligned for TMA)."""
+    def prepare(self, field_struct, block=None):
+        """Fills the folded / re-laid-out MLP block the kernel stages into shared memory (for a field with
+        positional encodings: the separate basis / layer-1 operand images, 1024-byte aligned for TMA) -> the
+        block: `block` rewritten in place when it has the size and device, else a new one."""
         dev = self.basis_mat.weight.device
         n = _lib.lib().lrf_prepared_bytes_for(C.byref(field_struct))
         if n == 0:
             raise NotImplementedError("localrf_b200: fea_pe / view_pe above 8 are not built")
-        if self._prepared is None or self._prepared.device != dev or self._prepared.numel() != n:
+        if block is None or block.device != dev or block.numel() != n:
             raw = torch.empty(n + 1024, dtype=torch.uint8, device=dev)
             off = (-raw.data_ptr()) % 1024
-            self._prepared = raw[off:off + n]
-        _lib.check(_lib.lib().lrf_field_prepare(C.byref(field_struct), _ptr(self._prepared),
-                                                _stream(dev)))
-        return self._prepared
+            block = raw[off:off + n]
+        _lib.check(_lib.lib().lrf_field_prepare(C.byref(field_struct), _ptr(block), _stream(dev)))
+        return block
 
     def shade_products(self, products, viewdirs):
         """basis_mat + renderModule on explicit plane x line products [M,72] and normalised view
@@ -632,8 +625,7 @@ class TensorBase(torch.nn.Module):
         v = viewdirs.detach().to(dev, torch.float32).contiguous()
         out = torch.empty(x.shape[0], 3, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            fs, keep = self._field_struct(None)
-            prep = self.prepare(fs)
+            _, prep = self.field_and_prepared(None, fp32=True)
             _lib.check(_lib.lib().lrf_mlp_forward(_ptr(prep), _ptr(x), _ptr(v), x.shape[0],
                                                   _ptr(out), _stream(dev)))
         return out
@@ -673,28 +665,21 @@ class TensorBase(torch.nn.Module):
 
     def _grad_params(self):
         """Parameters in the order _RenderFn.backward returns their gradients."""
-        rm = self.renderModule
-        return (*self.density_plane, *self.density_line, *self.app_plane, *self.app_line,
-                self.basis_mat.weight, rm.mlp[0].weight, rm.mlp[0].bias, rm.mlp[2].weight,
-                rm.mlp[2].bias, rm.mlp_view[0].weight, rm.mlp_view[0].bias)
+        grids, mlp = self._tensors()
+        return grids + mlp
 
     def _prepared_backward(self):
-        """Folded / transposed MLP block of lrf_render_backward, rebuilt when the weights change."""
-        rm = self.renderModule
-        mlp = (self.basis_mat.weight, rm.mlp[0].weight, rm.mlp[0].bias, rm.mlp[2].weight,
-               rm.mlp[2].bias, rm.mlp_view[0].weight, rm.mlp_view[0].bias)
-        key = tuple((t.data_ptr(), t._version) for t in mlp)
-        memo = self.__dict__.get("_bprep_memo")
-        dev = mlp[0].device
-        if memo is None or memo[0] != key or memo[1].device != dev:
-            lib = _lib.lib()
-            buf = memo[1] if memo is not None and memo[1].device == dev else \
-                torch.empty(lib.lrf_prepared_backward_bytes(), dtype=torch.uint8, device=dev)
-            fs, keep = self._field_struct(None)
-            _lib.check(lib.lrf_field_prepare_backward(C.byref(fs), _ptr(buf), _stream(dev)))
-            memo = (key, buf, mlp)
-            self.__dict__["_bprep_memo"] = memo
-        return memo[1]
+        """Folded / transposed MLP block of lrf_render_backward, rebuilt in place when the MLP / basis weights
+        change."""
+        mlp = self._tensors()[1]
+
+        def build(block):
+            dev, lib = mlp[0].device, _lib.lib()
+            if block is None or block.device != dev:
+                block = torch.empty(lib.lrf_prepared_backward_bytes(), dtype=torch.uint8, device=dev)
+            _lib.check(lib.lrf_field_prepare_backward(C.byref(self._field()), _ptr(block), _stream(dev)))
+            return block
+        return _memo(self, "prepared_backward", _key(mlp), build, mlp)
 
     def _render_fused(self, rays, z, bg, floater_thresh, return_weights, stats, refine=True, fp32=False):
         """One lrf_render launch on explicit rays [n,6] (contiguous fp32) -> (rgb [n,3], depth [n])."""
@@ -801,9 +786,8 @@ class TensorBase(torch.nn.Module):
         mask = torch.empty(dims[::-1], dtype=torch.float32, device=dev) if want_mask else None
         kept = torch.zeros(1, dtype=torch.int64, device=dev)
         with torch.cuda.device(dev):
-            fs, _ = self._field_struct(None, need_mlp=False)
             _lib.check(_lib.lib().lrf_alpha_mask_build(
-                C.byref(fs), (C.c_int32 * 3)(*dims), float(self.stepSize), float(self.alphaMask_thres),
+                C.byref(self._field()), (C.c_int32 * 3)(*dims), float(self.stepSize), float(self.alphaMask_thres),
                 _ptr(alpha), _ptr(mask), _ptr(kept), _stream(dev)))
         return alpha, mask, kept
 
@@ -837,7 +821,7 @@ class TensorBase(torch.nn.Module):
         pts = torch.empty(n, S, 3, dtype=torch.float32, device=dev)
         z = torch.empty(n, S, dtype=torch.float32, device=dev)
         inside = torch.empty(n, S, dtype=torch.uint8, device=dev)
-        aabb = self._host_copy("_aabb_host", self.aabb)
+        aabb = self._host_copy("aabb", self.aabb)
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().lrf_sample_ray(
                 _ptr(rays), _ptr(jitter), n, S, (C.c_float * 6)(*aabb), float(self.near_far[0]),
@@ -883,9 +867,7 @@ class TensorVMSplit(TensorBase):
         m = xyz.shape[0]
         out = torch.empty((m,) if width == 1 else (m, width), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            fs, keep = self._field_struct(None, need_mlp=False)
-            fn = getattr(_lib.lib(), fn_name)
-            _lib.check(fn(C.byref(fs), _ptr(xyz), m, _ptr(out), _stream(dev)))
+            _lib.check(getattr(_lib.lib(), fn_name)(C.byref(self._field()), _ptr(xyz), m, _ptr(out), _stream(dev)))
         return out
 
     @staticmethod

@@ -102,6 +102,20 @@ def test_test_frame_exposure_rule():
         torch.testing.assert_close(out, (E[vm] + E[vp]) / 2)
 
 
+def test_field_tensor_table_matches_modules():
+    """TensorBase._tensors reads the module attributes _FIELD_TENSORS names, in its order, which is _grad_params'
+    and the order the gradients of the fused backward come back in; after an upsample too (new grid tensors)."""
+    from gpu_helpers import module_from_golden
+    from localrf_b200.tensorf import _FIELD_TENSORS
+    m = module_from_golden(load_golden("cfg1_64"), device="cpu")
+    for _ in range(2):
+        grids, mlp = m._tensors()
+        assert len(grids) == 12 and len(mlp) == 7
+        assert all(t is m.get_parameter(attr) for (_, _, attr), t in zip(_FIELD_TENSORS, grids + mlp))
+        assert m._grad_params() == grids + mlp
+        m.upsample_volume_grid([20, 24, 28])
+
+
 def test_grid_storage_setting_host_side():
     """set_grid_storage: validation, propagation through LocalTensorfs, inheritance by appended fields; the
     parameters and the state_dict are untouched (the 16-bit copies are an inference cache)."""
