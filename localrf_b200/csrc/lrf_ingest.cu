@@ -261,14 +261,15 @@ __global__ void __launch_bounds__(INGEST_THREADS) resize_linear_kernel(const flo
   const long long p = (long long)blockIdx.x * INGEST_THREADS + threadIdx.x;
   if (p >= (long long)W * H) return;
   const int x = (int)(p % W), y = (int)(p / W);
-  float* out = dst + y * dst_stride + 3 * x;
+  // pixel offsets in 64 bits: a row may hold up to 2^31 - 1 pixels, so 3 x alone can pass 2^31
+  float* out = dst + y * dst_stride + 3LL * x;
   if (mode == 1) {
-    for (int c = 0; c < 3; ++c) out[c] = src[y * src_stride + 3 * x + c];
+    for (int c = 0; c < 3; ++c) out[c] = src[y * src_stride + 3LL * x + c];
     return;
   }
   if (mode == 2) {
     for (int c = 0; c < 3; ++c) {
-      auto v = [&](int dy, int dx) { return src[(long long)(2 * y + dy) * src_stride + 3 * (2 * x + dx) + c]; };
+      auto v = [&](int dy, int dx) { return src[(long long)(2 * y + dy) * src_stride + 3LL * (2LL * x + dx) + c]; };
       out[c] = reduce_block(2, v);
     }
     return;
@@ -277,13 +278,15 @@ __global__ void __launch_bounds__(INGEST_THREADS) resize_linear_kernel(const flo
   float fx, fy;
   linear_coeff(x, scale_x, sx, fx);
   if (sx < 0) sx = 0, fx = 0.f;
-  const bool copy = sx + 1 >= w0;                         // cv2's xmax: every later column copies too
+  // cv2's xmax (sx + 1 >= w0): every later column copies too.  sx + 1 and sy + 1 are not formed at the last index,
+  // where a float index of 2^31 has converted to INT_MAX.
+  const bool copy = sx >= w0 - 1;
   if (copy) sx = w0 - 1;
   linear_coeff(y, scale_y, sy, fy);                       // rows are not reset at the borders
-  const int sy0 = min(max(sy, 0), h0 - 1), sy1 = min(max(sy + 1, 0), h0 - 1);
+  const int sy0 = min(max(sy, 0), h0 - 1), sy1 = sy >= h0 - 1 ? h0 - 1 : max(sy + 1, 0);
   const float ax = __fsub_rn(1.f, fx), ay = __fsub_rn(1.f, fy);
-  const float* r0 = src + sy0 * src_stride + 3 * sx;
-  const float* r1 = src + sy1 * src_stride + 3 * sx;
+  const float* r0 = src + sy0 * src_stride + 3LL * sx;
+  const float* r1 = src + sy1 * src_stride + 3LL * sx;
   for (int c = 0; c < 3; ++c) {
     const float h0v = copy ? r0[c] : __fadd_rn(__fmul_rn(r0[c], ax), __fmul_rn(r0[3 + c], fx));
     const float h1v = copy ? r1[c] : __fadd_rn(__fmul_rn(r1[c], ax), __fmul_rn(r1[3 + c], fx));

@@ -23,21 +23,26 @@ def resize_nearest(a, W, H):
     return a[nearest_index(a.shape[0], H)][:, nearest_index(a.shape[1], W)]
 
 
-def quantile(a, q=0.9):
-    """np.quantile(a, q) (method "linear") for a float32 array, restated: numpy 2.x keeps q, the virtual index
-    (n - 1) * q, its floor and the interpolation weight in float32, and interpolates with _lerp's two branches."""
-    a = np.asarray(a, dtype=F32).ravel()
-    n = a.size
-    if np.isnan(a).any():
-        return F32(np.nan)
+def quantile_ranks(n, q=0.9):
+    """-> (lo, hi, gamma): the ranks np.quantile(., q) interpolates between in n float32 values, and its weight.
+    numpy 2.x keeps q, the virtual index (n - 1) * q, its floor and the weight in float32.  Above 2^24 the float32
+    floor + 1 rounds to even, so hi is lo itself or two ranks up as often as the next rank."""
     vi = F32(n - 1) * F32(q)
     prev = np.floor(vi)
     nxt = prev + F32(1)
     lo, hi = int(prev), int(nxt)
     if vi >= F32(n - 1):
         lo = hi = n - 1
-    hi = min(hi, n - 1)
-    gamma = F32(vi - prev)
+    return lo, min(hi, n - 1), F32(vi - prev)
+
+
+def quantile(a, q=0.9):
+    """np.quantile(a, q) (method "linear") for a float32 array, restated: the ranks of quantile_ranks, interpolated
+    with _lerp's two branches."""
+    a = np.asarray(a, dtype=F32).ravel()
+    if np.isnan(a).any():
+        return F32(np.nan)
+    lo, hi, gamma = quantile_ranks(a.size, q)
     s = np.sort(a, kind="stable")
     A, B = s[lo], s[hi]
     with np.errstate(invalid="ignore", over="ignore"):
@@ -45,6 +50,23 @@ def quantile(a, q=0.9):
         if gamma >= F32(0.5):
             return F32(B - F32(d * F32(F32(1) - gamma)))
         return F32(A + F32(d * gamma))
+
+
+def hi_mode(W, H):
+    """Where numpy's upper neighbour of the 0.9 quantile of a W x H frame's 2 W H values lies: 0 the lower rank
+    itself, 1 the next rank, 2 two ranks up (lrf_panels.cu's hi_mode)."""
+    lo, hi, _ = quantile_ranks(2 * W * H)
+    return hi - lo
+
+
+def neighbour_gt(W, H, inf_from, seed):
+    """A ground-truth channel of W H values such that [zeros(W H); gt] sorted is finite below rank `inf_from` and
+    +inf from it on (inf_from >= W H; None: no infinity): shuffled negatives and positives, then the infinities."""
+    N = W * H
+    k_inf = 0 if inf_from is None else 2 * N - inf_from
+    g = np.random.default_rng(seed)
+    finite = g.uniform(0.5, 2.0, N - k_inf) * np.where(g.random(N - k_inf) < 0.5, -1.0, 1.0)
+    return g.permutation(np.concatenate([finite, np.full(k_inf, np.inf)])).astype(F32)
 
 
 def lower_median(a):
@@ -131,7 +153,11 @@ FULL_OUTPUT_PIXELS = 64 * 48          # cases up to this size store whole panels
 
 def make_case(name):
     """-> dict of the case's inputs, float32 numpy (directions of a pinhole camera, as get_ray_directions_lean)."""
-    seed, W, H, h0, w0, n_cams, idx, kind = CASES[name]
+    return build_case(*CASES[name])
+
+
+def build_case(seed, W, H, h0, w0, n_cams, idx, kind="random"):
+    """The inputs of one frame of the given sizes and kind (see CASES), regenerated from `seed`."""
     g = np.random.default_rng(seed)
     rot = []
     for _ in range(n_cams):

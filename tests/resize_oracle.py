@@ -50,6 +50,27 @@ def linear(a, W, H):
     return (rows[sy0] * ay[:, None, None] + rows[sy1] * fy[:, None, None]).astype(F32)
 
 
+def row_chunk(row, W, x0, x1):
+    """Columns [x0, x1) of linear(a, W, 1) for a 1-row image a whose row is the torch float32 tensor `row` [w0, 3],
+    on row's device: the same rule as _coeffs and linear (the index in float64, rounded to float32, then every
+    product and sum of the blend a separate float32 operation).  For rows too long to restate on the host."""
+    import torch
+    w0 = row.shape[0]
+    x = torch.arange(x0, x1, dtype=torch.float64, device=row.device)
+    f = ((x + 0.5) * (1.0 / (float(W) / w0)) - 0.5).to(torch.float32)
+    s = torch.floor(f)
+    fx = f - s
+    s = s.to(torch.int64)
+    neg = s < 0
+    s = torch.where(neg, 0, s)
+    fx = torch.where(neg, 0, fx)
+    copy = (s + 1 >= w0)[:, None]
+    a0, a1 = row[s.clamp(max=w0 - 1)], row[(s + 1).clamp(max=w0 - 1)]
+    h = torch.where(copy, a0, a0 * (1 - fx)[:, None] + a1 * fx[:, None])
+    _, fy = _coeffs(1, 1)                                 # one row: weights (1, 0) on the row itself
+    return h * float(F32(1) - fy[0]) + h * float(fy[0])
+
+
 def resize(a, W, H):
     """cv2.resize(a, (W, H)) of a float32 [h0, w0, 3] image, as OpenCV computes it without IPP."""
     a = np.ascontiguousarray(a, dtype=F32)

@@ -99,6 +99,29 @@ def test_quantile_restatement_equals_numpy():
         assert bits_equal(PO.quantile(a), want), (a.size, want)
 
 
+# (W, H, hi_mode): frames whose 2 W H values put numpy's float32 virtual index above 2^24
+NEIGHBOUR_SIZES = [(4096, 2276, 0), (4096, 2304, 2), (4096, 2272, 1), (7680, 4320, 0)]
+# the offset from the lower rank where the infinities of each of the four statistics' arrays begin (None: none);
+# numpy's quantile is NaN exactly when its upper neighbour is an infinity (gamma is 0 at these sizes)
+INF_OFFSETS = (1, 2, 3, None)
+
+
+@pytest.mark.parametrize("W,H,mode", NEIGHBOUR_SIZES)
+def test_quantile_restatement_at_the_neighbour_sizes(W, H, mode):
+    """The restatement the device's neighbour tests rest on: at sizes where numpy's upper neighbour is the lower rank
+    itself (0), the next rank (1) or two ranks up (2), its ranks, and its value on arrays whose first infinity sits
+    just past the lower rank, equal np.quantile's."""
+    assert PO.hi_mode(W, H) == mode
+    lo, hi, gamma = PO.quantile_ranks(2 * W * H)
+    assert gamma == 0 and lo > W * H
+    for k, off in enumerate(INF_OFFSETS[:2] if mode != 2 else INF_OFFSETS[:3]):
+        a = np.concatenate([np.zeros(W * H, np.float32), PO.neighbour_gt(W, H, lo + off, k)])
+        with np.errstate(invalid="ignore"):
+            want = np.quantile(a, 0.9)
+        assert np.isnan(want) == (lo + off <= hi), (off, want)
+        assert bits_equal(PO.quantile(a), want), (off, PO.quantile(a), want)
+
+
 def test_lower_median_equals_sorted_rule():
     rng = np.random.default_rng(8)
     for n in (1, 2, 3, 4, 9, 10, 1001):
@@ -114,6 +137,16 @@ def test_nearest_index_equals_cv2():
         for (W, H) in ((64, 48), (37, 23), (480, 270), (1, 1), (3, 7), (2 * w0 + 1, 3 * h0)):
             want = cv2.resize(src, (W, H), interpolation=cv2.INTER_NEAREST).reshape(H, W)
             assert np.array_equal(PO.resize_nearest(src, W, H), want), (h0, w0, W, H)
+    for (h0, w0), (H, W) in NEAREST_EXTREMES:
+        src = np.arange(h0 * w0, dtype=np.float32).reshape(h0, w0)             # indices below 2^24: exact
+        want = cv2.resize(src, (W, H), interpolation=cv2.INTER_NEAREST).reshape(H, W)
+        assert np.array_equal(PO.resize_nearest(src, W, H), want), (h0, w0, W, H)
+
+
+# ((h0, w0), (H, W)): a pixel to a 4096 x 2304 frame and back, neighbouring sizes, 3 <-> 7
+NEAREST_EXTREMES = [((1, 1), (2304, 4096)), ((2304, 4096), (1, 1)), ((1000, 999), (999, 1000)),
+                    ((999, 1000), (1000, 999)), ((3, 7), (7, 3)), ((7, 3), (3, 7)), ((3, 7), (2304, 4096)),
+                    ((2304, 4096), (7, 3)), ((1, 4096), (2304, 1)), ((2304, 1), (1, 4096))]
 
 
 # ---- the C ABI without a device ------------------------------------------------------------------------------
