@@ -154,7 +154,7 @@ int lrf_version(void);
 const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
  * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor, 7 LrfCameraGrads, 8 LrfFrameStore,
- * 9 LrfRayGather, 10 LrfPanelFrame (0 for any other index).  Bindings compare these with their own mirrors at load
+ * 9 LrfRayGather, 10 LrfPanelFrame, 11 LrfIngestFrame, 12 LrfPointFrame, 13 LrfVoxelTable (0 for any other index).  Bindings compare these with their own mirrors at load
  * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
@@ -606,6 +606,69 @@ size_t lrf_test_panels_scratch_bytes(int32_t W, int32_t H);
  * on, and scratch that is NULL, not 8-byte aligned or too small.  No atomics on floats, no host synchronisation:
  * bitwise repeatable. */
 int lrf_test_panels(const LrfPanelFrame *frame, void *scratch, size_t scratch_bytes, lrf_stream_t stream);
+
+/* ---- point-cloud export: the training views rendered, back-projected and voxel-merged on the device ----------------
+ * A ray's point is its normalised expected depth along its camera-space direction, in the world frame of cam2world
+ * (the frame transforms.json is written in): s = depth / acc, c = dir s, p_a = ((R_a0 c_0 + R_a1 c_1) + R_a2 c_2) + t_a.
+ * Points are merged per voxel of a world-space grid as 64-bit integer sums, so the cloud is bitwise repeatable
+ * whatever the ray chunking, frame order or thread scheduling. */
+
+/* Blended opacity of a batch's rays, called after each field's lrf_render with LrfOutputs.weights set:
+ * acc_k = (float) sum_s (double) weights[r][s] in sample order, then acc[r] = b acc_k (accumulate = 0, the first field)
+ * or acc[r] += b acc_k (later fields) in fp32 without FMA, b = blend[(r / (n_rays / n_views)) blend_stride] (1 when
+ * blend is NULL), the batch's own LrfBatch.blend.  weights is [n_rays][n_samples] device memory.  One launch, no
+ * atomics.  LRF_ERR_INVALID before any device work for NULL weights / acc, n_rays < 0 or at least 2^31, n_rays not a
+ * multiple of n_views >= 1, and n_samples < 1. */
+int lrf_ray_opacity(const float *weights, int64_t n_rays, int32_t n_samples, int64_t n_views, const float *blend,
+                    int64_t blend_stride, int32_t accumulate, float *acc, lrf_stream_t stream);
+
+/* The rendered rays of one view (LocalTensorfs.forward's outputs with the opacity above).  Device memory. */
+typedef struct LrfPointFrame {
+  int64_t n_rays;
+  const float *rgb;            /* [n_rays][3] */
+  const float *depth;          /* [n_rays] */
+  const float *acc;            /* [n_rays] blended opacity (lrf_ray_opacity) */
+  const float *directions;     /* [n_rays][3] camera-space directions */
+  const float *cam2world;      /* [3][4] the view's camera */
+  const float *world2rf;       /* [n_fields][3] */
+  const float *blend;          /* [n_fields] the view's blending weights, or NULL (every field weight 1) */
+  int32_t n_fields;
+  float min_acc;               /* a ray is kept when acc >= min_acc, acc > 0 and depth is finite ... */
+  float max_norm;              /* ... and max_a |p_a + world2rf_k_a| <= max_norm for a field k with blend > 0 */
+} LrfPointFrame;
+
+/* An open-addressing table of voxels (linear probing from splitmix64 of the key, key claimed by atomicCAS).  Zero
+ * keys, sums and stats before the first frame.  The table holds at most capacity / 2 voxels (probes stay short):
+ * stats[2] > capacity / 2 means it overflowed, and its content is then incomplete. */
+typedef struct LrfVoxelTable {
+  int64_t capacity;            /* slots: a power of two in [2, 2^30] */
+  float voxel_size;            /* > 0, finite */
+  float origin[3];             /* finite */
+  unsigned long long *keys;    /* [capacity] voxel key + 1, 0 = empty */
+  unsigned long long *sums;    /* [capacity][7] count, sum f_x, f_y, f_z, sum r, g, b */
+  unsigned long long *stats;   /* [3] += points merged, points whose key is out of range; occupied slots */
+} LrfVoxelTable;
+
+/* Adds one view's kept rays to the table.  q_a = (p_a - origin_a) / voxel_size, k_a = floor(q_a), f_a = q_a - k_a
+ * (fp32, round to nearest, in this order).  A k_a outside [-2^20, 2^20) drops the point into stats[1]; otherwise the
+ * key (k_x + 2^20) << 42 | (k_y + 2^20) << 21 | (k_z + 2^20) gets count += 1, sum f_a += min((uint64)(f_a 2^32),
+ * 2^32 - 1), sum c += (uint32)(clamp(rgb_c, 0, 1) 2^24).  Once the table has overflowed, rays are skipped.  One
+ * launch, one thread per ray, no host synchronisation.  LRF_ERR_INVALID before any device work for a NULL frame,
+ * table or pointer (blend excepted), n_rays < 0 or at least 2^31, n_fields < 1, a NaN min_acc or max_norm, and a table
+ * whose capacity, voxel_size or origin is out of range or whose arrays are not 8-byte aligned. */
+int lrf_frame_points(const LrfPointFrame *frame, const LrfVoxelTable *table, lrf_stream_t stream);
+
+/* Device scratch bytes of lrf_voxel_extract (256-byte aligned); 0 for a capacity lrf_frame_points refuses or when the
+ * device cannot be queried (the sort's temporary storage depends on it). */
+size_t lrf_voxel_extract_scratch_bytes(int64_t capacity);
+/* One point per voxel with count >= min_count, in ascending key order (x-major): rows [0, *n_voxels) of xyz
+ * [capacity][3], rgb [capacity][3] and count [capacity] (int32, saturated), computed in fp64 and rounded once:
+ * xyz_a = (float)(origin_a + (k_a + sum f_a / (count 2^32)) voxel_size), rgb_c = (uint8)floor(sum c / (count 2^24) 255
+ * + 0.5).  *n_voxels (device) is written.  Three launches and CUB's radix sort; no atomics, no host synchronisation.
+ * LRF_ERR_INVALID before any device work for a NULL table or output, a table lrf_frame_points refuses, min_count < 1,
+ * and scratch that is NULL, not 256-byte aligned or smaller than lrf_voxel_extract_scratch_bytes(capacity). */
+int lrf_voxel_extract(const LrfVoxelTable *table, int64_t min_count, float *xyz, uint8_t *rgb, int32_t *count,
+                      int64_t *n_voxels, void *scratch, size_t scratch_bytes, lrf_stream_t stream);
 
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */

@@ -8,7 +8,7 @@ backed by the C ABI in include/localrf_b200.h (localrf_b200/csrc/liblrf_b200.so)
 """
 from .tensorf import AlphaGridMask, MLPRender_Fea_late_view, TensorBase, TensorVMSplit  # noqa: F401
 from .local_tensorfs import LocalTensorfs, ids2pixel, ids2pixel_view  # noqa: F401
-from . import data, losses, metrics, optim, ray_utils, utils  # noqa: F401
+from . import data, export, losses, metrics, optim, ray_utils, utils  # noqa: F401
 from .data import DeviceFrameDataset, DeviceRaySampler  # noqa: F401
 from .losses import supervision_losses  # noqa: F401
 from .optim import adam_step  # noqa: F401

@@ -12,7 +12,7 @@ _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
            "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_panels.cu", "lrf_ingest.cu",
-           "lrf_abi.cu"]
+           "lrf_export.cu", "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", "lrf_launch.cuh", "lrf_reproject.cuh", "lrf_select.cuh",
            os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -97,6 +97,17 @@ class LrfIngestFrame(C.Structure):
                 ("mask", _vp), ("wm", C.c_int32), ("hm", C.c_int32), ("mask_stride", C.c_int64)]
 
 
+class LrfPointFrame(C.Structure):
+    _fields_ = [("n_rays", C.c_int64), ("rgb", _vp), ("depth", _vp), ("acc", _vp), ("directions", _vp),
+                ("cam2world", _vp), ("world2rf", _vp), ("blend", _vp), ("n_fields", C.c_int32),
+                ("min_acc", C.c_float), ("max_norm", C.c_float)]
+
+
+class LrfVoxelTable(C.Structure):
+    _fields_ = [("capacity", C.c_int64), ("voxel_size", C.c_float), ("origin", C.c_float * 3), ("keys", _vp),
+                ("sums", _vp), ("stats", _vp)]
+
+
 class LrfBatch(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int64),
@@ -145,7 +156,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_supervision_losses", "lrf_supervision_losses_backward", "lrf_adam_step",
            "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch", "lrf_gather_rays",
            "lrf_test_panels_scratch_bytes", "lrf_test_panels", "lrf_ingest_scratch_bytes", "lrf_ingest_frame",
-           "lrf_resize_linear"]
+           "lrf_resize_linear", "lrf_ray_opacity", "lrf_frame_points", "lrf_voxel_extract_scratch_bytes",
+           "lrf_voxel_extract"]
 
 
 def _stale():
@@ -200,7 +212,7 @@ def lib():
     L.lrf_sizeof.argtypes = [C.c_int32]
     for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
                                      LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather, LrfPanelFrame,
-                                     LrfIngestFrame)):
+                                     LrfIngestFrame, LrfPointFrame, LrfVoxelTable)):
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -259,6 +271,11 @@ def lib():
     L.lrf_ingest_scratch_bytes.argtypes = [C.c_int64]
     L.lrf_ingest_frame.argtypes = [C.POINTER(LrfFrameStore), C.POINTER(LrfIngestFrame), _vp, C.c_size_t, _vp]
     L.lrf_resize_linear.argtypes = [_vp, C.c_int32, C.c_int32, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_int64, _vp]
+    L.lrf_ray_opacity.argtypes = [_vp, C.c_int64, C.c_int32, C.c_int64, _vp, C.c_int64, C.c_int32, _vp, _vp]
+    L.lrf_frame_points.argtypes = [C.POINTER(LrfPointFrame), C.POINTER(LrfVoxelTable), _vp]
+    L.lrf_voxel_extract_scratch_bytes.restype = C.c_size_t
+    L.lrf_voxel_extract_scratch_bytes.argtypes = [C.c_int64]
+    L.lrf_voxel_extract.argtypes = [C.POINTER(LrfVoxelTable), C.c_int64, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

@@ -3,6 +3,7 @@
 
 #include <atomic>
 #include <climits>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
@@ -90,6 +91,12 @@ cudaError_t launch_render_backward_batch(const FieldDev& F, const BatchDev& B, c
                                          const float* g_rgb, const float* g_depth, const float* g_dirs,
                                          const LrfGradients& G, const LrfCameraGrads& CG, void* scratch,
                                          long long n_views, int n_sms, cudaStream_t stream);
+cudaError_t launch_ray_opacity(const float* w, long long n, int S, long long n_views, const float* blend,
+                               long long blend_stride, int accumulate, float* acc, cudaStream_t stream);
+cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, cudaStream_t stream);
+cudaError_t voxel_extract_scratch_bytes(long long cap, size_t& bytes);
+cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, float* xyz, unsigned char* rgb,
+                                 int* count, long long* n_out, void* scratch, cudaStream_t stream);
 }  // namespace lrf
 
 namespace {
@@ -347,6 +354,8 @@ size_t lrf_sizeof(int32_t which) {
     case 9: return sizeof(LrfRayGather);
     case 10: return sizeof(LrfPanelFrame);
     case 11: return sizeof(LrfIngestFrame);
+    case 12: return sizeof(LrfPointFrame);
+    case 13: return sizeof(LrfVoxelTable);
     default: return 0;
   }
 }
@@ -797,6 +806,65 @@ int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t 
   if (flow_count(*g) != n_flow)
     return fail(LRF_ERR_INVALID, "the flow outputs must be set exactly when the store has the flow group");
   return cuda_status(lrf::launch_gather_rays(*s, *g, (cudaStream_t)stream), "gather_rays_kernel");
+}
+
+// the voxel table of lrf_frame_points and lrf_voxel_extract
+static int check_voxel_table(const LrfVoxelTable* t) {
+  if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
+  if (t->capacity < 2 || t->capacity > (1LL << 30) || (t->capacity & (t->capacity - 1)))
+    return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  if (!(t->voxel_size > 0.0f) || !std::isfinite(t->voxel_size)) return fail(LRF_ERR_INVALID, "voxel_size must be > 0 and finite");
+  if (!std::isfinite(t->origin[0]) || !std::isfinite(t->origin[1]) || !std::isfinite(t->origin[2]))
+    return fail(LRF_ERR_INVALID, "origin must be finite");
+  if (!t->keys || !t->sums || !t->stats) return fail(LRF_ERR_INVALID, "keys / sums / stats of the table is NULL");
+  if (((uintptr_t)t->keys | (uintptr_t)t->sums | (uintptr_t)t->stats) & 7)
+    return fail(LRF_ERR_INVALID, "keys / sums / stats of the table must be 8-byte aligned");
+  return LRF_OK;
+}
+
+int lrf_ray_opacity(const float* weights, int64_t n_rays, int32_t n_samples, int64_t n_views, const float* blend,
+                    int64_t blend_stride, int32_t accumulate, float* acc, lrf_stream_t stream) {
+  if (!weights || !acc) return fail(LRF_ERR_INVALID, "weights / acc is NULL");
+  if (n_rays < 0 || n_views < 1 || n_rays % n_views != 0)
+    return fail(LRF_ERR_INVALID, "n_rays must be a multiple of n_views >= 1");
+  if (n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  if (n_samples < 1) return fail(LRF_ERR_INVALID, "n_samples must be >= 1");
+  return cuda_status(lrf::launch_ray_opacity(weights, n_rays, n_samples, n_views, blend, blend_stride, accumulate, acc,
+                                             (cudaStream_t)stream), "ray_opacity_kernel");
+}
+
+int lrf_frame_points(const LrfPointFrame* f, const LrfVoxelTable* t, lrf_stream_t stream) {
+  if (!f) return fail(LRF_ERR_INVALID, "frame is NULL");
+  int rc = check_voxel_table(t);
+  if (rc != LRF_OK) return rc;
+  if (f->n_rays < 0 || f->n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must lie in [0, 2^31)");
+  if (f->n_fields < 1) return fail(LRF_ERR_INVALID, "n_fields must be >= 1");
+  if (!f->rgb || !f->depth || !f->acc || !f->directions || !f->cam2world || !f->world2rf)
+    return fail(LRF_ERR_INVALID, "rgb / depth / acc / directions / cam2world / world2rf of the frame is NULL");
+  if (std::isnan(f->min_acc) || std::isnan(f->max_norm)) return fail(LRF_ERR_INVALID, "min_acc / max_norm is NaN");
+  return cuda_status(lrf::launch_frame_points(*f, *t, (cudaStream_t)stream), "frame_points_kernel");
+}
+
+size_t lrf_voxel_extract_scratch_bytes(int64_t capacity) {
+  if (capacity < 2 || capacity > (1LL << 30) || (capacity & (capacity - 1))) return 0;
+  size_t bytes = 0;
+  return lrf::voxel_extract_scratch_bytes(capacity, bytes) == cudaSuccess ? bytes : 0;
+}
+
+int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uint8_t* rgb, int32_t* count,
+                      int64_t* n_voxels, void* scratch, size_t scratch_bytes, lrf_stream_t stream) {
+  int rc = check_voxel_table(t);
+  if (rc != LRF_OK) return rc;
+  if (min_count < 1) return fail(LRF_ERR_INVALID, "min_count must be >= 1");
+  if (!xyz || !rgb || !count || !n_voxels) return fail(LRF_ERR_INVALID, "xyz / rgb / count / n_voxels is NULL");
+  if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
+  size_t need = 0;
+  const cudaError_t e = lrf::voxel_extract_scratch_bytes(t->capacity, need);
+  if (e != cudaSuccess) return cuda_fail(e, "voxel_extract (sort size)");
+  if (scratch_bytes < need)
+    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_voxel_extract_scratch_bytes(capacity)");
+  return cuda_status(lrf::launch_voxel_extract(*t, min_count, xyz, rgb, (int*)count, (long long*)n_voxels, scratch,
+                                               (cudaStream_t)stream), "voxel_extract");
 }
 
 static bool panel_size_ok(int32_t W, int32_t H) {

@@ -1,0 +1,251 @@
+// lrf_export.cu -- the scene's geometry as a coloured point cloud: each rendered ray's expected-depth point in the
+// world frame, merged into a voxel grid on the device.
+//
+// lrf_ray_opacity folds a field's per-sample weights (LrfOutputs.weights of its lrf_render launch) into the ray's
+// blended opacity.  lrf_frame_points back-projects each kept ray of one view and adds it to an open-addressing table
+// of 64-bit integer sums keyed by voxel; integer sums commute, so the table's content does not depend on thread
+// scheduling, on how the rays are chunked or on the order of the frames, and atomics are used freely.
+// lrf_voxel_extract sorts the occupied slots by key (CUB's radix sort) and writes one point per voxel: whatever the
+// slot layout, the output is bitwise repeatable.
+//
+// The back-projection and the key are written with explicit round-to-nearest fp32 operations in a fixed order (no
+// FMA contraction), so a numpy float32 restatement reproduces them bit for bit; the per-voxel means are fp64, rounded
+// once.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <cub/device/device_radix_sort.cuh>
+
+#include "../../include/localrf_b200.h"
+#include "lrf_launch.cuh"
+
+namespace lrf {
+
+namespace {
+
+constexpr int OP_RAYS = 128;           // rays per CTA of ray_opacity_kernel (one per thread)
+constexpr int OP_TILE = 32;            // samples per tile staged through shared memory
+constexpr int PT_THREADS = 256;
+constexpr int EX_THREADS = 256;
+constexpr int KEY_BITS = 21;           // per axis: keys in [-2^20, 2^20), 63 bits in all
+constexpr float KEY_LIM = 1048576.0f;  // 2^20
+constexpr unsigned long long NO_KEY = ~0ull;
+
+// One thread per ray sums its weights in sample order in fp64.  The [rays][S] rows are read a tile at a time,
+// coalesced, into padded shared rows, so every thread's sequential sum reads its own row without bank conflicts.
+__global__ void __launch_bounds__(OP_RAYS) ray_opacity_kernel(const float* __restrict__ w, long long n, int S,
+                                                              long long rays_per_view, const float* __restrict__ blend,
+                                                              long long blend_stride, int accumulate, float* acc) {
+  __shared__ float tile[OP_RAYS][OP_TILE + 1];
+  const long long r0 = (long long)blockIdx.x * OP_RAYS;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  double s = 0.0;
+  for (int k0 = 0; k0 < S; k0 += OP_TILE) {
+    __syncthreads();
+    for (int row = warp; row < OP_RAYS; row += OP_RAYS / 32) {
+      const long long r = r0 + row;
+      const int k = k0 + lane;
+      tile[row][lane] = (r < n && k < S) ? __ldg(w + r * S + k) : 0.0f;
+    }
+    __syncthreads();
+    const int m = min(OP_TILE, S - k0);
+    for (int j = 0; j < m; ++j) s += (double)tile[threadIdx.x][j];
+  }
+  const long long r = r0 + threadIdx.x;
+  if (r >= n) return;
+  const float b = blend ? blend[(r / rays_per_view) * blend_stride] : 1.0f;
+  const float a = __fmul_rn(b, (float)s);
+  acc[r] = accumulate ? __fadd_rn(acc[r], a) : a;
+}
+
+// splitmix64's finaliser: the probe start of a key
+__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
+  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27; x *= 0x94d049bb133111ebull;
+  return x ^ (x >> 31);
+}
+
+__device__ __forceinline__ unsigned long long occupied(const LrfVoxelTable& t) {
+  return *reinterpret_cast<volatile unsigned long long*>(t.stats + 2);
+}
+
+__global__ void __launch_bounds__(PT_THREADS) frame_points_kernel(const LrfPointFrame f, const LrfVoxelTable t) {
+  const long long r = (long long)blockIdx.x * PT_THREADS + threadIdx.x;
+  const unsigned long long half = (unsigned long long)t.capacity >> 1;
+  bool keep = false, out = false;
+  unsigned long long key = 0, fs[3];
+  unsigned int cs[3];
+  if (r < f.n_rays && occupied(t) <= half) {
+    const float a = f.acc[r], d = f.depth[r];
+    if (a >= f.min_acc && a > 0.0f && isfinite(d)) {
+      const float s = __fdiv_rn(d, a);
+      float c[3], p[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) c[i] = __fmul_rn(f.directions[3 * r + i], s);
+      const float* M = f.cam2world;
+#pragma unroll
+      for (int i = 0; i < 3; ++i)
+        p[i] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(M[4 * i], c[0]), __fmul_rn(M[4 * i + 1], c[1])),
+                                   __fmul_rn(M[4 * i + 2], c[2])), M[4 * i + 3]);
+      bool inside = false;
+      for (int k = 0; k < f.n_fields && !inside; ++k) {
+        if (f.blend && !(f.blend[k] > 0.0f)) continue;
+        const float* o = f.world2rf + 3 * k;         // (each comparison is false for NaN)
+        inside = fabsf(__fadd_rn(p[0], o[0])) <= f.max_norm && fabsf(__fadd_rn(p[1], o[1])) <= f.max_norm &&
+                 fabsf(__fadd_rn(p[2], o[2])) <= f.max_norm;
+      }
+      if (inside) {
+        bool in_range = true;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          const float q = __fdiv_rn(__fsub_rn(p[i], t.origin[i]), t.voxel_size);
+          const float k = floorf(q);
+          in_range = in_range && k >= -KEY_LIM && k < KEY_LIM;
+          if (in_range) {
+            const float fr = __fsub_rn(q, k);
+            const unsigned long long u = __float2ull_rz(__fmul_rn(fr, 4294967296.0f));
+            fs[i] = u < 0xffffffffull ? u : 0xffffffffull;
+            key = (key << KEY_BITS) | (unsigned long long)((int)k + (1 << 20));
+          }
+        }
+        keep = in_range;
+        out = !in_range;
+        if (keep)
+#pragma unroll
+          for (int i = 0; i < 3; ++i)
+            cs[i] = __float2uint_rz(__fmul_rn(fminf(fmaxf(f.rgb[3 * r + i], 0.0f), 1.0f), 16777216.0f));
+      }
+    }
+  }
+  const unsigned mk = __ballot_sync(0xffffffffu, keep), mo = __ballot_sync(0xffffffffu, out);
+  if ((threadIdx.x & 31) == 0) {
+    if (mk) atomicAdd(t.stats + 0, (unsigned long long)__popc(mk));
+    if (mo) atomicAdd(t.stats + 1, (unsigned long long)__popc(mo));
+  }
+  if (!keep) return;
+  const unsigned long long mask = (unsigned long long)t.capacity - 1, tag = key + 1;
+  unsigned long long slot = mix64(key) & mask;
+  for (long long probe = 0; probe < t.capacity; ++probe, slot = (slot + 1) & mask) {
+    unsigned long long cur = __ldcg(t.keys + slot);        // a slot, once claimed, never changes
+    if (cur == 0) {
+      cur = atomicCAS(t.keys + slot, 0ull, tag);
+      if (cur == 0) {
+        if (atomicAdd(t.stats + 2, 1ull) >= half) return;   // more than capacity / 2 voxels: overflow
+        cur = tag;
+      }
+    }
+    if (cur == tag) {
+      unsigned long long* v = t.sums + 7 * slot;
+      atomicAdd(v, 1ull);
+#pragma unroll
+      for (int i = 0; i < 3; ++i) atomicAdd(v + 1 + i, fs[i]);
+#pragma unroll
+      for (int i = 0; i < 3; ++i) atomicAdd(v + 4 + i, (unsigned long long)cs[i]);
+      return;
+    }
+    if (occupied(t) > half) return;
+  }
+}
+
+// sort input: the key of every slot holding at least min_count points, NO_KEY (sorted last) for the others
+__global__ void __launch_bounds__(EX_THREADS) voxel_keys_kernel(const LrfVoxelTable t, unsigned long long min_count,
+                                                                unsigned long long* keys, unsigned int* slots) {
+  const long long i = (long long)blockIdx.x * EX_THREADS + threadIdx.x;
+  if (i >= t.capacity) return;
+  const unsigned long long tag = t.keys[i];
+  keys[i] = (tag != 0 && t.sums[7 * i] >= min_count) ? tag - 1 : NO_KEY;
+  slots[i] = (unsigned int)i;
+}
+
+__global__ void __launch_bounds__(EX_THREADS) voxel_write_kernel(const LrfVoxelTable t, const unsigned long long* keys,
+                                                                 const unsigned int* slots, float* xyz,
+                                                                 unsigned char* rgb, int* count, long long* n_out) {
+  const long long i = (long long)blockIdx.x * EX_THREADS + threadIdx.x;
+  if (i >= t.capacity) return;
+  const unsigned long long key = keys[i];
+  if (key == NO_KEY) {
+    if (i == 0) *n_out = 0;
+    return;
+  }
+  if (i + 1 == t.capacity || keys[i + 1] == NO_KEY) *n_out = i + 1;
+  const unsigned long long* v = t.sums + 7 * (unsigned long long)slots[i];
+  const unsigned long long n = v[0];
+  const double cnt = __ull2double_rn(n);
+  const double fden = __dmul_rn(cnt, 4294967296.0), cden = __dmul_rn(cnt, 16777216.0);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const long long k = (long long)((key >> (KEY_BITS * (2 - a))) & ((1ull << KEY_BITS) - 1)) - (1 << 20);
+    const double pos = __dadd_rn((double)k, __ddiv_rn(__ull2double_rn(v[1 + a]), fden));
+    xyz[3 * i + a] = __double2float_rn(__dadd_rn((double)t.origin[a], __dmul_rn(pos, (double)t.voxel_size)));
+    const double c = __dadd_rn(__dmul_rn(__ddiv_rn(__ull2double_rn(v[4 + a]), cden), 255.0), 0.5);
+    rgb[3 * i + a] = (unsigned char)floor(c);
+  }
+  count[i] = n < 2147483647ull ? (int)n : 2147483647;
+}
+
+// The extract's scratch: the keys and slot indices (two buffers each, for CUB's double-buffered sort), then CUB's own
+// temporary storage.  With a null base only the size is computed.
+struct ExtractScratch {
+  cub::DoubleBuffer<unsigned long long> keys;
+  cub::DoubleBuffer<unsigned int> slots;
+  void* temp;
+  size_t temp_bytes;
+  size_t total;
+};
+
+cudaError_t extract_scratch(void* base, long long cap, ExtractScratch& x) {
+  ScratchCarver c(base);
+  unsigned long long* k0 = c.take<unsigned long long>(cap * 8, 256);
+  unsigned long long* k1 = c.take<unsigned long long>(cap * 8, 256);
+  unsigned int* s0 = c.take<unsigned int>(cap * 4, 256);
+  unsigned int* s1 = c.take<unsigned int>(cap * 4, 256);
+  x.keys = cub::DoubleBuffer<unsigned long long>(k0, k1);
+  x.slots = cub::DoubleBuffer<unsigned int>(s0, s1);
+  x.temp_bytes = 0;
+  const cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, x.temp_bytes, x.keys, x.slots, (int)cap, 0, 64);
+  x.temp = c.take(x.temp_bytes, 256);
+  x.total = c.size(256);
+  return e;
+}
+
+}  // namespace
+
+cudaError_t launch_ray_opacity(const float* w, long long n, int S, long long n_views, const float* blend,
+                               long long blend_stride, int accumulate, float* acc, cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  const unsigned blocks = (unsigned)((n + OP_RAYS - 1) / OP_RAYS);
+  ray_opacity_kernel<<<blocks, OP_RAYS, 0, stream>>>(w, n, S, n / n_views, blend, blend_stride, accumulate, acc);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, cudaStream_t stream) {
+  if (f.n_rays == 0) return cudaSuccess;
+  const unsigned blocks = (unsigned)((f.n_rays + PT_THREADS - 1) / PT_THREADS);
+  frame_points_kernel<<<blocks, PT_THREADS, 0, stream>>>(f, t);
+  return cudaGetLastError();
+}
+
+cudaError_t voxel_extract_scratch_bytes(long long cap, size_t& bytes) {
+  ExtractScratch x;
+  const cudaError_t e = extract_scratch(nullptr, cap, x);
+  bytes = x.total;
+  return e;
+}
+
+cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, float* xyz, unsigned char* rgb,
+                                 int* count, long long* n_out, void* scratch, cudaStream_t stream) {
+  ExtractScratch x;
+  cudaError_t e = extract_scratch(scratch, t.capacity, x);
+  if (e != cudaSuccess) return e;
+  const unsigned blocks = (unsigned)((t.capacity + EX_THREADS - 1) / EX_THREADS);
+  voxel_keys_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, (unsigned long long)min_count, x.keys.Current(),
+                                                        x.slots.Current());
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  e = cub::DeviceRadixSort::SortPairs(x.temp, x.temp_bytes, x.keys, x.slots, (int)t.capacity, 0, 64, stream);
+  if (e != cudaSuccess) return e;
+  voxel_write_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, x.keys.Current(), x.slots.Current(), xyz, rgb, count,
+                                                         n_out);
+  return cudaGetLastError();
+}
+
+}  // namespace lrf

@@ -784,3 +784,32 @@ class LocalTensorfs(torch.nn.Module):
             if exchange is not None:
                 exchange[0].close_step(stream)
         return rgbs, depth, directions, ij
+
+    def _eval_plan(self, view, n, W, H, test_id, dev):
+        """The (uncached) plan of an eval forward of `n` rays of one view, with forward's defaults (white background,
+        floater_thresh = 0), or None when no field renders the view."""
+        active = torch.nonzero(self._blend_host()[view])[:, 0].tolist()
+        if not active:
+            return None
+        blend = self.blending_weights.detach()[view:view + 1].to(dev, torch.float32).contiguous()
+        return self._resolve([view], n, W, H, True, False, None, self.world2rf, None, blend, active, n, test_id, 0, dev)
+
+    def _run_weights(self, plan, ids_ptr, outs, weights, acc):
+        """_run for a one-chunk eval plan without exchange, where every launch also writes its per-sample weights into
+        `weights` (fp32, at least n x S of every field) and lrf_ray_opacity folds them, with the launch's blend, into
+        the blended opacity `acc` [n]."""
+        _, rgbs, depth, directions, ij = outs
+        o = _lib.LrfOutputs(rgb=rgbs.data_ptr(), depth=depth.data_ptr(), weights=weights.data_ptr(),
+                            directions=directions.data_ptr(), ij=ij.data_ptr())
+        lib = _lib.lib()
+        with torch.cuda.device(plan.dev):
+            stream = _stream(plan.dev)
+            for pos, (rf, z, b, lo, last) in enumerate(plan.launches):
+                fs, prep = rf.field_and_prepared(z)
+                if b.n_rays * fs.n_samples > weights.numel():
+                    raise ValueError("localrf_b200: the weights buffer is smaller than n_rays x n_samples")
+                b.ray_ids = ids_ptr
+                _lib.check(lib.lrf_render(C.byref(fs), _ptr(prep), C.byref(b), C.byref(o), stream))
+                _lib.check(lib.lrf_ray_opacity(o.weights, b.n_rays, fs.n_samples, b.n_views, b.blend, b.blend_stride,
+                                               int(pos > 0), acc.data_ptr(), stream))
+        return rgbs, depth, directions, ij
