@@ -2,7 +2,6 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
-#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -11,93 +10,7 @@
 #include "../../include/localrf_b200.h"
 #include "lrf_common.cuh"
 #include "lrf_launch.cuh"
-
-namespace lrf {
-size_t render_smem_bytes(int S, bool floater, int max_smem, bool pe);
-int render_threads();
-cudaError_t launch_render(const FieldDev& F, const BatchDev& B, int n_sms, int max_smem,
-                          cudaStream_t stream);
-cudaError_t launch_prepare(const float* basis, const float* w1, const float* b1, const float* w2,
-                           const float* b2, const float* w3, const float* b3, unsigned char* prep,
-                           cudaStream_t stream);
-cudaError_t launch_prepare_pe(const float* basis, const float* w1, const float* b1, const float* w2,
-                              const float* b2, const float* w3, const float* b3, int fea_pe, int view_pe,
-                              unsigned char* prep, cudaStream_t stream);
-cudaError_t launch_mlp(const float* prep, const float* feats, const float* viewdirs, long long M,
-                       float* rgb, int n_sms, cudaStream_t stream);
-cudaError_t launch_density_feature(const FieldDev& F, const float* xyz, long long M, float* out,
-                                   cudaStream_t stream);
-cudaError_t launch_app_feature(const FieldDev& F, const float* basis, const float* xyz,
-                               long long M, float* out, cudaStream_t stream);
-cudaError_t launch_repack(const float* src, float* dst, int C, long long HW, cudaStream_t stream);
-cudaError_t launch_pack_bf16(const float* src, void* dst, long long n, int n_sms, cudaStream_t stream);
-cudaError_t launch_alpha_mask_build(const FieldDev& F, const float* aabb_max, const int* dims, float length,
-                                    float thres, float* alpha_scratch, float* mask,
-                                    unsigned long long* kept, int n_sms, cudaStream_t stream);
-cudaError_t launch_upsample(const float* src, int H, int W, float* dst, int H2, int W2, int C, int n_sms,
-                            cudaStream_t stream);
-cudaError_t launch_density_l1(const FieldDev& F, double* sum, int n_sms, cudaStream_t stream);
-cudaError_t launch_density_l1_backward(const FieldDev& F, const float* gout, float* const* d_plane,
-                                       float* const* d_line, cudaStream_t stream);
-cudaError_t launch_tv(const float* x, int H, int W, int C, double* sums, int n_sms, cudaStream_t stream);
-cudaError_t launch_tv_backward(const float* x, int H, int W, int C, const float* gout, float kh, float kw,
-                               float* dx, int n_sms, cudaStream_t stream);
-cudaError_t launch_sample_ray(const float* rays, const float* jitter, long long N, int S, const float* aabb,
-                              float near, float far, float step, float* pts, float* z,
-                              unsigned char* inside, int n_sms, cudaStream_t stream);
-cudaError_t launch_peer_barrier(unsigned long long* const* peer_flags, int rank, int world,
-                                unsigned long long seq, unsigned long long wait_seq, cudaStream_t stream);
-cudaError_t launch_frame_u8(const float* rgb, int rgb_stride, const float* depth, int depth_stride, long long N,
-                            double d_lo, double d_hi, const unsigned char* lut, unsigned char* rgb8,
-                            unsigned char* depth8, int n_sms, cudaStream_t stream);
-size_t metrics_scratch_bytes(int H, int W);
-cudaError_t launch_image_metrics(const float* img, int img_stride, const float* gt, int gt_stride, int H, int W,
-                                 int fs, double sigma, double c1, double c2, double* out, double* ssim_map,
-                                 void* scratch, cudaStream_t stream);
-size_t losses_scratch_bytes(long long N, long long V);
-cudaError_t launch_supervision_losses(const LrfLossBatch& b, float* losses, void* scratch, cudaStream_t stream);
-cudaError_t launch_supervision_losses_backward(const LrfLossBatch& b, const float* grad_losses, const LrfLossGrads& g,
-                                               void* scratch, cudaStream_t stream);
-cudaError_t launch_adam_step(const LrfAdamTensor* t, long long n, cudaStream_t stream);
-cudaError_t launch_gather_rays(const LrfFrameStore& s, const LrfRayGather& g, cudaStream_t stream);
-size_t panels_scratch_bytes(long long n_px);
-cudaError_t launch_test_panels(const LrfPanelFrame& f, void* scratch, int n_sms, cudaStream_t stream);
-size_t ingest_scratch_bytes(long long n_px);
-int ingest_resize_mode(int ws, int hs, int w, int h);
-cudaError_t launch_ingest_frame(const LrfFrameStore& st, const LrfIngestFrame& f, void* scratch, cudaStream_t stream);
-cudaError_t launch_resize_linear(const float* src, int w0, int h0, long long src_stride, float* dst, int W, int H,
-                                 long long dst_stride, cudaStream_t stream);
-cudaError_t launch_app_products(const FieldDev& F, const float* xyz, long long M, float* out,
-                                cudaStream_t stream);
-cudaError_t launch_density_backward(const FieldDev& F, float* const* d_plane, float* const* d_line,
-                                    const float* xyz, const float* gout, long long M, float* dxyz,
-                                    cudaStream_t stream);
-cudaError_t launch_app_products_backward(const FieldDev& F, float* const* d_plane,
-                                         float* const* d_line, const float* xyz, const float* gout,
-                                         long long M, float* dxyz, cudaStream_t stream);
-size_t backward_prepared_bytes();
-size_t backward_scratch_bytes(long long n_rays, int S);
-cudaError_t launch_prepare_backward(const float* basis, const float* w1, const float* b1,
-                                    const float* w2, const float* b2, const float* w3,
-                                    const float* b3, float* bp, cudaStream_t stream);
-cudaError_t launch_render_backward_abi(const FieldDev& F, const float* rays, long long n_rays,
-                                       int white_bg, const float* g_rgb, const float* g_depth,
-                                       const float* bp, const LrfGradients& G, void* scratch,
-                                       int n_sms, cudaStream_t stream, float* dpos = nullptr);
-size_t train_backward_scratch_bytes(long long n, int S, long long V);
-cudaError_t launch_exposure_clamp(const float* x, const float* E, long long n, long long V, float* rgb, int n_sms,
-                                  cudaStream_t stream);
-cudaError_t launch_render_backward_batch(const FieldDev& F, const BatchDev& B, const float* bp, const float* x,
-                                         const float* g_rgb, const float* g_depth, const float* g_dirs,
-                                         const LrfGradients& G, const LrfCameraGrads& CG, void* scratch,
-                                         long long n_views, int n_sms, cudaStream_t stream);
-cudaError_t launch_ray_opacity(const float* w, long long n, int S, long long n_views, const float* blend,
-                               long long blend_stride, int accumulate, float* acc, cudaStream_t stream);
-cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, cudaStream_t stream);
-cudaError_t voxel_extract_scratch_bytes(long long cap, size_t& bytes);
-cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, float* xyz, unsigned char* rgb,
-                                 int* count, long long* n_out, void* scratch, cudaStream_t stream);
-}  // namespace lrf
+#include "lrf_launchers.cuh"
 
 namespace {
 
@@ -116,70 +29,135 @@ int cuda_fail(cudaError_t e, const char* where) {
 // the status an entry point returns for the launch it ends with
 int cuda_status(cudaError_t e, const char* where) { return e == cudaSuccess ? LRF_OK : cuda_fail(e, where); }
 
+constexpr int MAX_DEVICES = 64;
+constexpr unsigned int SCHED_RING = 256;
+
+// what the launches need of a device, queried once, and its ring of per-launch ray counters
 struct DevInfo {
   int n_sms = 0;
-  int max_smem = 0;
+  int max_smem = 0;                      // the opt-in limit of dynamic shared memory per block
+  int smem_per_sm = 0;                   // shared memory per SM
+  int smem_reserved = 0;                 // shared memory the system reserves per block
   bool ok = false;
   unsigned long long* sched = nullptr;   // ring of per-launch ray counters (device memory)
   unsigned int next = 0;                 // the ring's slot lrf_render took last
 };
-constexpr unsigned int SCHED_RING = 256;
 
-// per-device launch resources, process-global (one ring of launch counters per device, allocated on first
-// use by whichever host thread gets there first; the autograd engine's worker threads share it).  take_slot:
-// advance the ring for the render launch that asks (d.next is then its slot).
+// The shared-memory settings of the kernels that change them (a handful), per device.  An entry's kernel is set once
+// and never changes, so a reader that finds its kernel's setting in place needs no lock.
+struct KernelSmem {
+  std::atomic<const void*> kernel{nullptr};
+  std::atomic<int> max_dynamic[MAX_DEVICES] = {};   // the dynamic shared memory the kernel may use
+  std::atomic<int> carveout_for[MAX_DEVICES] = {};  // the CTA size its carveout was chosen for (0: none chosen)
+};
+
+// Per-device launch state, process-global: each device's record is filled on first use by whichever host thread gets
+// there first (the autograd engine's worker threads share it).  g_mu guards g_devices and the writers of g_kernels.
+DevInfo g_devices[MAX_DEVICES];
+KernelSmem g_kernels[16];
+std::mutex g_mu;
+
+// fills the record of device `dev` (in [0, MAX_DEVICES)) on its first use; on failure `where` names the call that
+// failed.  Call with g_mu held.
+cudaError_t fill_device(int dev, const char*& where) {
+  DevInfo& d = g_devices[dev];
+  if (d.ok) return cudaSuccess;
+  cudaDeviceProp p;
+  cudaError_t e = cudaGetDeviceProperties(&p, dev);
+  if (e != cudaSuccess) { where = "cudaGetDeviceProperties"; return e; }
+  d.n_sms = p.multiProcessorCount;
+  d.max_smem = (int)p.sharedMemPerBlockOptin;
+  d.smem_per_sm = (int)p.sharedMemPerMultiprocessor;
+  d.smem_reserved = (int)p.reservedSharedMemPerBlock;
+  e = cudaMalloc(&d.sched, 2 * SCHED_RING * sizeof(unsigned long long));
+  if (e != cudaSuccess) { where = "cudaMalloc(ray counters)"; return e; }
+  d.ok = true;
+  return cudaSuccess;
+}
+
+// the current device's record.  take_slot: advance the ring for the render launch that asks (d.next is then its slot).
 int device_info(DevInfo& d, bool take_slot = false) {
-  static DevInfo cache[64];
-  static std::mutex mu;
-  std::lock_guard<std::mutex> lock(mu);
+  std::lock_guard<std::mutex> lock(g_mu);
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
-  if (dev < 0 || dev >= 64) return fail(LRF_ERR_INVALID, "device index out of range");
-  if (!cache[dev].ok) {
-    cudaDeviceProp p;
-    e = cudaGetDeviceProperties(&p, dev);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaGetDeviceProperties");
-    cache[dev].n_sms = p.multiProcessorCount;
-    cache[dev].max_smem = (int)p.sharedMemPerBlockOptin;
-    e = cudaMalloc(&cache[dev].sched, 2 * SCHED_RING * sizeof(unsigned long long));
-    if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc(ray counters)");
-    cache[dev].ok = true;
-  }
-  if (take_slot) cache[dev].next = (cache[dev].next + 1) % SCHED_RING;
-  d = cache[dev];
+  if (dev < 0 || dev >= MAX_DEVICES) return fail(LRF_ERR_INVALID, "device index out of range");
+  const char* where = "";
+  if ((e = fill_device(dev, where)) != cudaSuccess) return cuda_fail(e, where);
+  if (take_slot) g_devices[dev].next = (g_devices[dev].next + 1) % SCHED_RING;
+  d = g_devices[dev];
   return LRF_OK;
+}
+
+// the current device's SM count, for the entry points whose launch needs nothing else of the device
+int sm_count(int& n_sms) {
+  DevInfo d;
+  const int rc = device_info(d);
+  n_sms = d.n_sms;
+  return rc;
+}
+
+// the kernel's entry, read without the lock; null when it has none
+const KernelSmem* find_kernel(const void* kernel) {
+  for (const KernelSmem& t : g_kernels)
+    if (t.kernel.load(std::memory_order_acquire) == kernel) return &t;
+  return nullptr;
+}
+
+// the kernel's entry, claimed on first use; null when the table is full.  Call with g_mu held.
+KernelSmem* claim_kernel(const void* kernel) {
+  for (KernelSmem& t : g_kernels) {
+    const void* k = t.kernel.load(std::memory_order_relaxed);
+    if (k == kernel) return &t;
+    if (!k) {
+      t.kernel.store(kernel, std::memory_order_release);
+      return &t;
+    }
+  }
+  return nullptr;
 }
 
 }  // namespace
 
-// The dynamic shared memory each kernel may use, per device, for the kernels that raise it (a handful).  An entry's
-// kernel is set once and never changes, so a reader that finds its kernel configured needs no lock.
 cudaError_t lrf::set_max_dynamic_smem(const void* kernel, int bytes) {
-  struct OptIn {
-    std::atomic<const void*> kernel{nullptr};
-    std::atomic<int> bytes[64] = {};
-  };
-  static OptIn table[16];
-  static std::mutex mu;
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64) return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  for (const OptIn& t : table)
-    if (t.kernel.load(std::memory_order_acquire) == kernel && t.bytes[dev].load(std::memory_order_acquire) >= bytes)
-      return cudaSuccess;
-  std::lock_guard<std::mutex> lock(mu);
-  for (OptIn& t : table) {
-    const void* k = t.kernel.load(std::memory_order_relaxed);
-    if (k && k != kernel) continue;
-    if (!k) t.kernel.store(kernel, std::memory_order_release);
-    if (t.bytes[dev].load(std::memory_order_relaxed) >= bytes) return cudaSuccess;
-    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e == cudaSuccess) t.bytes[dev].store(bytes, std::memory_order_release);
-    return e;
-  }
-  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);   // the table is full
+  if (dev < 0 || dev >= MAX_DEVICES)
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  const KernelSmem* t = find_kernel(kernel);
+  if (t && t->max_dynamic[dev].load(std::memory_order_acquire) >= bytes) return cudaSuccess;
+  std::lock_guard<std::mutex> lock(g_mu);
+  KernelSmem* w = claim_kernel(kernel);
+  if (w && w->max_dynamic[dev].load(std::memory_order_relaxed) >= bytes) return cudaSuccess;
+  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess && w) w->max_dynamic[dev].store(bytes, std::memory_order_release);   // unless the table is full
+  return e;
+}
+
+// The carveout is the smallest step of the SM's shared memory that holds the CTA and the memory reserved per block,
+// so the L1 gets the rest; it is the code's choice, not the driver's.  A percentage that is not a step rounds up to
+// the next step.
+cudaError_t lrf::set_smem_carveout(const void* kernel, int cta_bytes) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= MAX_DEVICES) return cudaSuccess;   // no record of the device: the driver chooses
+  const KernelSmem* t = find_kernel(kernel);
+  if (t && t->carveout_for[dev].load(std::memory_order_acquire) == cta_bytes) return cudaSuccess;
+  std::lock_guard<std::mutex> lock(g_mu);
+  KernelSmem* w = claim_kernel(kernel);
+  if (w && w->carveout_for[dev].load(std::memory_order_relaxed) == cta_bytes) return cudaSuccess;
+  const char* where = "";
+  if ((e = fill_device(dev, where)) != cudaSuccess) return e;
+  const int per_sm = g_devices[dev].smem_per_sm, reserved = g_devices[dev].smem_reserved;
+  static const int steps_kb[] = {0, 8, 16, 32, 64, 100, 132, 164, 196, 228};   // sm_90
+  int pct = 100;
+  for (int kb : steps_kb)
+    if (kb * 1024 >= cta_bytes + reserved && kb * 1024 <= per_sm) { pct = (int)(kb * 1024LL * 100 / per_sm); break; }
+  e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+  if (e == cudaSuccess && w) w->carveout_for[dev].store(cta_bytes, std::memory_order_release);   // unless the table is full
+  return e;
 }
 
 namespace {
@@ -251,16 +229,32 @@ int make_field(const LrfField* f, bool need_mlp, bool need_table, const void* pr
   return LRF_OK;
 }
 
-// validates a batch of n_rays >= 1 -- its split into views when `per_view`, n_rays <= max_rays, and in ray-generation
-// mode (rays == NULL) its camera -- and fills the batch fields the render and its backward both read
-int make_batch(const LrfBatch* b, bool per_view, long long max_rays, lrf::BatchDev& B) {
+// n_rays >= 1 (>= 0 with allow_empty) rays split evenly into n_views >= 1 views
+bool views_ok(long long n_rays, long long n_views, bool allow_empty) {
+  return n_rays >= (allow_empty ? 0 : 1) && n_views >= 1 && n_rays % n_views == 0;
+}
+
+int check_views(long long n_rays, long long n_views, bool allow_empty) {
+  if (views_ok(n_rays, n_views, allow_empty)) return LRF_OK;
+  return fail(LRF_ERR_INVALID, allow_empty ? "n_rays must be a multiple of n_views >= 1"
+                                           : "n_rays must be a positive multiple of n_views");
+}
+
+// the ray count of a kernel that indexes rays with 32-bit integers
+int check_31_bits(long long n_rays) {
+  return n_rays > 2147483647LL ? fail(LRF_ERR_INVALID, "n_rays must fit 31 bits") : LRF_OK;
+}
+
+// validates a batch of n_rays >= 1 -- its split into views when `per_view`, n_rays < 2^31 when `fit_31`, and in
+// ray-generation mode (rays == NULL) its camera -- and fills the batch fields the render and its backward both read
+int make_batch(const LrfBatch* b, bool per_view, bool fit_31, lrf::BatchDev& B) {
   memset(&B, 0, sizeof(B));
+  int rc;
   if (per_view) {
-    if (b->n_rays < 1 || b->n_views < 1 || b->n_rays % b->n_views != 0)
-      return fail(LRF_ERR_INVALID, "n_rays must be a positive multiple of n_views");
+    if ((rc = check_views(b->n_rays, b->n_views, false)) != LRF_OK) return rc;
     B.rays_per_view = b->n_rays / b->n_views;
   }
-  if (b->n_rays > max_rays) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  if (fit_31 && (rc = check_31_bits(b->n_rays)) != LRF_OK) return rc;
   if (!b->rays) {
     if (!b->ray_ids || !b->cam2world) return fail(LRF_ERR_INVALID, "ray_ids/cam2world is NULL");
     if (b->W < 1 || b->H < 1) return fail(LRF_ERR_INVALID, "W/H must be positive");
@@ -331,6 +325,63 @@ int check_store(const LrfFrameStore* s, int& n_flow) {
   if (n_flow != 0 && n_flow != 4)
     return fail(LRF_ERR_INVALID, "the store's flow group is partly given: set all of fwd_flow, fwd_mask, bwd_flow, "
                                  "bwd_mask or none");
+  return LRF_OK;
+}
+
+// the plane / line gradient buffers of the lookups' backward and lrf_density_l1_backward; `aligned16`: the lookups'
+// backward adds into them with 16-byte vector atomics (lrf_density_l1_backward's scalar adds need float alignment only)
+int check_grads(float* const d_plane[3], float* const d_line[3], bool aligned16) {
+  if (!d_plane || !d_line) return fail(LRF_ERR_INVALID, "gradient pointer arrays are NULL");
+  for (int i = 0; i < 3; ++i) {
+    if (!d_plane[i] || !d_line[i]) return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
+    if (aligned16 && (((uintptr_t)d_plane[i] | (uintptr_t)d_line[i]) & 15))
+      return fail(LRF_ERR_INVALID, "plane/line gradient buffers must be 16-byte aligned");
+  }
+  return LRF_OK;
+}
+
+// the batch and scratch block of lrf_supervision_losses and its backward
+int check_loss_batch(const LrfLossBatch* b, const void* scratch, size_t scratch_bytes) {
+  if (!b) return fail(LRF_ERR_INVALID, "batch is NULL");
+  const int rc = check_views(b->n_rays, b->n_views, false);
+  if (rc != LRF_OK) return rc;
+  if (b->n_cams < 1) return fail(LRF_ERR_INVALID, "n_cams must be >= 1");
+  if (!b->rgb_map || !b->rgb_train || !b->loss_weights)
+    return fail(LRF_ERR_INVALID, "rgb_map / rgb_train / loss_weights is NULL");
+  if (b->use_flow && (!b->view_ids || !b->depth_map || !b->directions || !b->ij || !b->cam2world || !b->focal ||
+                      !b->center || !b->fwd_flow || !b->bwd_flow || !b->fwd_mask || !b->bwd_mask))
+    return fail(LRF_ERR_INVALID, "a pointer of the flow term is NULL");
+  if (b->use_depth && (!b->depth_map || !b->invdepths))
+    return fail(LRF_ERR_INVALID, "a pointer of the depth term is NULL");
+  if (b->n_rays / b->n_views > 4096) return fail(LRF_ERR_UNSUPPORTED, "more than 4096 rays per view");
+  return check_scratch(scratch, scratch_bytes, lrf::losses_scratch_bytes(b->n_rays, b->n_views), 8,
+                       "scratch_bytes is smaller than lrf_supervision_scratch_bytes(n_rays, n_views, n_cams)");
+}
+
+// the voxel table of lrf_frame_points and lrf_voxel_extract
+int check_voxel_table(const LrfVoxelTable* t) {
+  if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
+  if (t->capacity < 2 || t->capacity > (1LL << 30) || (t->capacity & (t->capacity - 1)))
+    return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  if (!(t->voxel_size > 0.0f) || !std::isfinite(t->voxel_size)) return fail(LRF_ERR_INVALID, "voxel_size must be > 0 and finite");
+  if (!std::isfinite(t->origin[0]) || !std::isfinite(t->origin[1]) || !std::isfinite(t->origin[2]))
+    return fail(LRF_ERR_INVALID, "origin must be finite");
+  if (!t->keys || !t->sums || !t->stats) return fail(LRF_ERR_INVALID, "keys / sums / stats of the table is NULL");
+  if (((uintptr_t)t->keys | (uintptr_t)t->sums | (uintptr_t)t->stats) & 7)
+    return fail(LRF_ERR_INVALID, "keys / sums / stats of the table must be 8-byte aligned");
+  return LRF_OK;
+}
+
+// the panel size of lrf_test_panels: two W x H panels index with 32-bit integers
+bool panel_size_ok(int32_t W, int32_t H) {
+  return W >= 1 && H >= 1 && 2 * (int64_t)W * H <= 2147483647LL;
+}
+
+// a plane of ws x hs with `per_px` values per pixel and a row stride of `stride` elements
+int check_plane(const void* p, int32_t ws, int32_t hs, int64_t stride, int per_px, const char* name) {
+  if (!p) return fail(LRF_ERR_INVALID, "%s is NULL", name);
+  if (ws < 1 || hs < 1) return fail(LRF_ERR_INVALID, "the %s plane's sizes must be >= 1", name);
+  if (stride < (int64_t)per_px * ws) return fail(LRF_ERR_INVALID, "the %s plane's row stride is shorter than a row", name);
   return LRF_OK;
 }
 
@@ -410,7 +461,7 @@ int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const
   }
   if (!o->pix && (!o->rgb || !o->depth)) return fail(LRF_ERR_INVALID, "rgb/depth output is NULL");
   lrf::BatchDev B;
-  rc = make_batch(b, b->blend || b->exposure || !b->rays, LLONG_MAX, B);
+  rc = make_batch(b, b->blend || b->exposure || !b->rays, /*fit_31=*/false, B);
   if (rc != LRF_OK) return rc;
   B.blend = b->blend;
   B.blend_stride = b->blend_stride;
@@ -470,11 +521,11 @@ int lrf_mlp_forward(const void* prepared, const float* feats, const float* viewd
   if ((uintptr_t)prepared & 15) return fail(LRF_ERR_INVALID, "prepared must be 16-byte aligned");
   if (M < 0 || (M > 0 && (!feats || !viewdirs || !rgb))) return fail(LRF_ERR_INVALID, "bad feats/viewdirs/rgb/M");
   if (M == 0) return LRF_OK;
-  DevInfo d;
-  int rc = device_info(d);
+  int n_sms = 0;
+  const int rc = sm_count(n_sms);
   if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_mlp(static_cast<const float*>(prepared), feats, viewdirs, M, rgb,
-                                     d.n_sms, (cudaStream_t)stream), "mlp_kernel");
+                                     n_sms, (cudaStream_t)stream), "mlp_kernel");
 }
 
 int lrf_density_feature(const LrfField* f, const float* xyz, int64_t M, float* out,
@@ -505,18 +556,6 @@ int lrf_app_products(const LrfField* f, const float* xyz, int64_t M, float* out,
   if (M < 0 || (M > 0 && (!xyz || !out))) return fail(LRF_ERR_INVALID, "bad xyz/out/M");
   if ((uintptr_t)out & 15) return fail(LRF_ERR_INVALID, "out must be 16-byte aligned");
   return cuda_status(lrf::launch_app_products(F, xyz, M, out, (cudaStream_t)stream), "app_products_kernel");
-}
-
-// the plane / line gradient buffers of the lookups' backward and lrf_density_l1_backward; `aligned16`: the lookups'
-// backward adds into them with 16-byte vector atomics (lrf_density_l1_backward's scalar adds need float alignment only)
-static int check_grads(float* const d_plane[3], float* const d_line[3], bool aligned16) {
-  if (!d_plane || !d_line) return fail(LRF_ERR_INVALID, "gradient pointer arrays are NULL");
-  for (int i = 0; i < 3; ++i) {
-    if (!d_plane[i] || !d_line[i]) return fail(LRF_ERR_INVALID, "gradient buffer is NULL");
-    if (aligned16 && (((uintptr_t)d_plane[i] | (uintptr_t)d_line[i]) & 15))
-      return fail(LRF_ERR_INVALID, "plane/line gradient buffers must be 16-byte aligned");
-  }
-  return LRF_OK;
 }
 
 int lrf_density_feature_backward(const LrfField* f, const float* xyz, const float* gout, int64_t M,
@@ -570,34 +609,32 @@ int lrf_render_backward(const LrfField* f, const void* prepared_bwd, const float
   if (rc != LRF_OK) return rc;
   if (n_rays < 0) return fail(LRF_ERR_INVALID, "n_rays < 0");
   if (n_rays == 0) return LRF_OK;
-  if (n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  if ((rc = check_31_bits(n_rays)) != LRF_OK) return rc;
   if (!rays || !grad_rgb || !grad_depth || !g) return fail(LRF_ERR_INVALID, "rays / grad_rgb / grad_depth / grads is NULL");
   if ((rc = check_field_grads(g, true)) != LRF_OK) return rc;
   if ((rc = check_scratch(scratch, scratch_bytes, lrf::backward_scratch_bytes(n_rays, F.S), 16,
                           "scratch is smaller than lrf_backward_scratch_bytes(n_rays, n_samples)")) != LRF_OK)
     return rc;
-  DevInfo d;
-  rc = device_info(d);
-  if (rc != LRF_OK) return rc;
+  int n_sms = 0;
+  if ((rc = sm_count(n_sms)) != LRF_OK) return rc;
   return cuda_status(lrf::launch_render_backward_abi(F, rays, n_rays, white_bg, grad_rgb, grad_depth,
                                                      static_cast<const float*>(prepared_bwd), *g, scratch,
-                                                     d.n_sms, (cudaStream_t)stream), "render_backward");
+                                                     n_sms, (cudaStream_t)stream), "render_backward");
 }
 
 int lrf_exposure_clamp(const float* x, const float* exposure, int64_t n_rays, int64_t n_views, float* rgb,
                        lrf_stream_t stream) {
-  if (n_rays < 0 || n_views < 1 || n_rays % n_views != 0)
-    return fail(LRF_ERR_INVALID, "n_rays must be a multiple of n_views >= 1");
-  if (n_rays > 0 && (!x || !rgb)) return fail(LRF_ERR_INVALID, "rgb_linear / rgb is NULL");
-  DevInfo d;
-  int rc = device_info(d);
+  int rc = check_views(n_rays, n_views, true);
   if (rc != LRF_OK) return rc;
-  return cuda_status(lrf::launch_exposure_clamp(x, exposure, n_rays, n_views, rgb, d.n_sms,
+  if (n_rays > 0 && (!x || !rgb)) return fail(LRF_ERR_INVALID, "rgb_linear / rgb is NULL");
+  int n_sms = 0;
+  if ((rc = sm_count(n_sms)) != LRF_OK) return rc;
+  return cuda_status(lrf::launch_exposure_clamp(x, exposure, n_rays, n_views, rgb, n_sms,
                                                 (cudaStream_t)stream), "exposure_clamp_kernel");
 }
 
 size_t lrf_backward_batch_scratch_bytes(int64_t n_rays, int32_t n_samples, int64_t n_views) {
-  if (n_rays < 1 || n_samples < 2 || n_views < 1 || n_rays % n_views != 0) return 0;
+  if (n_samples < 2 || !views_ok(n_rays, n_views, false)) return 0;
   return lrf::train_backward_scratch_bytes(n_rays, n_samples, n_views);
 }
 
@@ -614,18 +651,18 @@ int lrf_render_backward_batch(const LrfField* f, const void* prepared_bwd, const
   if (b->accumulate) return fail(LRF_ERR_INVALID, "accumulate is not supported by the batch backward");
   if (b->blend) return fail(LRF_ERR_INVALID, "a blend pointer is not supported by the batch backward");
   lrf::BatchDev B;
-  if ((rc = make_batch(b, true, 2147483647LL, B)) != LRF_OK) return rc;
+  if ((rc = make_batch(b, true, /*fit_31=*/true, B)) != LRF_OK) return rc;
   if (!x || !grad_rgb || !grad_depth) return fail(LRF_ERR_INVALID, "rgb_linear / grad_rgb / grad_depth is NULL");
   if ((rc = check_field_grads(g, false)) != LRF_OK) return rc;
   rc = check_scratch(scratch, scratch_bytes, lrf::train_backward_scratch_bytes(b->n_rays, F.S, b->n_views), 16,
                      "scratch is smaller than lrf_backward_batch_scratch_bytes(n_rays, n_samples, n_views)");
   if (rc != LRF_OK) return rc;
   if (b->floater_thresh > 0.0f) return fail(LRF_ERR_UNSUPPORTED, "the backward is built for floater_thresh = 0");
-  DevInfo d;
-  if ((rc = device_info(d)) != LRF_OK) return rc;
+  int n_sms = 0;
+  if ((rc = sm_count(n_sms)) != LRF_OK) return rc;
   return cuda_status(lrf::launch_render_backward_batch(F, B, static_cast<const float*>(prepared_bwd), x, grad_rgb,
                                                        grad_depth, grad_directions, *g, *cg, scratch, b->n_views,
-                                                       d.n_sms, (cudaStream_t)stream), "render_backward_batch");
+                                                       n_sms, (cudaStream_t)stream), "render_backward_batch");
 }
 
 int lrf_alpha_mask_build(const LrfField* f, const int32_t dims[3], float length, float thres,
@@ -636,11 +673,11 @@ int lrf_alpha_mask_build(const LrfField* f, const int32_t dims[3], float length,
   if (!dims || dims[0] < 1 || dims[1] < 1 || dims[2] < 1) return fail(LRF_ERR_INVALID, "lattice dims must be >= 1");
   if (!alpha_scratch) return fail(LRF_ERR_INVALID, "alpha_scratch is NULL");
   if (mask && !kept) return fail(LRF_ERR_INVALID, "kept is NULL");
-  DevInfo d;
-  if ((rc = device_info(d)) != LRF_OK) return rc;
+  int n_sms = 0;
+  if ((rc = sm_count(n_sms)) != LRF_OK) return rc;
   const int dd[3] = {dims[0], dims[1], dims[2]};
   return cuda_status(lrf::launch_alpha_mask_build(F, f->aabb + 3, dd, length, thres, alpha_scratch, mask, kept,
-                                                  d.n_sms, (cudaStream_t)stream), "alpha_mask_build");
+                                                  n_sms, (cudaStream_t)stream), "alpha_mask_build");
 }
 
 int lrf_upsample(const float* src, int32_t H, int32_t W, float* dst, int32_t H2, int32_t W2, int32_t C,
@@ -648,10 +685,10 @@ int lrf_upsample(const float* src, int32_t H, int32_t W, float* dst, int32_t H2,
   if (!src || !dst || H < 1 || W < 1 || H2 < 1 || W2 < 1 || C < 4 || (C & 3))
     return fail(LRF_ERR_INVALID, "bad upsample arguments (C must be a positive multiple of 4)");
   if (((uintptr_t)src | (uintptr_t)dst) & 15) return fail(LRF_ERR_INVALID, "upsample buffers must be 16-byte aligned");
-  DevInfo d;
-  int rc = device_info(d);
+  int n_sms = 0;
+  const int rc = sm_count(n_sms);
   if (rc != LRF_OK) return rc;
-  return cuda_status(lrf::launch_upsample(src, H, W, dst, H2, W2, C, d.n_sms, (cudaStream_t)stream), "upsample_kernel");
+  return cuda_status(lrf::launch_upsample(src, H, W, dst, H2, W2, C, n_sms, (cudaStream_t)stream), "upsample_kernel");
 }
 
 int lrf_density_l1(const LrfField* f, double* sum, lrf_stream_t stream) {
@@ -659,9 +696,9 @@ int lrf_density_l1(const LrfField* f, double* sum, lrf_stream_t stream) {
   int rc = make_field(f, false, false, nullptr, F);
   if (rc != LRF_OK) return rc;
   if (!sum) return fail(LRF_ERR_INVALID, "sum is NULL");
-  DevInfo d;
-  if ((rc = device_info(d)) != LRF_OK) return rc;
-  return cuda_status(lrf::launch_density_l1(F, sum, d.n_sms, (cudaStream_t)stream), "density_l1_fwd_kernel");
+  int n_sms = 0;
+  if ((rc = sm_count(n_sms)) != LRF_OK) return rc;
+  return cuda_status(lrf::launch_density_l1(F, sum, n_sms, (cudaStream_t)stream), "density_l1_fwd_kernel");
 }
 
 int lrf_density_l1_backward(const LrfField* f, const float* grad_out, float* const d_plane[3],
@@ -677,19 +714,19 @@ int lrf_density_l1_backward(const LrfField* f, const float* grad_out, float* con
 
 int lrf_tv_sums(const float* x, int32_t H, int32_t W, int32_t C, double* sums, lrf_stream_t stream) {
   if (!x || !sums || H < 1 || W < 1 || C < 1) return fail(LRF_ERR_INVALID, "bad tv arguments");
-  DevInfo d;
-  int rc = device_info(d);
+  int n_sms = 0;
+  const int rc = sm_count(n_sms);
   if (rc != LRF_OK) return rc;
-  return cuda_status(lrf::launch_tv(x, H, W, C, sums, d.n_sms, (cudaStream_t)stream), "tv_fwd_kernel");
+  return cuda_status(lrf::launch_tv(x, H, W, C, sums, n_sms, (cudaStream_t)stream), "tv_fwd_kernel");
 }
 
 int lrf_tv_sums_backward(const float* x, int32_t H, int32_t W, int32_t C, const float* grad_out, float kh,
                          float kw, float* dx, lrf_stream_t stream) {
   if (!x || !dx || !grad_out || H < 1 || W < 1 || C < 1) return fail(LRF_ERR_INVALID, "bad tv arguments");
-  DevInfo d;
-  int rc = device_info(d);
+  int n_sms = 0;
+  const int rc = sm_count(n_sms);
   if (rc != LRF_OK) return rc;
-  return cuda_status(lrf::launch_tv_backward(x, H, W, C, grad_out, kh, kw, dx, d.n_sms,
+  return cuda_status(lrf::launch_tv_backward(x, H, W, C, grad_out, kh, kw, dx, n_sms,
                                              (cudaStream_t)stream), "tv_bwd_kernel");
 }
 
@@ -698,10 +735,10 @@ int lrf_sample_ray(const float* rays, const float* jitter, int64_t N, int32_t S,
                    lrf_stream_t stream) {
   if (N < 0 || S < 1 || !aabb) return fail(LRF_ERR_INVALID, "bad sample_ray sizes");
   if (N > 0 && (!rays || !pts || !z || !inside)) return fail(LRF_ERR_INVALID, "sample_ray buffer is NULL");
-  DevInfo d;
-  int rc = device_info(d);
+  int n_sms = 0;
+  const int rc = sm_count(n_sms);
   if (rc != LRF_OK) return rc;
-  return cuda_status(lrf::launch_sample_ray(rays, jitter, N, S, aabb, near, far, step, pts, z, inside, d.n_sms,
+  return cuda_status(lrf::launch_sample_ray(rays, jitter, N, S, aabb, near, far, step, pts, z, inside, n_sms,
                                             (cudaStream_t)stream), "sample_ray_kernel");
 }
 
@@ -711,11 +748,11 @@ int lrf_frame_to_u8(const float* rgb, int32_t rgb_stride, const float* depth, in
   if (N < 0) return fail(LRF_ERR_INVALID, "N < 0");
   if (rgb8 && (!rgb || rgb_stride < 3)) return fail(LRF_ERR_INVALID, "rgb8 requested without rgb / stride >= 3");
   if (depth8 && (!depth || depth_stride < 1 || !lut)) return fail(LRF_ERR_INVALID, "depth8 requested without depth / lut");
-  DevInfo d;
-  int rc = device_info(d);
+  int n_sms = 0;
+  const int rc = sm_count(n_sms);
   if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_frame_u8(rgb, rgb_stride, depth, depth_stride, N, d_lo, d_hi, lut, rgb8, depth8,
-                                          d.n_sms, (cudaStream_t)stream), "frame_u8_kernel");
+                                          n_sms, (cudaStream_t)stream), "frame_u8_kernel");
 }
 
 size_t lrf_image_metrics_scratch_bytes(int32_t H, int32_t W, int32_t filter_size) {
@@ -742,25 +779,8 @@ int lrf_image_metrics(const float* img, int32_t img_stride, const float* gt, int
                                                out, ssim_map, scratch, (cudaStream_t)stream), "metrics_tile_kernel");
 }
 
-static int check_loss_batch(const LrfLossBatch* b, const void* scratch, size_t scratch_bytes) {
-  if (!b) return fail(LRF_ERR_INVALID, "batch is NULL");
-  if (b->n_rays < 1 || b->n_views < 1 || b->n_rays % b->n_views != 0)
-    return fail(LRF_ERR_INVALID, "n_rays must be a positive multiple of n_views");
-  if (b->n_cams < 1) return fail(LRF_ERR_INVALID, "n_cams must be >= 1");
-  if (!b->rgb_map || !b->rgb_train || !b->loss_weights)
-    return fail(LRF_ERR_INVALID, "rgb_map / rgb_train / loss_weights is NULL");
-  if (b->use_flow && (!b->view_ids || !b->depth_map || !b->directions || !b->ij || !b->cam2world || !b->focal ||
-                      !b->center || !b->fwd_flow || !b->bwd_flow || !b->fwd_mask || !b->bwd_mask))
-    return fail(LRF_ERR_INVALID, "a pointer of the flow term is NULL");
-  if (b->use_depth && (!b->depth_map || !b->invdepths))
-    return fail(LRF_ERR_INVALID, "a pointer of the depth term is NULL");
-  if (b->n_rays / b->n_views > 4096) return fail(LRF_ERR_UNSUPPORTED, "more than 4096 rays per view");
-  return check_scratch(scratch, scratch_bytes, lrf::losses_scratch_bytes(b->n_rays, b->n_views), 8,
-                       "scratch_bytes is smaller than lrf_supervision_scratch_bytes(n_rays, n_views, n_cams)");
-}
-
 size_t lrf_supervision_scratch_bytes(int64_t n_rays, int64_t n_views, int64_t n_cams) {
-  if (n_rays < 1 || n_views < 1 || n_rays % n_views != 0 || n_cams < 1) return 0;
+  if (!views_ok(n_rays, n_views, false) || n_cams < 1) return 0;
   return lrf::losses_scratch_bytes(n_rays, n_views);
 }
 
@@ -794,11 +814,10 @@ int lrf_adam_step(const LrfAdamTensor* t, int64_t n, lrf_stream_t stream) {
 int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t stream) {
   if (!s || !g) return fail(LRF_ERR_INVALID, "store / gather is NULL");
   int n_flow = 0;
-  const int rc = check_store(s, n_flow);
+  int rc = check_store(s, n_flow);
   if (rc != LRF_OK) return rc;
-  if (g->n_rays < 0 || g->n_views < 1 || g->n_rays % g->n_views != 0)
-    return fail(LRF_ERR_INVALID, "n_rays must be a multiple of n_views >= 1");
-  if (g->n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  if ((rc = check_views(g->n_rays, g->n_views, true)) != LRF_OK) return rc;
+  if ((rc = check_31_bits(g->n_rays)) != LRF_OK) return rc;
   if (!g->ids || !g->idx || !g->rgb || !g->loss_weight)
     return fail(LRF_ERR_INVALID, "ids / idx / rgb / loss_weight of the gather is NULL");
   if (!s->invdepth != !g->invdepth)
@@ -808,26 +827,12 @@ int lrf_gather_rays(const LrfFrameStore* s, const LrfRayGather* g, lrf_stream_t 
   return cuda_status(lrf::launch_gather_rays(*s, *g, (cudaStream_t)stream), "gather_rays_kernel");
 }
 
-// the voxel table of lrf_frame_points and lrf_voxel_extract
-static int check_voxel_table(const LrfVoxelTable* t) {
-  if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
-  if (t->capacity < 2 || t->capacity > (1LL << 30) || (t->capacity & (t->capacity - 1)))
-    return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
-  if (!(t->voxel_size > 0.0f) || !std::isfinite(t->voxel_size)) return fail(LRF_ERR_INVALID, "voxel_size must be > 0 and finite");
-  if (!std::isfinite(t->origin[0]) || !std::isfinite(t->origin[1]) || !std::isfinite(t->origin[2]))
-    return fail(LRF_ERR_INVALID, "origin must be finite");
-  if (!t->keys || !t->sums || !t->stats) return fail(LRF_ERR_INVALID, "keys / sums / stats of the table is NULL");
-  if (((uintptr_t)t->keys | (uintptr_t)t->sums | (uintptr_t)t->stats) & 7)
-    return fail(LRF_ERR_INVALID, "keys / sums / stats of the table must be 8-byte aligned");
-  return LRF_OK;
-}
-
 int lrf_ray_opacity(const float* weights, int64_t n_rays, int32_t n_samples, int64_t n_views, const float* blend,
                     int64_t blend_stride, int32_t accumulate, float* acc, lrf_stream_t stream) {
   if (!weights || !acc) return fail(LRF_ERR_INVALID, "weights / acc is NULL");
-  if (n_rays < 0 || n_views < 1 || n_rays % n_views != 0)
-    return fail(LRF_ERR_INVALID, "n_rays must be a multiple of n_views >= 1");
-  if (n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
+  int rc = check_views(n_rays, n_views, true);
+  if (rc != LRF_OK) return rc;
+  if ((rc = check_31_bits(n_rays)) != LRF_OK) return rc;
   if (n_samples < 1) return fail(LRF_ERR_INVALID, "n_samples must be >= 1");
   return cuda_status(lrf::launch_ray_opacity(weights, n_rays, n_samples, n_views, blend, blend_stride, accumulate, acc,
                                              (cudaStream_t)stream), "ray_opacity_kernel");
@@ -867,10 +872,6 @@ int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uin
                                                (cudaStream_t)stream), "voxel_extract");
 }
 
-static bool panel_size_ok(int32_t W, int32_t H) {
-  return W >= 1 && H >= 1 && 2 * (int64_t)W * H <= 2147483647LL;
-}
-
 size_t lrf_test_panels_scratch_bytes(int32_t W, int32_t H) {
   return panel_size_ok(W, H) ? lrf::panels_scratch_bytes((long long)W * H) : 0;
 }
@@ -893,21 +894,12 @@ int lrf_test_panels(const LrfPanelFrame* f, void* scratch, size_t scratch_bytes,
   int rc = check_scratch(scratch, scratch_bytes, lrf_test_panels_scratch_bytes(f->W, f->H), 8,
                          "scratch_bytes is smaller than lrf_test_panels_scratch_bytes(W, H)");
   if (rc != LRF_OK) return rc;
-  DevInfo d;
-  rc = device_info(d);
-  if (rc != LRF_OK) return rc;
-  return cuda_status(lrf::launch_test_panels(*f, scratch, d.n_sms, (cudaStream_t)stream), "test_panels");
+  int n_sms = 0;
+  if ((rc = sm_count(n_sms)) != LRF_OK) return rc;
+  return cuda_status(lrf::launch_test_panels(*f, scratch, n_sms, (cudaStream_t)stream), "test_panels");
 }
 
 size_t lrf_ingest_scratch_bytes(int64_t n_px) { return n_px >= 1 ? lrf::ingest_scratch_bytes(n_px) : 0; }
-
-// a plane of ws x hs with `per_px` values per pixel and a row stride of `stride` elements
-static int check_plane(const void* p, int32_t ws, int32_t hs, int64_t stride, int per_px, const char* name) {
-  if (!p) return fail(LRF_ERR_INVALID, "%s is NULL", name);
-  if (ws < 1 || hs < 1) return fail(LRF_ERR_INVALID, "the %s plane's sizes must be >= 1", name);
-  if (stride < (int64_t)per_px * ws) return fail(LRF_ERR_INVALID, "the %s plane's row stride is shorter than a row", name);
-  return LRF_OK;
-}
 
 int lrf_ingest_frame(const LrfFrameStore* s, const LrfIngestFrame* f, void* scratch, size_t scratch_bytes,
                      lrf_stream_t stream) {
@@ -978,10 +970,10 @@ int lrf_peer_signal_wait(unsigned long long* const* peer_flags, int32_t rank, in
 int lrf_pack_bf16(const float* src, void* dst, int64_t n, lrf_stream_t stream) {
   if (n < 0 || (n > 0 && (!src || !dst))) return fail(LRF_ERR_INVALID, "bad src/dst/n");
   if ((uintptr_t)dst & 1) return fail(LRF_ERR_INVALID, "dst must be 2-byte aligned");
-  DevInfo d;
-  int rc = device_info(d);
+  int n_sms = 0;
+  const int rc = sm_count(n_sms);
   if (rc != LRF_OK) return rc;
-  return cuda_status(lrf::launch_pack_bf16(src, dst, n, d.n_sms, (cudaStream_t)stream), "pack_bf16_kernel");
+  return cuda_status(lrf::launch_pack_bf16(src, dst, n, n_sms, (cudaStream_t)stream), "pack_bf16_kernel");
 }
 
 int lrf_repack_nchw_to_nhwc(const float* src, float* dst, int32_t C, int32_t H, int32_t W,

@@ -2,6 +2,7 @@
 // explicit features (lrf_mlp_forward), weight preparation, stand-alone feature lookups, repack.
 #include "lrf_device.cuh"
 #include "lrf_launch.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

@@ -27,6 +27,7 @@
 
 #include "lrf_device.cuh"
 #include "lrf_launch.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 
@@ -719,9 +720,6 @@ __global__ void prepare_backward_kernel(const float* __restrict__ basis, const f
 
 // ---- host-side launchers --------------------------------------------------------------------------
 size_t backward_prepared_bytes() { return (size_t)BP_FLOATS * sizeof(float); }
-cudaError_t launch_prepare(const float* basis, const float* w1, const float* b1, const float* w2,
-                           const float* b2, const float* w3, const float* b3, unsigned char* prep,
-                           cudaStream_t stream);
 size_t backward_scratch_bytes(long long n_rays, int S) {
   ScratchCarver c(nullptr);
   carve(c, n_rays, S);

@@ -11,6 +11,7 @@
 #include <stdint.h>
 
 #include "../../include/localrf_b200.h"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

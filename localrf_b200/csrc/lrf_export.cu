@@ -18,6 +18,7 @@
 
 #include "../../include/localrf_b200.h"
 #include "lrf_launch.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

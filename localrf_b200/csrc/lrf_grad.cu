@@ -6,6 +6,7 @@
 // used by compute_densityfeature / compute_appfeature (models/tensoRF.py:112-196); a clipped
 // coordinate gets zero gradient (ATen clip_coordinates_set_grad).
 #include "lrf_device.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

@@ -1,6 +1,6 @@
 // lrf_launch.cuh -- the launch conventions the kernel files share: the fixed-order fp64 CTA sum, the CTA count of a
 // capped grid-stride launch, the carving of a caller's scratch block, and the one-time opt-in to large dynamic shared
-// memory.
+// memory and choice of the shared-memory carveout.
 //
 // Not included from lrf_common.cuh or lrf_device.cuh: tests/host_emul compiles those with a host compiler.
 #pragma once
@@ -55,5 +55,10 @@ struct ScratchCarver {
 // exceeds what this kernel already has there.  Safe under concurrent callers; a kernel already configured takes no
 // lock.  Defined in lrf_abi.cu.
 cudaError_t set_max_dynamic_smem(const void* kernel, int bytes);
+
+// Sets `kernel`'s shared-memory carveout on the current device to the smallest step that holds a CTA of `cta_bytes`
+// of shared memory, when it was last set for another CTA size.  Safe under concurrent callers, as above.  Defined in
+// lrf_abi.cu.
+cudaError_t set_smem_carveout(const void* kernel, int cta_bytes);
 
 }  // namespace lrf

@@ -22,6 +22,7 @@
 #include "lrf_reproject.cuh"
 #define LRF_SELECT_KEYS_ONLY
 #include "lrf_select.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

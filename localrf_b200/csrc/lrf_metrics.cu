@@ -16,6 +16,7 @@
 #include <cuda_runtime.h>
 
 #include "lrf_launch.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

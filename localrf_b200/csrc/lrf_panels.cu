@@ -22,6 +22,7 @@
 #include "lrf_launch.cuh"
 #include "lrf_reproject.cuh"
 #include "lrf_select.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

@@ -35,6 +35,7 @@
 // the L1 60 KB for the texel gathers.
 #include "lrf_device.cuh"
 #include "lrf_launch.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 
@@ -666,26 +667,8 @@ cudaError_t launch_render(const FieldDev& F, const BatchDev& B, int n_sms, int m
   const void* kern = variant == 1 ? (const void*)render_kernel_t<true, false>
                    : variant == 2 ? (const void*)render_kernel_t<false, true> : (const void*)render_kernel_t<false, false>;
   cudaError_t e = set_max_dynamic_smem(kern, (int)smem);
+  if (e == cudaSuccess) e = set_smem_carveout(kern, (int)smem);   // the L1 gets what the CTA leaves
   if (e != cudaSuccess) return e;
-  int dev = 0;
-  e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  // The shared-memory carveout is the smallest step that holds this launch's CTA, so the L1 gets the rest;
-  // it is the code's choice, not the driver's.  A percentage that is not a step rounds up to the next step.
-  static size_t carved[3][64] = {{0}, {0}, {0}};       // per kernel, per device: the CTA size the carveout was set for
-  if (dev >= 0 && dev < 64 && smem != carved[variant][dev]) {
-    int per_sm = 0, reserved = 0;
-    e = cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
-    if (e != cudaSuccess) return e;
-    static const int steps_kb[] = {0, 8, 16, 32, 64, 100, 132, 164, 196, 228};   // sm_90
-    int pct = 100;
-    for (int kb : steps_kb)
-      if (kb * 1024 >= (int)smem + reserved && kb * 1024 <= per_sm) { pct = (int)(kb * 1024LL * 100 / per_sm); break; }
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-    if (e != cudaSuccess) return e;
-    carved[variant][dev] = smem;
-  }
   e = cudaMemsetAsync(B.sched, 0, 2 * sizeof(unsigned long long), stream);   // ray counter + finished-CTA counter
   if (e != cudaSuccess) return e;
   // a CTA per SM, but never more CTAs than there are groups of 8 rays

@@ -8,6 +8,7 @@
 //   sample_ray                     ray-AABB intersection sampler       models/tensorBase.py:396-417
 #include "lrf_device.cuh"
 #include "lrf_launch.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
 

@@ -15,14 +15,9 @@
 #include "../../include/localrf_b200.h"
 #include "lrf_device.cuh"
 #include "lrf_launch.cuh"
+#include "lrf_launchers.cuh"
 
 namespace lrf {
-
-size_t backward_scratch_bytes(long long n_rays, int S);
-cudaError_t launch_render_backward_abi(const FieldDev& F, const float* rays, long long n_rays, int white_bg,
-                                       const float* g_rgb, const float* g_depth, const float* bp,
-                                       const LrfGradients& G, void* scratch, int n_sms, cudaStream_t stream,
-                                       float* dpos);
 
 namespace {
 
