@@ -32,15 +32,16 @@ constexpr int KEY_BITS = 21;           // per axis: keys in [-2^20, 2^20), 63 bi
 constexpr float KEY_LIM = 1048576.0f;  // 2^20
 constexpr unsigned long long NO_KEY = ~0ull;
 
-// One thread per ray sums its weights in sample order in fp64.  The [rays][S] rows are read a tile at a time,
-// coalesced, into padded shared rows, so every thread's sequential sum reads its own row without bank conflicts.
+// One thread per ray sums its weights in sample order in fp64, from -0 (the identity of IEEE addition, so a row of -0
+// sums to -0 as np.cumsum does).  The [rays][S] rows are read a tile at a time, coalesced, into padded shared rows, so
+// every thread's sequential sum reads its own row without bank conflicts.
 __global__ void __launch_bounds__(OP_RAYS) ray_opacity_kernel(const float* __restrict__ w, long long n, int S,
                                                               long long rays_per_view, const float* __restrict__ blend,
                                                               long long blend_stride, int accumulate, float* acc) {
   __shared__ float tile[OP_RAYS][OP_TILE + 1];
   const long long r0 = (long long)blockIdx.x * OP_RAYS;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  double s = 0.0;
+  double s = -0.0;
   for (int k0 = 0; k0 < S; k0 += OP_TILE) {
     __syncthreads();
     for (int row = warp; row < OP_RAYS; row += OP_RAYS / 32) {

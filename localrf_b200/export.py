@@ -31,7 +31,9 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
     (max-norm) of the centre of a field that renders the view.  Views in `test_ids` use the neighbour-averaged exposure
     of held-out frames (forward's test_id).  Voxels with fewer than `min_count` points are dropped.  The voxel table has
     `capacity` slots (a power of two) and holds at most capacity / 2 voxels; a scene with more raises RuntimeError.  A
-    view renders in chunks of at most weights_budget / (4 S) rays (S: the largest sample count of the fields).
+    view renders in chunks of at most weights_budget / (4 S) rays, S the longest eval distance table of the fields
+    (`TensorBase.sample_table`, 2 (nSamples // 6) samples: the weights each ray's render writes).  W or H below 1
+    raises ValueError.
 
     -> dict(xyz [P,3] float32, rgb [P,3] uint8, count [P] int32 (CUDA tensors, one row per voxel in ascending voxel-key
     order: x, then y, then z), n_rays (rays rendered), n_kept (points merged), n_out_of_range (points whose voxel index
@@ -46,11 +48,14 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
     tests = {int(v) for v in test_ids}
     if not tests <= set(views):
         raise ValueError("test_ids must be among the exported view_ids")
-    S = max(int(rf.nSamples) for rf in lt.tensorfs)
+    W, H = int(W), int(H)
+    if W < 1 or H < 1:
+        raise ValueError(f"W and H must be >= 1 (got W={W}, H={H})")
+    S = max(rf.sample_table(False, -1, dev).numel() for rf in lt.tensorfs)
     per_chunk = int(weights_budget) // (4 * S)
     if per_chunk < 1:
         raise ValueError(f"weights_budget must hold one ray's weights ({4 * S} bytes)")
-    n = int(W) * int(H)
+    n = W * H
     per_chunk = min(per_chunk, n)
     capacity = int(capacity)
     if capacity < 2 or capacity > 1 << 30 or capacity & (capacity - 1):

@@ -97,6 +97,110 @@ def extract(table, min_count, voxel_size, origin):
     return xyz, rgb, count
 
 
+def mix64(x):
+    """splitmix64's finaliser of uint64 keys (numpy array or int), the probe start of lrf_frame_points."""
+    x = np.asarray(x, np.uint64)
+    with np.errstate(over="ignore"):
+        x = (x ^ (x >> np.uint64(30))) * np.uint64(0xbf58476d1ce4e5b9)
+        x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94d049bb133111eb)
+    return x ^ (x >> np.uint64(31))
+
+
+def pack_key(k):
+    """voxel index [.., 3] (each in [-2^20, 2^20)) -> the table's 63-bit key."""
+    k = np.asarray(k, np.int64) + KEY_LIM
+    return (k[..., 0] << 2 * KEY_BITS) | (k[..., 1] << KEY_BITS) | k[..., 2]
+
+
+def probe_table(keys, capacity):
+    """The occupied slots of an insert-only linear-probing table of `capacity` (a power of two) slots after the
+    distinct `keys` are inserted, each probing from mix64(key) & (capacity - 1) upwards and wrapping to 0.  The set of
+    occupied slots does not depend on the insertion order, so a concurrent insert ends with the same set."""
+    mask = capacity - 1
+    taken = set()
+    for h in (mix64(np.asarray(sorted(set(int(k) for k in keys)), np.uint64)) & np.uint64(mask)).tolist():
+        slot = int(h)
+        while slot in taken:
+            slot = (slot + 1) & mask
+        taken.add(slot)
+    return taken
+
+
+U32 = 2.0 ** -24                      # unit roundoff of float32
+
+
+def point_cloud64(frames, cam2world, world2rf, blend_rows, min_acc, max_norm, voxel_size, origin, min_count=1,
+                  slack=2.0):
+    """An independent float64 reference of localrf_b200.export.point_cloud from the rendered chunks.
+
+    frames: (view, rgb [m,3], depth [m], acc [m], dirs [m,3]) per chunk; cam2world [V,3,4] the views' camera-to-world
+    matrices (LocalTensorfs.get_cam2world()), used as o = c2w[:, 3], R = c2w[:, :3]; world2rf [F,3]; blend_rows [V,F].
+    A ray's point is o + (dirs @ R^T) depth / acc in float64; it is kept when acc >= min_acc, acc > 0, depth is finite
+    and max_a |p_a + world2rf_k_a| <= max_norm for a field with blend > 0, and lands in voxel floor((p - origin) /
+    voxel_size).  (voxel_size and origin are the float32 values the table holds.)
+
+    Each ray also gets a bound on the float32 pipeline's error in p (`slack` times the unit roundoff of each of its
+    operations); a ray is ambiguous when a decision lies within that bound of its boundary: acc against min_acc, |p_a +
+    world2rf_k_a| against max_norm, or q_a = (p_a - origin_a) / voxel_size against an integer.
+
+    -> dict(voxels {key: [count, sum p (3), sum clamp(rgb) (3), largest error bound of a float32 point's position in
+    its voxel: q_a's bound times voxel_size]} of the voxels with at least min_count points, ambiguous {(chunk index,
+    ray)}, ambiguous_keys {keys of the 27 voxels around each ambiguous ray}, kept, n_rays)."""
+    vs = float(f32(voxel_size))
+    org = np.array([float(f32(o)) for o in origin])
+    w2 = np.asarray(world2rf, np.float64).reshape(-1, 3)
+    voxels, ambiguous, amb_keys = {}, set(), set()
+    kept = n_rays = 0
+    for ci, (v, rgb, depth, acc, dirs) in enumerate(frames):
+        rgb, depth, acc, dirs = (np.asarray(a, np.float64) for a in (rgb, depth, acc, dirs))
+        M = np.asarray(cam2world[v], np.float64)
+        o, R = M[:, 3], M[:, :3]
+        n_rays += len(acc)
+        with np.errstate(all="ignore"):
+            s = depth / acc
+            c = dirs * s[:, None]
+            p = o + (dirs @ R.T) * s[:, None]
+            # float32: s, c (2 roundings), three products and three sums per axis, then q (two more)
+            err = slack * U32 * (2 * np.abs(c) @ np.abs(R).T * 3 + np.abs(o) + np.abs(p))
+            keep = (acc >= min_acc) & (acc > 0) & np.isfinite(depth)
+            amb = np.abs(acc - min_acc) <= slack * U32 * abs(min_acc)
+            inside = np.zeros(len(acc), bool)
+            for k in range(w2.shape[0]):
+                if not blend_rows[v][k] > 0:
+                    continue
+                d = np.abs(p + w2[k])
+                e = err + slack * U32 * (np.abs(w2[k]) + d)
+                inside |= np.all(d <= max_norm, axis=1)
+                amb |= np.any(np.abs(d - max_norm) <= e, axis=1)
+            keep &= inside
+            q = (p - org) / vs
+            eq = (err + slack * U32 * np.abs(p - org)) / vs + slack * U32 * np.abs(q)
+            kf = np.floor(q)
+            keep &= np.all((kf >= -KEY_LIM) & (kf < KEY_LIM), axis=1)
+            amb |= np.any(np.abs(q - np.round(q)) <= eq, axis=1)
+            cl = np.clip(np.nan_to_num(rgb, nan=0.0), 0.0, 1.0)
+        amb &= np.isfinite(p).all(1) & (acc > 0) & np.isfinite(depth)
+        for r in np.nonzero(amb)[0].tolist():
+            ambiguous.add((ci, r))
+            base = np.floor(q[r])
+            for dk in np.ndindex(3, 3, 3):
+                kk = base + np.array(dk) - 1
+                if np.all(np.abs(kk + 0.5) < KEY_LIM):
+                    amb_keys.add(int(pack_key(kk.astype(np.int64))))
+        idx = np.nonzero(keep)[0]
+        kept += len(idx)
+        keys = pack_key(kf[idx].astype(np.int64))
+        for r, key in zip(idx.tolist(), keys.tolist()):
+            cur = voxels.setdefault(key, [0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0])
+            cur[0] += 1
+            for a in range(3):
+                cur[1 + a] += p[r, a]
+                cur[4 + a] += cl[r, a]
+            cur[7] = max(cur[7], float(eq[r].max()) * vs)
+    voxels = {k: v for k, v in voxels.items() if v[0] >= min_count}
+    return dict(voxels=voxels, ambiguous=ambiguous, ambiguous_keys=amb_keys, kept=kept, n_rays=n_rays)
+
+
 def read_ply(data):
     """(xyz, rgb) of a binary little-endian PLY with one vertex element of float x, y, z, uchar red, green, blue."""
     end = data.index(b"end_header\n") + len(b"end_header\n")

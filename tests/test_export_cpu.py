@@ -203,3 +203,51 @@ def test_voxel_extract_invalid():
     _refused(call(_table(), s=None), b"scratch")
     _refused(call(_table(), s=FAKE + 16), b"256-byte aligned")
     assert L.lrf_voxel_extract_scratch_bytes(6) == 0 and L.lrf_voxel_extract_scratch_bytes(2 ** 31) == 0
+
+
+def test_point_cloud64_agrees_with_ray_points():
+    """The float64 reference on hand-built rays of a rotated, translated camera: the same rays kept and the same
+    voxels as the float32 restatement, with no ray near a boundary (so none is ambiguous)."""
+    rng = np.random.default_rng(5)
+    n = 400
+    a, b = 0.4, -0.7
+    Rx = np.array([[1, 0, 0], [0, np.cos(a), -np.sin(a)], [0, np.sin(a), np.cos(a)]])
+    Ry = np.array([[np.cos(b), 0, np.sin(b)], [0, 1, 0], [-np.sin(b), 0, np.cos(b)]])
+    c2w = np.concatenate([Rx @ Ry, [[0.1], [-0.2], [0.3]]], 1).astype(np.float32)
+    w2rf = np.array([[-0.1, 0.2, -0.3], [-5.0, 0.0, 0.0]], np.float32)
+    dirs = np.concatenate([rng.uniform(-0.6, 0.6, (n, 2)), -np.ones((n, 1))], 1).astype(np.float32)
+    depth = rng.uniform(0.1, 0.9, n).astype(np.float32)
+    acc = rng.uniform(0.0, 1.0, n).astype(np.float32)
+    rgb = rng.uniform(-0.2, 1.2, (n, 3)).astype(np.float32)
+    depth[:5] = np.nan
+    acc[5:10] = 0.0
+    blend = np.array([1.0, 0.0], np.float32)
+    args = (rgb, depth, acc, dirs)
+    vs, origin, min_acc, max_norm = 1 / 32, (0.0, 0.0, 0.0), 0.25, 0.8
+    keep, _, key, _, _ = eo.ray_points(*args, c2w, w2rf, blend, min_acc, max_norm, vs, origin)
+    ref = eo.point_cloud64([(0, *args)], c2w[None], w2rf, blend[None], min_acc, max_norm, vs, origin)
+    assert not ref["ambiguous"] and ref["n_rays"] == n
+    assert ref["kept"] == int(keep.sum()) > 100
+    want = {}
+    for k in key[keep].tolist():
+        want[k] = want.get(k, 0) + 1
+    assert {k: v[0] for k, v in ref["voxels"].items()} == want
+    # x = 0.75 (1 / 3) lies on the face x = 8 voxels in float64; float32's 1 / 3 may put it in voxel 7: ambiguous
+    near = eo.point_cloud64([(0, rgb[:1], np.ones(1, np.float32), np.full(1, 3.0, np.float32),
+                              np.array([[0.75, 0.9, -1.2]], np.float32))], EYE[None], [[0, 0, 0]], [[1.0]], 0.5, 1.0,
+                            vs, origin)
+    assert near["ambiguous"] == {(0, 0)}
+    assert {eo.pack_key([k, 9, -13]) for k in (7, 8)} <= near["ambiguous_keys"]
+
+
+def test_probe_table_wraps_at_the_last_slot():
+    cap = 64
+    cand = np.arange(1, 200000, dtype=np.uint64)
+    last = cand[(eo.mix64(cand) & np.uint64(cap - 1)) == cap - 1][:5]
+    assert len(last) == 5
+    assert eo.probe_table(last, cap) == {63, 0, 1, 2, 3}                  # 63, then wrapped to 0, 1, 2, 3
+    assert eo.probe_table(last[::-1], cap) == {63, 0, 1, 2, 3}
+    mid = cand[(eo.mix64(cand) & np.uint64(cap - 1)) == 1][:2]
+    assert eo.probe_table(np.concatenate([last, mid]), cap) == {63, 0, 1, 2, 3, 4, 5}
+    assert int(eo.mix64(np.uint64(0))) == 0 and int(eo.mix64(np.uint64(1))) == 0x5692161d100b05e5
+    assert eo.pack_key([-(1 << 20), 0, (1 << 20) - 1]) == (1 << 41) | (1 << 21) - 1

@@ -190,20 +190,25 @@ def test_repeatable_across_runs_orders_and_chunks(scene):
     a = point_cloud(scene, W, H, **kw)
     b = point_cloud(scene, W, H, **kw)
     c = point_cloud(scene, W, H, view_ids=[2, 0, 1], **kw)
-    S = max(int(rf.nSamples) for rf in scene.tensorfs)
+    S = max(rf.sample_table(False, -1, "cuda").numel() for rf in scene.tensorfs)       # the eval table's length
     d = point_cloud(scene, W, H, weights_budget=4 * S * 97, **kw)            # chunks of 97 rays
     assert a["n_kept"] > 100 and len(a["xyz"]) > 50
     assert _bytes(a) == _bytes(b) == _bytes(c) == _bytes(d)
     assert a["n_rays"] == 3 * W * H and a["n_kept"] == c["n_kept"] == d["n_kept"]
 
 
-def test_scene_renders_opacity_and_cloud(scene):
+def test_scene_renders_opacity_and_cloud_in_eval_table_chunks(scene):
+    """The weights budget is counted in eval-table samples (2 (nSamples // 6) per ray): 4 S 500 bytes renders every
+    view in chunks of exactly 500 rays."""
     lt = scene
     frames = []
     vs, origin, min_acc, max_norm = 1 / 128, (0.01, -0.02, 0.0), 0.05, 0.9
+    S = max(rf.sample_table(False, -1, "cuda").numel() for rf in lt.tensorfs)
+    assert S == max(2 * (int(rf.nSamples) // 6) for rf in lt.tensorfs)
     cloud = point_cloud(lt, W, H, test_ids=[1], voxel_size=vs, origin=origin, min_acc=min_acc, max_norm=max_norm,
-                        capacity=1 << 16, weights_budget=4 * 700 * 500, _frames=frames)
-    assert len({(v, lo) for v, lo, *_ in frames}) == len(frames) and len(frames) > 3
+                        capacity=1 << 16, weights_budget=4 * S * 500, _frames=frames)         # chunks of 500 rays
+    assert [(v, lo, f[0].shape[0]) for v, lo, *f in frames] == \
+        [(v, lo, min(500, W * H - lo)) for v in range(3) for lo in range(0, W * H, 500)]
     table = eo.new_table()
     w2rf = torch.stack([w.detach() for w in lt.world2rf]).cpu().numpy()
     bw = lt.blending_weights.detach().cpu().numpy()

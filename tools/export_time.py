@@ -51,7 +51,7 @@ def split_times(lt, W, H, views, voxel_size, capacity, min_acc):
     from localrf_b200.tensorf import _stream
     dev = torch.device("cuda")
     n = W * H
-    S = max(int(rf.nSamples) for rf in lt.tensorfs)
+    S = max(rf.sample_table(False, -1, dev).numel() for rf in lt.tensorfs)
     per_chunk = min((256 << 20) // (4 * S), n)
     store = torch.zeros(8 * capacity + 4, dtype=torch.int64, device=dev)
     t = _lib.LrfVoxelTable(capacity=capacity, voxel_size=voxel_size, keys=store.data_ptr(),
