@@ -154,7 +154,8 @@ int lrf_version(void);
 const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
  * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor, 7 LrfCameraGrads, 8 LrfFrameStore,
- * 9 LrfRayGather, 10 LrfPanelFrame, 11 LrfIngestFrame, 12 LrfPointFrame, 13 LrfVoxelTable (0 for any other index).  Bindings compare these with their own mirrors at load
+ * 9 LrfRayGather, 10 LrfPanelFrame, 11 LrfIngestFrame, 12 LrfPointFrame, 13 LrfVoxelTable, 14 LrfMeshScene,
+ * 15 LrfMeshTable (0 for any other index).  Bindings compare these with their own mirrors at load
  * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
@@ -669,6 +670,74 @@ size_t lrf_voxel_extract_scratch_bytes(int64_t capacity);
  * and scratch that is NULL, not 256-byte aligned or smaller than lrf_voxel_extract_scratch_bytes(capacity). */
 int lrf_voxel_extract(const LrfVoxelTable *table, int64_t min_count, float *xyz, uint8_t *rgb, int32_t *count,
                       int64_t *n_voxels, void *scratch, size_t scratch_bytes, lrf_stream_t stream);
+
+/* ---- mesh export: marching cubes over the fields' density on a world-space lattice, on the device -----------------
+ * Lattice point i = (ix, iy, iz) sits at p_a = origin_a + i_a voxel_size (fp32, round to nearest).  The scalar field at
+ * a world point p is A(p): the owner is the field k with the smallest max_a |p_a + world2rf_k_a| (fp32 adds; ties to
+ * the lowest k); A = 0 when that norm is above max_norm or no field has a finite one; else A is getDenseAlpha's value
+ * (1 - exp(-sigma stepSize), an alpha mask culling) of the owner at contract(p + world2rf_owner). */
+#define LRF_MESH_MAX_FIELDS 64
+
+typedef struct LrfMeshScene {
+  int32_t n_fields;            /* [1, LRF_MESH_MAX_FIELDS] */
+  const LrfField *fields;      /* host array [n_fields]: fp32 grids (LRF_GRID_F32); the MLP pointers are not read */
+  const float *step_size;      /* host array [n_fields]: each field's stepSize (getDenseAlpha's length) */
+  const float *world2rf;       /* device [n_fields][3] */
+  float voxel_size;            /* > 0, finite */
+  float origin[3];             /* finite */
+  float max_norm;              /* > 0, finite */
+  float level;                 /* > 0, finite: a lattice point is inside when A >= level (NaN is outside) */
+} LrfMeshScene;
+
+/* The cut edges (an open-addressing table keyed like LrfVoxelTable's) and the triangles of a mesh.  Zero keys and stats
+ * before the first brick.  The table holds at most capacity / 2 vertices and max_triangles triangles: stats[0] >
+ * capacity / 2 or stats[1] > max_triangles means it overflowed, and its content is then incomplete. */
+typedef struct LrfMeshTable {
+  int64_t capacity;            /* slots: a power of two in [2, 2^30] */
+  int64_t max_triangles;       /* [1, 2^31) */
+  unsigned long long *keys;    /* [capacity] edge key + 1, 0 = empty */
+  float *verts;                /* [capacity][3] the vertex of each claimed slot */
+  unsigned long long *tri_keys;/* [max_triangles] sort key of each triangle: cell key << 3 | index within its case */
+  int32_t *tri_slots;          /* [max_triangles][3] the slots of its three edges */
+  unsigned long long *stats;   /* [2] claimed slots (vertices), appended triangles */
+} LrfMeshTable;
+
+/* A at every point of one brick: values[(x dims_y + y) dims_z + z] = A(lattice point lo + (x, y, z)).  The brick's
+ * points must lie in [-2^19, 2^19) on every axis.  One launch, no atomics.  LRF_ERR_INVALID before any device work for
+ * a NULL scene, field array, step array, world2rf or values, n_fields outside [1, LRF_MESH_MAX_FIELDS], a field
+ * lrf_alpha_mask_build refuses or one with bf16 grid storage, a voxel_size, max_norm or level that is not > 0 and
+ * finite, an origin that is not finite, dims < 2 on some axis, a brick outside the key range, and more than 2^31
+ * points. */
+int lrf_mesh_lattice(const LrfMeshScene *scene, const int32_t lo[3], const int32_t dims[3], float *values,
+                     lrf_stream_t stream);
+/* Marching cubes over each cell of the brick lrf_mesh_lattice wrote (the same scene, lo and dims): a corner is inside
+ * when its value >= level.  Each cut edge is keyed (i_x + 2^19) << 42 | (i_y + 2^19) << 22 | (i_z + 2^19) << 2 | axis by
+ * its lower point i; the first cell to reach it claims its slot and stores the vertex: t = (level - v_lo) / (v_hi -
+ * v_lo) (fp32, round to nearest; 0 when not finite, clamped to [0, 1]) moves the lower point along the axis by t
+ * voxel_size (pa + t (pb - pa)).  Every cell computes the same bits for an edge.  Triangles of the 256-case table are
+ * appended with their three slots, wound counter-clockwise seen from outside (the right-hand normal points to lower
+ * A).  Bricks that share a face share its points, so consecutive bricks overlap by one point.  One launch, no host
+ * synchronisation.  LRF_ERR_INVALID as lrf_mesh_lattice, and for a NULL table or a table whose capacity or
+ * max_triangles is out of range or whose arrays are NULL or misaligned. */
+int lrf_mesh_cells(const LrfMeshScene *scene, const int32_t lo[3], const int32_t dims[3], const float *values,
+                   const LrfMeshTable *table, lrf_stream_t stream);
+/* Device scratch bytes of lrf_mesh_extract (256-byte aligned); 0 for sizes lrf_mesh_cells refuses or when the device
+ * cannot be queried. */
+size_t lrf_mesh_extract_scratch_bytes(int64_t capacity, int64_t max_triangles);
+/* The mesh in a canonical order: vertices in ascending edge-key order (rows [0, counts[0]) of xyz [capacity / 2][3]),
+ * triangles in ascending sort-key order as vertex indices (rows [0, counts[1]) of faces [max_triangles][3] int32).
+ * counts (device, [2]) receive the claimed slots and appended triangles; past either limit nothing is written beyond
+ * the buffers, and the caller must treat the mesh as incomplete.  The output is bitwise the same whatever the brick
+ * size, the brick order or the thread scheduling.  CUB radix sorts; no host synchronisation.  LRF_ERR_INVALID for a
+ * table lrf_mesh_cells refuses, NULL outputs, and scratch that is NULL, not 256-byte aligned or too small. */
+int lrf_mesh_extract(const LrfMeshTable *table, float *xyz, int32_t *faces, int64_t *counts, void *scratch,
+                     size_t scratch_bytes, lrf_stream_t stream);
+/* Per vertex: g_a = A(x + h e_a) - A(x - h e_a), h = voxel_size / 2 (fp32); normals = -g / |g| (outward), (0, 0, 0)
+ * when |g| is 0 or not finite; owner = the field of smallest max-norm at x (without the max_norm cut; -1 when none is
+ * finite).  xyz, normals [n][3] and owner [n] are device memory.  LRF_ERR_INVALID as lrf_mesh_lattice for the scene,
+ * n < 0 or at least 2^31, and NULL arrays with n > 0. */
+int lrf_mesh_normals(const LrfMeshScene *scene, const float *xyz, int64_t n, float *normals, int32_t *owner,
+                     lrf_stream_t stream);
 
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */

@@ -12,7 +12,7 @@ _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
            "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_panels.cu", "lrf_ingest.cu",
-           "lrf_export.cu", "lrf_abi.cu"]
+           "lrf_export.cu", "lrf_mesh.cu", "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", "lrf_launch.cuh", "lrf_launchers.cuh", "lrf_reproject.cuh",
            "lrf_select.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -108,6 +108,19 @@ class LrfVoxelTable(C.Structure):
                 ("sums", _vp), ("stats", _vp)]
 
 
+class LrfMeshScene(C.Structure):
+    _fields_ = [("n_fields", C.c_int32), ("fields", C.POINTER(LrfField)), ("step_size", _fp), ("world2rf", _vp),
+                ("voxel_size", C.c_float), ("origin", C.c_float * 3), ("max_norm", C.c_float), ("level", C.c_float)]
+
+
+class LrfMeshTable(C.Structure):
+    _fields_ = [("capacity", C.c_int64), ("max_triangles", C.c_int64), ("keys", _vp), ("verts", _vp),
+                ("tri_keys", _vp), ("tri_slots", _vp), ("stats", _vp)]
+
+
+MESH_MAX_FIELDS = 64
+
+
 class LrfBatch(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int64),
@@ -157,7 +170,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_exposure_clamp", "lrf_backward_batch_scratch_bytes", "lrf_render_backward_batch", "lrf_gather_rays",
            "lrf_test_panels_scratch_bytes", "lrf_test_panels", "lrf_ingest_scratch_bytes", "lrf_ingest_frame",
            "lrf_resize_linear", "lrf_ray_opacity", "lrf_frame_points", "lrf_voxel_extract_scratch_bytes",
-           "lrf_voxel_extract"]
+           "lrf_voxel_extract", "lrf_mesh_lattice", "lrf_mesh_cells", "lrf_mesh_extract_scratch_bytes",
+           "lrf_mesh_extract", "lrf_mesh_normals"]
 
 
 def _stale():
@@ -212,7 +226,7 @@ def lib():
     L.lrf_sizeof.argtypes = [C.c_int32]
     for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
                                      LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather, LrfPanelFrame,
-                                     LrfIngestFrame, LrfPointFrame, LrfVoxelTable)):
+                                     LrfIngestFrame, LrfPointFrame, LrfVoxelTable, LrfMeshScene, LrfMeshTable)):
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -276,6 +290,13 @@ def lib():
     L.lrf_voxel_extract_scratch_bytes.restype = C.c_size_t
     L.lrf_voxel_extract_scratch_bytes.argtypes = [C.c_int64]
     L.lrf_voxel_extract.argtypes = [C.POINTER(LrfVoxelTable), C.c_int64, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]
+    L.lrf_mesh_lattice.argtypes = [C.POINTER(LrfMeshScene), C.c_int32 * 3, C.c_int32 * 3, _vp, _vp]
+    L.lrf_mesh_cells.argtypes = [C.POINTER(LrfMeshScene), C.c_int32 * 3, C.c_int32 * 3, _vp, C.POINTER(LrfMeshTable),
+                                 _vp]
+    L.lrf_mesh_extract_scratch_bytes.restype = C.c_size_t
+    L.lrf_mesh_extract_scratch_bytes.argtypes = [C.c_int64, C.c_int64]
+    L.lrf_mesh_extract.argtypes = [C.POINTER(LrfMeshTable), _vp, _vp, _vp, _vp, C.c_size_t, _vp]
+    L.lrf_mesh_normals.argtypes = [C.POINTER(LrfMeshScene), _vp, C.c_int64, _vp, _vp, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

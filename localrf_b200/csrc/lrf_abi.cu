@@ -372,6 +372,65 @@ int check_voxel_table(const LrfVoxelTable* t) {
   return LRF_OK;
 }
 
+static_assert(LRF_MESH_MAX_FIELDS == lrf::MESH_MAX_FIELDS, "the header's field limit is the kernels'");
+
+bool positive_finite(float x) { return x > 0.0f && std::isfinite(x); }
+
+// the scene of the lrf_mesh_* entry points -> its device view
+int make_mesh_scene(const LrfMeshScene* s, lrf::MeshSceneDev& S) {
+  if (!s) return fail(LRF_ERR_INVALID, "scene is NULL");
+  if (s->n_fields < 1 || s->n_fields > LRF_MESH_MAX_FIELDS)
+    return fail(LRF_ERR_INVALID, "n_fields must be in [1, LRF_MESH_MAX_FIELDS]");
+  if (!s->fields || !s->step_size || !s->world2rf)
+    return fail(LRF_ERR_INVALID, "fields / step_size / world2rf of the scene is NULL");
+  if (!positive_finite(s->voxel_size)) return fail(LRF_ERR_INVALID, "voxel_size must be > 0 and finite");
+  if (!positive_finite(s->max_norm)) return fail(LRF_ERR_INVALID, "max_norm must be > 0 and finite");
+  if (!positive_finite(s->level)) return fail(LRF_ERR_INVALID, "level must be > 0 and finite");
+  if (!std::isfinite(s->origin[0]) || !std::isfinite(s->origin[1]) || !std::isfinite(s->origin[2]))
+    return fail(LRF_ERR_INVALID, "origin must be finite");
+  for (int k = 0; k < s->n_fields; ++k) {
+    const int rc = make_field(s->fields + k, false, false, nullptr, S.f[k]);
+    if (rc != LRF_OK) return rc;
+    if (!positive_finite(s->step_size[k])) return fail(LRF_ERR_INVALID, "step_size must be > 0 and finite");
+    S.length[k] = s->step_size[k];
+  }
+  S.w2rf = s->world2rf;
+  S.n_fields = s->n_fields;
+  S.voxel = s->voxel_size;
+  for (int a = 0; a < 3; ++a) S.origin[a] = s->origin[a];
+  S.max_norm = s->max_norm;
+  S.level = s->level;
+  return LRF_OK;
+}
+
+// a brick of lrf_mesh_lattice / lrf_mesh_cells: dims >= 2 points per axis, fewer than 2^31 points, every point's
+// index in [-2^19, 2^19)
+int check_brick(const int32_t lo[3], const int32_t dims[3]) {
+  if (!lo || !dims) return fail(LRF_ERR_INVALID, "lo / dims is NULL");
+  for (int a = 0; a < 3; ++a) {
+    if (dims[a] < 2) return fail(LRF_ERR_INVALID, "a brick needs dims >= 2 on every axis");
+    if (lo[a] < -(1 << 19) || (int64_t)lo[a] + dims[a] > (1 << 19))
+      return fail(LRF_ERR_INVALID, "the brick's lattice indices must lie in [-2^19, 2^19)");
+  }
+  if ((int64_t)dims[0] * dims[1] * dims[2] > 2147483647LL) return fail(LRF_ERR_INVALID, "a brick must hold < 2^31 points");
+  return LRF_OK;
+}
+
+// the edge and triangle table of lrf_mesh_cells and lrf_mesh_extract
+int check_mesh_table(const LrfMeshTable* t) {
+  if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
+  if (t->capacity < 2 || t->capacity > (1LL << 30) || (t->capacity & (t->capacity - 1)))
+    return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  if (t->max_triangles < 1 || t->max_triangles > 2147483647LL)
+    return fail(LRF_ERR_INVALID, "max_triangles must be in [1, 2^31)");
+  if (!t->keys || !t->verts || !t->tri_keys || !t->tri_slots || !t->stats)
+    return fail(LRF_ERR_INVALID, "keys / verts / tri_keys / tri_slots / stats of the table is NULL");
+  if ((((uintptr_t)t->keys | (uintptr_t)t->tri_keys | (uintptr_t)t->stats) & 7) ||
+      (((uintptr_t)t->verts | (uintptr_t)t->tri_slots) & 3))
+    return fail(LRF_ERR_INVALID, "the table's 64-bit arrays must be 8-byte and its 32-bit arrays 4-byte aligned");
+  return LRF_OK;
+}
+
 // the panel size of lrf_test_panels: two W x H panels index with 32-bit integers
 bool panel_size_ok(int32_t W, int32_t H) {
   return W >= 1 && H >= 1 && 2 * (int64_t)W * H <= 2147483647LL;
@@ -407,6 +466,8 @@ size_t lrf_sizeof(int32_t which) {
     case 11: return sizeof(LrfIngestFrame);
     case 12: return sizeof(LrfPointFrame);
     case 13: return sizeof(LrfVoxelTable);
+    case 14: return sizeof(LrfMeshScene);
+    case 15: return sizeof(LrfMeshTable);
     default: return 0;
   }
 }
@@ -870,6 +931,61 @@ int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uin
     return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_voxel_extract_scratch_bytes(capacity)");
   return cuda_status(lrf::launch_voxel_extract(*t, min_count, xyz, rgb, (int*)count, (long long*)n_voxels, scratch,
                                                (cudaStream_t)stream), "voxel_extract");
+}
+
+// (the scene's device view is ~17 KB: static storage per host thread rather than stack)
+int lrf_mesh_lattice(const LrfMeshScene* scene, const int32_t lo[3], const int32_t dims[3], float* values,
+                     lrf_stream_t stream) {
+  static thread_local lrf::MeshSceneDev S;
+  int rc = make_mesh_scene(scene, S);
+  if (rc != LRF_OK) return rc;
+  if ((rc = check_brick(lo, dims)) != LRF_OK) return rc;
+  if (!values) return fail(LRF_ERR_INVALID, "values is NULL");
+  return cuda_status(lrf::launch_mesh_lattice(S, lo, dims, values, (cudaStream_t)stream), "mesh_lattice_kernel");
+}
+
+int lrf_mesh_cells(const LrfMeshScene* scene, const int32_t lo[3], const int32_t dims[3], const float* values,
+                   const LrfMeshTable* table, lrf_stream_t stream) {
+  static thread_local lrf::MeshSceneDev S;
+  int rc = make_mesh_scene(scene, S);
+  if (rc != LRF_OK) return rc;
+  if ((rc = check_brick(lo, dims)) != LRF_OK) return rc;
+  if (!values) return fail(LRF_ERR_INVALID, "values is NULL");
+  if ((rc = check_mesh_table(table)) != LRF_OK) return rc;
+  return cuda_status(lrf::launch_mesh_cells(S, lo, dims, values, *table, (cudaStream_t)stream), "mesh_cells_kernel");
+}
+
+size_t lrf_mesh_extract_scratch_bytes(int64_t capacity, int64_t max_triangles) {
+  if (capacity < 2 || capacity > (1LL << 30) || (capacity & (capacity - 1))) return 0;
+  if (max_triangles < 1 || max_triangles > 2147483647LL) return 0;
+  size_t bytes = 0;
+  return lrf::mesh_extract_scratch_bytes(capacity, max_triangles, bytes) == cudaSuccess ? bytes : 0;
+}
+
+int lrf_mesh_extract(const LrfMeshTable* table, float* xyz, int32_t* faces, int64_t* counts, void* scratch,
+                     size_t scratch_bytes, lrf_stream_t stream) {
+  int rc = check_mesh_table(table);
+  if (rc != LRF_OK) return rc;
+  if (!xyz || !faces || !counts) return fail(LRF_ERR_INVALID, "xyz / faces / counts is NULL");
+  if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
+  size_t need = 0;
+  const cudaError_t e = lrf::mesh_extract_scratch_bytes(table->capacity, table->max_triangles, need);
+  if (e != cudaSuccess) return cuda_fail(e, "mesh_extract (sort size)");
+  if (scratch_bytes < need)
+    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_mesh_extract_scratch_bytes(capacity, max_triangles)");
+  return cuda_status(lrf::launch_mesh_extract(*table, xyz, (int*)faces, (long long*)counts, scratch,
+                                              (cudaStream_t)stream), "mesh_extract");
+}
+
+int lrf_mesh_normals(const LrfMeshScene* scene, const float* xyz, int64_t n, float* normals, int32_t* owner,
+                     lrf_stream_t stream) {
+  static thread_local lrf::MeshSceneDev S;
+  int rc = make_mesh_scene(scene, S);
+  if (rc != LRF_OK) return rc;
+  if (n < 0 || n > 2147483647LL) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
+  if (n > 0 && (!xyz || !normals || !owner)) return fail(LRF_ERR_INVALID, "xyz / normals / owner is NULL");
+  return cuda_status(lrf::launch_mesh_normals(S, xyz, n, normals, (int*)owner, (cudaStream_t)stream),
+                     "mesh_normals_kernel");
 }
 
 size_t lrf_test_panels_scratch_bytes(int32_t W, int32_t H) {

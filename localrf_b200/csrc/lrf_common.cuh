@@ -86,6 +86,16 @@ struct FieldDev {
   int grid16;                 // 1: the twelve plane / line pointers address bfloat16 texels (LrfField.grid_dtype)
 };
 
+// the mesh export's scene (LrfMeshScene): the fields' device views and stepSizes, the lattice and the owner rule
+constexpr int MESH_MAX_FIELDS = 64;
+struct MeshSceneDev {
+  FieldDev f[MESH_MAX_FIELDS];
+  float length[MESH_MAX_FIELDS];
+  const float* w2rf;          // device [n_fields][3]
+  int n_fields;
+  float voxel, origin[3], max_norm, level;
+};
+
 struct BatchDev {
   long long n_rays;
   const float* rays;

@@ -459,6 +459,19 @@ __device__ __forceinline__ void app_plane_features_t(const FieldDev& F, int i, c
   for (int c = 0; c < CA; c += 8) vm_products<8>(t, texels<H16>(F.aplane[i]), texels<H16>(F.aline[i]), c, out + c);
 }
 
+// ---- getDenseAlpha's value at one point (tensorBase.py:501-515 + compute_alpha, :538-558) ------------------
+// alpha = 1 - exp(-sigma length) at p in the field's (contracted) frame, read from the fp32 grids; an existing alpha
+// mask culls (sigma = 0) exactly as compute_alpha does.  The dense-alpha lattice and the mesh export share it.
+__device__ __forceinline__ float dense_alpha_at(const FieldDev& F, const float* p, float length) {
+  float q[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) q[a] = (p[a] - F.amin[a]) * F.ainv[a] - 1.0f;
+  float sigma = 0.0f;
+  if (!F.alpha_vol || alpha_mask(F, p) > 0.0f)
+    sigma = feature2density(density_feature_t<false>(F, q), F.density_shift, F.act);
+  return 1.0f - expf(-sigma * length);
+}
+
 // ---- one sample of the march (tensorBase.py:581-610) ---------------------------------------------
 // alpha of sample k < S of ray R; fe = its density feature and valid = whether it was looked up (not the
 // last sample, inside the alpha mask), fe = 0 where not

@@ -13,6 +13,7 @@ namespace lrf {
 
 struct FieldDev;
 struct BatchDev;
+struct MeshSceneDev;
 
 // lrf_render.cu
 int render_threads();
@@ -119,5 +120,16 @@ cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, 
 cudaError_t voxel_extract_scratch_bytes(long long cap, size_t& bytes);
 cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, float* xyz, unsigned char* rgb,
                                  int* count, long long* n_out, void* scratch, cudaStream_t stream);
+
+// lrf_mesh.cu
+cudaError_t launch_mesh_lattice(const MeshSceneDev& S, const int* lo, const int* dims, float* values,
+                                cudaStream_t stream);
+cudaError_t launch_mesh_cells(const MeshSceneDev& S, const int* lo, const int* dims, const float* values,
+                              const LrfMeshTable& t, cudaStream_t stream);
+cudaError_t mesh_extract_scratch_bytes(long long cap, long long max_tri, size_t& bytes);
+cudaError_t launch_mesh_extract(const LrfMeshTable& t, float* xyz, int* faces, long long* counts, void* scratch,
+                                cudaStream_t stream);
+cudaError_t launch_mesh_normals(const MeshSceneDev& S, const float* xyz, long long n, float* normals, int* owner,
+                                cudaStream_t stream);
 
 }  // namespace lrf

@@ -30,16 +30,10 @@ __global__ void dense_alpha_kernel(const FieldDev F, const float3 amax, int gx, 
     const int k = (int)(e % gz), j = (int)((e / gz) % gy), i = (int)(e / ((long long)gz * gy));
     const float t[3] = {linspace01(i, gx), linspace01(j, gy), linspace01(k, gz)};
     const float hi[3] = {amax.x, amax.y, amax.z};
-    float p[3], q[3];
+    float p[3];
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      p[a] = __fadd_rn(__fmul_rn(F.amin[a], __fsub_rn(1.0f, t[a])), __fmul_rn(hi[a], t[a]));
-      q[a] = (p[a] - F.amin[a]) * F.ainv[a] - 1.0f;
-    }
-    float sigma = 0.0f;
-    if (!F.alpha_vol || alpha_mask(F, p) > 0.0f)
-      sigma = feature2density(density_feature_t<false>(F, q), F.density_shift, F.act);
-    alpha[e] = 1.0f - expf(-sigma * length);
+    for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(__fmul_rn(F.amin[a], __fsub_rn(1.0f, t[a])), __fmul_rn(hi[a], t[a]));
+    alpha[e] = dense_alpha_at(F, p, length);
   }
 }
 

@@ -9,13 +9,22 @@ lrf_frame_points / lrf_voxel_extract): the cloud is bitwise repeatable whatever 
 
     cloud = point_cloud(local_tensorfs, W, H)
     write_ply("points.ply", cloud["xyz"], cloud["rgb"])
+
+The surface as a triangle mesh, in the same frame: marching cubes over the fields' density on a world-space lattice
+(include/localrf_b200.h, lrf_mesh_lattice / lrf_mesh_cells / lrf_mesh_extract / lrf_mesh_normals), each lattice point
+read from the field whose centre is nearest, so overlapping fields give one surface:
+
+    m = mesh(local_tensorfs)
+    write_ply("mesh.ply", m["xyz"], m["rgb"], faces=m["faces"], normals=m["normals"])
 """
 import ctypes as C
+import math
 
 import numpy as np
 import torch
 
 from . import _lib
+from .ray_utils import contract
 from .tensorf import _stream
 
 _TABLE_WORDS = 8          # per slot: the key, then count, sum f_x, f_y, f_z, sum r, g, b
@@ -110,23 +119,161 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
                 n_out_of_range=out_of_range)
 
 
-def write_ply(path, xyz, rgb):
-    """Writes a binary little-endian PLY with one `vertex` element: float x, y, z and uchar red, green, blue.  xyz
-    [P,3] and rgb [P,3] are numpy arrays or tensors (on any device)."""
+def _mesh_bricks(w2rf, voxel_size, origin, max_norm, brick):
+    """The bricks (lattice index of the lower corner, multiples of `brick` cells) whose cells meet some field's max_norm
+    cube, widened by one lattice step so that a surface cut by the cube's boundary closes outside it."""
+    out = set()
+    for w in w2rf:
+        lo, hi = [], []
+        for a in range(3):
+            lo.append(math.floor((-w[a] - max_norm - origin[a]) / voxel_size) - 1)
+            hi.append(math.ceil((-w[a] + max_norm - origin[a]) / voxel_size) + 1)
+        rng = [range(lo[a] // brick, (hi[a] - 1) // brick + 1) for a in range(3)]
+        out.update((bx * brick, by * brick, bz * brick) for bx in rng[0] for by in rng[1] for bz in rng[2])
+    return sorted(out)
+
+
+def mesh(local_tensorfs, voxel_size=1 / 128, level=0.005, origin=(0, 0, 0), max_norm=1.0, capacity=1 << 24,
+         max_triangles=1 << 25, _brick=64):
+    """The iso-surface A = `level` of the scene's density as a triangle mesh, in the world frame of get_cam2world().
+
+    A is sampled on the lattice origin + i voxel_size: at each point, the field whose centre is nearest (smallest
+    max-norm of p + world2rf_k, ties to the lowest k) gives getDenseAlpha's value (1 - exp(-sigma stepSize)) at its
+    contracted local position, and A = 0 beyond `max_norm` of every centre.  Marching cubes runs over the cells of the
+    bricks (`_brick` cells per axis, tests only) that meet some field's cube.  The table holds at most capacity / 2
+    vertices (`capacity` a power of two) and `max_triangles` triangles; a larger mesh raises RuntimeError naming the
+    parameter to raise.  The default level is the one TensoRF's mesh export passes with getDenseAlpha.
+
+    -> dict(xyz [V,3] float32, normals [V,3] float32 (outward: -grad A / |grad A|, central differences of half a
+    voxel; 0 where the gradient vanishes), rgb [V,3] uint8, faces [T,3] int32 (counter-clockwise seen from outside)),
+    CUDA tensors: vertices in ascending edge-key order, triangles in ascending cell order, the same bits whatever the
+    brick size.  Colours: each vertex's owner field's appearance at the vertex, shaded by its renderModule looking at
+    the surface head-on (viewdirs = -normal, (0, 0, -1) where the normal is 0), without exposure, floor(255 c + 0.5).
+    The only host reads are world2rf and the stepSizes at the start and the counts at the end."""
+    lt = local_tensorfs
+    dev = lt.blending_weights.device
+    if dev.type != "cuda":
+        raise RuntimeError("localrf_b200: the scene model is on the CPU; the export runs only on a CUDA device")
+    n_fields = len(lt.tensorfs)
+    if n_fields > _lib.MESH_MAX_FIELDS:
+        raise NotImplementedError(f"localrf_b200: the mesh export is built for at most {_lib.MESH_MAX_FIELDS} fields")
+    capacity, max_triangles, brick = int(capacity), int(max_triangles), int(_brick)
+    if capacity < 2 or capacity > 1 << 30 or capacity & (capacity - 1):
+        raise ValueError("capacity must be a power of two in [2, 2^30]")
+    if max_triangles < 1 or max_triangles >= 1 << 31:
+        raise ValueError("max_triangles must be in [1, 2^31)")
+    if brick < 1:
+        raise ValueError("_brick must be >= 1")
+    voxel_size, level, max_norm = float(voxel_size), float(level), float(max_norm)
+    origin = [float(v) for v in origin]
+    lib = _lib.lib()
+    w2rf = torch.stack([w.detach().to(dev, torch.float32).reshape(3) for w in lt.world2rf]).contiguous()
+    w_host = w2rf.tolist()
+    steps = (C.c_float * n_fields)(*[float(rf.stepSize) for rf in lt.tensorfs])
+    fields = (_lib.LrfField * n_fields)(*[rf._field() for rf in lt.tensorfs])
+    scene = _lib.LrfMeshScene(n_fields=n_fields, fields=fields, step_size=steps, world2rf=w2rf.data_ptr(),
+                              voxel_size=voxel_size, max_norm=max_norm, level=level)
+    scene.origin[:] = origin
+    bricks = _mesh_bricks(w_host, voxel_size, origin, max_norm, brick)
+    key_lim = 1 << 19
+    if bricks and (min(min(b) for b in bricks) < -key_lim or max(max(b) for b in bricks) + brick >= key_lim):
+        raise ValueError("the lattice indices exceed [-2^19, 2^19): raise `voxel_size` or move `origin`")
+
+    # one device block: table keys, vertices, triangle keys and slots, stats (2) and counts (2)
+    words = capacity + (3 * capacity + 1) // 2 + max_triangles + (3 * max_triangles + 1) // 2
+    store = torch.zeros(words + 4, dtype=torch.int64, device=dev)
+    base = store.data_ptr()
+    keys_at, verts_at = base, base + 8 * capacity
+    tri_keys_at = verts_at + 8 * ((3 * capacity + 1) // 2)
+    tri_slots_at = tri_keys_at + 8 * max_triangles
+    tail = store[words:]
+    table = _lib.LrfMeshTable(capacity=capacity, max_triangles=max_triangles, keys=keys_at, verts=verts_at,
+                              tri_keys=tri_keys_at, tri_slots=tri_slots_at, stats=tail.data_ptr())
+    values = torch.empty((brick + 1) ** 3, dtype=torch.float32, device=dev)
+    dims = (C.c_int32 * 3)(brick + 1, brick + 1, brick + 1)
+    with torch.no_grad(), torch.cuda.device(dev):
+        stream = _stream(dev)
+        for b in bricks:
+            lo = (C.c_int32 * 3)(*b)
+            _lib.check(lib.lrf_mesh_lattice(C.byref(scene), lo, dims, values.data_ptr(), stream))
+            _lib.check(lib.lrf_mesh_cells(C.byref(scene), lo, dims, values.data_ptr(), C.byref(table), stream))
+        scratch_bytes = lib.lrf_mesh_extract_scratch_bytes(capacity, max_triangles)
+        if scratch_bytes == 0:
+            raise RuntimeError("localrf_b200: the mesh extract's scratch size could not be determined")
+        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
+        xyz = torch.empty(capacity // 2, 3, dtype=torch.float32, device=dev)
+        faces = torch.empty(max_triangles, 3, dtype=torch.int32, device=dev)
+        _lib.check(lib.lrf_mesh_extract(C.byref(table), xyz.data_ptr(), faces.data_ptr(), tail.data_ptr() + 16,
+                                        scratch.data_ptr(), scratch_bytes, stream))
+        del scratch
+        n_vert, n_tri = tail[2:].tolist()
+        if n_vert > capacity // 2:
+            raise RuntimeError(f"localrf_b200: the mesh has more vertices than the table holds (capacity / 2 = "
+                               f"{capacity // 2}); raise `capacity` or `voxel_size`")
+        if n_tri > max_triangles:
+            raise RuntimeError(f"localrf_b200: the mesh has more than max_triangles = {max_triangles} triangles; "
+                               "raise `max_triangles` or `voxel_size`")
+        xyz, faces = xyz[:n_vert].clone(), faces[:n_tri].clone()
+        del store
+        normals = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
+        owner = torch.empty(n_vert, dtype=torch.int32, device=dev)
+        _lib.check(lib.lrf_mesh_normals(C.byref(scene), xyz.data_ptr(), n_vert, normals.data_ptr(),
+                                        owner.data_ptr(), stream))
+        rgb = _mesh_colours(lt, xyz, normals, owner, w2rf)
+    return dict(xyz=xyz, normals=normals, rgb=rgb, faces=faces)
+
+
+def _mesh_colours(lt, xyz, normals, owner, w2rf):
+    """Each vertex's colour from its owner field: compute_appfeature at the normalised, contracted vertex, then the
+    field's renderModule with viewdirs = -normal ((0, 0, -1) where the normal is 0) and refine = is_refining, as the
+    eval render shades; no exposure.  -> [V, 3] uint8."""
+    rgb = torch.zeros(xyz.shape[0], 3, dtype=torch.uint8, device=xyz.device)
+    view = -normals
+    view[(normals == 0).all(-1)] = torch.tensor([0.0, 0.0, -1.0], device=xyz.device)
+    for k, rf in enumerate(lt.tensorfs):
+        sel = (owner == k).nonzero().reshape(-1)
+        if sel.numel() == 0:
+            continue
+        x =rf.normalize_coord(contract(xyz[sel] + w2rf[k]))
+        c = rf.renderModule(None, view[sel], rf.compute_appfeature(x), bool(lt.is_refining))
+        rgb[sel] = torch.floor(255 * c + 0.5).clamp(0, 255).to(torch.uint8)
+    return rgb
+
+
+def write_ply(path, xyz, rgb, faces=None, normals=None):
+    """Writes a binary little-endian PLY with one `vertex` element: float x, y, z (then float nx, ny, nz when `normals`
+    is given) and uchar red, green, blue; with `faces` [T,3], a `face` element of `property list uchar int
+    vertex_indices`.  xyz [P,3], rgb [P,3], normals [P,3] and faces are numpy arrays or tensors (on any device)."""
     as_np = lambda a: a.detach().cpu().numpy() if torch.is_tensor(a) else np.asarray(a)
     xyz, rgb = as_np(xyz), as_np(rgb)
     if xyz.ndim != 2 or xyz.shape[1] != 3 or rgb.shape != xyz.shape:
         raise ValueError("xyz and rgb must both be [P, 3]")
-    rec = np.empty(xyz.shape[0], dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"),
-                                        ("blue", "u1")])
+    names = ["x", "y", "z"] + (["nx", "ny", "nz"] if normals is not None else [])
+    rec = np.empty(xyz.shape[0], dtype=[(n, "<f4") for n in names] + [("red", "u1"), ("green", "u1"), ("blue", "u1")])
     for i, name in enumerate(("x", "y", "z")):
         rec[name] = xyz[:, i]
+    if normals is not None:
+        normals = as_np(normals)
+        if normals.shape != xyz.shape:
+            raise ValueError("normals must be [P, 3]")
+        for i, name in enumerate(("nx", "ny", "nz")):
+            rec[name] = normals[:, i]
     for i, name in enumerate(("red", "green", "blue")):
         rec[name] = rgb[:, i]
     header = ("ply\nformat binary_little_endian 1.0\n"
               f"element vertex {xyz.shape[0]}\n"
-              "property float x\nproperty float y\nproperty float z\n"
-              "property uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n")
+              + "".join(f"property float {n}\n" for n in names) +
+              "property uchar red\nproperty uchar green\nproperty uchar blue\n")
+    body = rec.tobytes()
+    if faces is not None:
+        faces = as_np(faces)
+        if faces.ndim != 2 or faces.shape[1] != 3:
+            raise ValueError("faces must be [T, 3]")
+        frec = np.empty(faces.shape[0], dtype=[("n", "u1"), ("v", "<i4", (3,))])
+        frec["n"] = 3
+        frec["v"] = faces
+        header += f"element face {faces.shape[0]}\nproperty list uchar int vertex_indices\n"
+        body += frec.tobytes()
     with open(path, "wb") as fh:
-        fh.write(header.encode("ascii"))
-        fh.write(rec.tobytes())
+        fh.write((header + "end_header\n").encode("ascii"))
+        fh.write(body)
