@@ -12,9 +12,9 @@ _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
            "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_panels.cu", "lrf_ingest.cu",
-           "lrf_export.cu", "lrf_mesh.cu", "lrf_abi.cu"]
+           "lrf_table.cu", "lrf_export.cu", "lrf_mesh.cu", "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", "lrf_launch.cuh", "lrf_launchers.cuh", "lrf_reproject.cuh",
-           "lrf_select.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
+           "lrf_select.cuh", "lrf_table.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 

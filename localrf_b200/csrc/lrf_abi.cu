@@ -358,11 +358,27 @@ int check_loss_batch(const LrfLossBatch* b, const void* scratch, size_t scratch_
                        "scratch_bytes is smaller than lrf_supervision_scratch_bytes(n_rays, n_views, n_cams)");
 }
 
+// the capacity of an export's open-addressing table (lrf_table.cuh): a power of two in [2, 2^30]
+bool table_capacity_ok(int64_t capacity) {
+  return capacity >= 2 && capacity <= (1LL << 30) && !(capacity & (capacity - 1));
+}
+
+// the scratch block of lrf_voxel_extract and lrf_mesh_extract: non-NULL and 256-byte aligned, then (the sort-size query
+// needs a device, so after those checks) at least the bytes need(bytes) reports; `where` names a failed query
+template <typename Need>
+int check_extract_scratch(const void* scratch, size_t bytes, Need need, const char* where, const char* too_small) {
+  if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
+  size_t n = 0;
+  const cudaError_t e = need(n);
+  if (e != cudaSuccess) return cuda_fail(e, where);
+  if (bytes < n) return fail(LRF_ERR_INVALID, "%s", too_small);
+  return LRF_OK;
+}
+
 // the voxel table of lrf_frame_points and lrf_voxel_extract
 int check_voxel_table(const LrfVoxelTable* t) {
   if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
-  if (t->capacity < 2 || t->capacity > (1LL << 30) || (t->capacity & (t->capacity - 1)))
-    return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  if (!table_capacity_ok(t->capacity)) return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
   if (!(t->voxel_size > 0.0f) || !std::isfinite(t->voxel_size)) return fail(LRF_ERR_INVALID, "voxel_size must be > 0 and finite");
   if (!std::isfinite(t->origin[0]) || !std::isfinite(t->origin[1]) || !std::isfinite(t->origin[2]))
     return fail(LRF_ERR_INVALID, "origin must be finite");
@@ -419,8 +435,7 @@ int check_brick(const int32_t lo[3], const int32_t dims[3]) {
 // the edge and triangle table of lrf_mesh_cells and lrf_mesh_extract
 int check_mesh_table(const LrfMeshTable* t) {
   if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
-  if (t->capacity < 2 || t->capacity > (1LL << 30) || (t->capacity & (t->capacity - 1)))
-    return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  if (!table_capacity_ok(t->capacity)) return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
   if (t->max_triangles < 1 || t->max_triangles > 2147483647LL)
     return fail(LRF_ERR_INVALID, "max_triangles must be in [1, 2^31)");
   if (!t->keys || !t->verts || !t->tri_keys || !t->tri_slots || !t->stats)
@@ -912,7 +927,7 @@ int lrf_frame_points(const LrfPointFrame* f, const LrfVoxelTable* t, lrf_stream_
 }
 
 size_t lrf_voxel_extract_scratch_bytes(int64_t capacity) {
-  if (capacity < 2 || capacity > (1LL << 30) || (capacity & (capacity - 1))) return 0;
+  if (!table_capacity_ok(capacity)) return 0;
   size_t bytes = 0;
   return lrf::voxel_extract_scratch_bytes(capacity, bytes) == cudaSuccess ? bytes : 0;
 }
@@ -923,12 +938,11 @@ int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uin
   if (rc != LRF_OK) return rc;
   if (min_count < 1) return fail(LRF_ERR_INVALID, "min_count must be >= 1");
   if (!xyz || !rgb || !count || !n_voxels) return fail(LRF_ERR_INVALID, "xyz / rgb / count / n_voxels is NULL");
-  if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
-  size_t need = 0;
-  const cudaError_t e = lrf::voxel_extract_scratch_bytes(t->capacity, need);
-  if (e != cudaSuccess) return cuda_fail(e, "voxel_extract (sort size)");
-  if (scratch_bytes < need)
-    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_voxel_extract_scratch_bytes(capacity)");
+  rc = check_extract_scratch(scratch, scratch_bytes,
+                             [&](size_t& need) { return lrf::voxel_extract_scratch_bytes(t->capacity, need); },
+                             "voxel_extract (sort size)",
+                             "scratch_bytes is smaller than lrf_voxel_extract_scratch_bytes(capacity)");
+  if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_voxel_extract(*t, min_count, xyz, rgb, (int*)count, (long long*)n_voxels, scratch,
                                                (cudaStream_t)stream), "voxel_extract");
 }
@@ -956,7 +970,7 @@ int lrf_mesh_cells(const LrfMeshScene* scene, const int32_t lo[3], const int32_t
 }
 
 size_t lrf_mesh_extract_scratch_bytes(int64_t capacity, int64_t max_triangles) {
-  if (capacity < 2 || capacity > (1LL << 30) || (capacity & (capacity - 1))) return 0;
+  if (!table_capacity_ok(capacity)) return 0;
   if (max_triangles < 1 || max_triangles > 2147483647LL) return 0;
   size_t bytes = 0;
   return lrf::mesh_extract_scratch_bytes(capacity, max_triangles, bytes) == cudaSuccess ? bytes : 0;
@@ -967,12 +981,12 @@ int lrf_mesh_extract(const LrfMeshTable* table, float* xyz, int32_t* faces, int6
   int rc = check_mesh_table(table);
   if (rc != LRF_OK) return rc;
   if (!xyz || !faces || !counts) return fail(LRF_ERR_INVALID, "xyz / faces / counts is NULL");
-  if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
-  size_t need = 0;
-  const cudaError_t e = lrf::mesh_extract_scratch_bytes(table->capacity, table->max_triangles, need);
-  if (e != cudaSuccess) return cuda_fail(e, "mesh_extract (sort size)");
-  if (scratch_bytes < need)
-    return fail(LRF_ERR_INVALID, "scratch_bytes is smaller than lrf_mesh_extract_scratch_bytes(capacity, max_triangles)");
+  rc = check_extract_scratch(
+      scratch, scratch_bytes,
+      [&](size_t& need) { return lrf::mesh_extract_scratch_bytes(table->capacity, table->max_triangles, need); },
+      "mesh_extract (sort size)",
+      "scratch_bytes is smaller than lrf_mesh_extract_scratch_bytes(capacity, max_triangles)");
+  if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_mesh_extract(*table, xyz, (int*)faces, (long long*)counts, scratch,
                                               (cudaStream_t)stream), "mesh_extract");
 }

@@ -5,8 +5,8 @@
 // blended opacity.  lrf_frame_points back-projects each kept ray of one view and adds it to an open-addressing table
 // of 64-bit integer sums keyed by voxel; integer sums commute, so the table's content does not depend on thread
 // scheduling, on how the rays are chunked or on the order of the frames, and atomics are used freely.
-// lrf_voxel_extract sorts the occupied slots by key (CUB's radix sort) and writes one point per voxel: whatever the
-// slot layout, the output is bitwise repeatable.
+// lrf_voxel_extract sorts the occupied slots by key (KeySlotSort, a radix sort) and writes one point per voxel:
+// whatever the slot layout, the output is bitwise repeatable.  The table's conventions are lrf_table.cuh's.
 //
 // The back-projection and the key are written with explicit round-to-nearest fp32 operations in a fixed order (no
 // FMA contraction), so a numpy float32 restatement reproduces them bit for bit; the per-voxel means are fp64, rounded
@@ -14,11 +14,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <cub/device/device_radix_sort.cuh>
-
 #include "../../include/localrf_b200.h"
 #include "lrf_launch.cuh"
 #include "lrf_launchers.cuh"
+#include "lrf_table.cuh"
 
 namespace lrf {
 
@@ -30,7 +29,6 @@ constexpr int PT_THREADS = 256;
 constexpr int EX_THREADS = 256;
 constexpr int KEY_BITS = 21;           // per axis: keys in [-2^20, 2^20), 63 bits in all
 constexpr float KEY_LIM = 1048576.0f;  // 2^20
-constexpr unsigned long long NO_KEY = ~0ull;
 
 // One thread per ray sums its weights in sample order in fp64, from -0 (the identity of IEEE addition, so a row of -0
 // sums to -0 as np.cumsum does).  The [rays][S] rows are read a tile at a time, coalesced, into padded shared rows, so
@@ -60,24 +58,14 @@ __global__ void __launch_bounds__(OP_RAYS) ray_opacity_kernel(const float* __res
   acc[r] = accumulate ? __fadd_rn(acc[r], a) : a;
 }
 
-// splitmix64's finaliser: the probe start of a key
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
-  x ^= x >> 27; x *= 0x94d049bb133111ebull;
-  return x ^ (x >> 31);
-}
-
-__device__ __forceinline__ unsigned long long occupied(const LrfVoxelTable& t) {
-  return *reinterpret_cast<volatile unsigned long long*>(t.stats + 2);
-}
-
+// The table's claim counter is stats[2], the occupied slots.
 __global__ void __launch_bounds__(PT_THREADS) frame_points_kernel(const LrfPointFrame f, const LrfVoxelTable t) {
   const long long r = (long long)blockIdx.x * PT_THREADS + threadIdx.x;
   const unsigned long long half = (unsigned long long)t.capacity >> 1;
   bool keep = false, out = false;
   unsigned long long key = 0, fs[3];
   unsigned int cs[3];
-  if (r < f.n_rays && occupied(t) <= half) {
+  if (r < f.n_rays && claim_count(t.stats + 2) <= half) {
     const float a = f.acc[r], d = f.depth[r];
     if (a >= f.min_acc && a > 0.0f && isfinite(d)) {
       const float s = __fdiv_rn(d, a);
@@ -125,28 +113,14 @@ __global__ void __launch_bounds__(PT_THREADS) frame_points_kernel(const LrfPoint
     if (mo) atomicAdd(t.stats + 1, (unsigned long long)__popc(mo));
   }
   if (!keep) return;
-  const unsigned long long mask = (unsigned long long)t.capacity - 1, tag = key + 1;
-  unsigned long long slot = mix64(key) & mask;
-  for (long long probe = 0; probe < t.capacity; ++probe, slot = (slot + 1) & mask) {
-    unsigned long long cur = __ldcg(t.keys + slot);        // a slot, once claimed, never changes
-    if (cur == 0) {
-      cur = atomicCAS(t.keys + slot, 0ull, tag);
-      if (cur == 0) {
-        if (atomicAdd(t.stats + 2, 1ull) >= half) return;   // more than capacity / 2 voxels: overflow
-        cur = tag;
-      }
-    }
-    if (cur == tag) {
-      unsigned long long* v = t.sums + 7 * slot;
-      atomicAdd(v, 1ull);
+  find_or_claim(t.keys, t.capacity, t.stats + 2, key, [&](unsigned long long slot, bool) {
+    unsigned long long* v = t.sums + 7 * slot;
+    atomicAdd(v, 1ull);
 #pragma unroll
-      for (int i = 0; i < 3; ++i) atomicAdd(v + 1 + i, fs[i]);
+    for (int i = 0; i < 3; ++i) atomicAdd(v + 1 + i, fs[i]);
 #pragma unroll
-      for (int i = 0; i < 3; ++i) atomicAdd(v + 4 + i, (unsigned long long)cs[i]);
-      return;
-    }
-    if (occupied(t) > half) return;
-  }
+    for (int i = 0; i < 3; ++i) atomicAdd(v + 4 + i, (unsigned long long)cs[i]);
+  });
 }
 
 // sort input: the key of every slot holding at least min_count points, NO_KEY (sorted last) for the others
@@ -185,11 +159,10 @@ __global__ void __launch_bounds__(EX_THREADS) voxel_write_kernel(const LrfVoxelT
   count[i] = n < 2147483647ull ? (int)n : 2147483647;
 }
 
-// The extract's scratch: the keys and slot indices (two buffers each, for CUB's double-buffered sort), then CUB's own
-// temporary storage.  With a null base only the size is computed.
+// The extract's scratch: the sort's buffers of the slots' keys and indices, then the sort's temporary storage.  With a
+// null base only the size is computed.
 struct ExtractScratch {
-  cub::DoubleBuffer<unsigned long long> keys;
-  cub::DoubleBuffer<unsigned int> slots;
+  KeySlotSort pairs;
   void* temp;
   size_t temp_bytes;
   size_t total;
@@ -197,14 +170,8 @@ struct ExtractScratch {
 
 cudaError_t extract_scratch(void* base, long long cap, ExtractScratch& x) {
   ScratchCarver c(base);
-  unsigned long long* k0 = c.take<unsigned long long>(cap * 8, 256);
-  unsigned long long* k1 = c.take<unsigned long long>(cap * 8, 256);
-  unsigned int* s0 = c.take<unsigned int>(cap * 4, 256);
-  unsigned int* s1 = c.take<unsigned int>(cap * 4, 256);
-  x.keys = cub::DoubleBuffer<unsigned long long>(k0, k1);
-  x.slots = cub::DoubleBuffer<unsigned int>(s0, s1);
-  x.temp_bytes = 0;
-  const cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, x.temp_bytes, x.keys, x.slots, (int)cap, 0, 64);
+  x.pairs.carve(c, cap);
+  const cudaError_t e = KeySlotSort::temp_bytes(cap, x.temp_bytes);
   x.temp = c.take(x.temp_bytes, 256);
   x.total = c.size(256);
   return e;
@@ -240,13 +207,11 @@ cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, fl
   cudaError_t e = extract_scratch(scratch, t.capacity, x);
   if (e != cudaSuccess) return e;
   const unsigned blocks = (unsigned)((t.capacity + EX_THREADS - 1) / EX_THREADS);
-  voxel_keys_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, (unsigned long long)min_count, x.keys.Current(),
-                                                        x.slots.Current());
+  voxel_keys_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, (unsigned long long)min_count, x.pairs.keys(),
+                                                        x.pairs.slots());
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  e = cub::DeviceRadixSort::SortPairs(x.temp, x.temp_bytes, x.keys, x.slots, (int)t.capacity, 0, 64, stream);
-  if (e != cudaSuccess) return e;
-  voxel_write_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, x.keys.Current(), x.slots.Current(), xyz, rgb, count,
-                                                         n_out);
+  if ((e = x.pairs.sort(t.capacity, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  voxel_write_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, x.pairs.keys(), x.pairs.slots(), xyz, rgb, count, n_out);
   return cudaGetLastError();
 }
 

@@ -1,8 +1,9 @@
 // lrf_launchers.cuh -- the host functions one .cu file defines and another calls: the launchers, the sizes of their
-// scratch, prepared and shared-memory blocks, and the ingest's resize rule.  Each defining file includes this header,
-// so the compiler checks every definition against the declaration its callers use.
+// scratch, prepared and shared-memory blocks, the ingest's resize rule and the extracts' sort.  Each defining file
+// includes this header, so the compiler checks every definition against the declaration its callers use.
 //
-// Declarations only, no device code.
+// Declarations, and one small host-side struct (KeySlotSort: the sort's buffer pointers and their accessors); no
+// device code.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -14,6 +15,7 @@ namespace lrf {
 struct FieldDev;
 struct BatchDev;
 struct MeshSceneDev;
+struct ScratchCarver;
 
 // lrf_render.cu
 int render_threads();
@@ -112,6 +114,20 @@ int ingest_resize_mode(int ws, int hs, int w, int h);
 cudaError_t launch_ingest_frame(const LrfFrameStore& st, const LrfIngestFrame& f, void* scratch, cudaStream_t stream);
 cudaError_t launch_resize_linear(const float* src, int w0, int h0, long long src_stride, float* dst, int W, int H,
                                  long long dst_stride, cudaStream_t stream);
+
+// lrf_table.cu: the extracts' radix sort of n (64-bit key, 32-bit slot) pairs by key, the library's one use of CUB.
+// carve() takes two key and two slot buffers of n from a scratch block, in that order; the caller writes the pairs to
+// keys() / slots(), and after sort() they hold the sorted pairs.
+struct KeySlotSort {
+  unsigned long long* key_buf[2] = {};
+  unsigned int* slot_buf[2] = {};
+  int cur = 0;                                // the buffer of each pair that keys() / slots() return
+  unsigned long long* keys() const { return key_buf[cur]; }
+  unsigned int* slots() const { return slot_buf[cur]; }
+  void carve(ScratchCarver& c, long long n);
+  static cudaError_t temp_bytes(long long n, size_t& bytes);   // the sort's temporary storage for n pairs
+  cudaError_t sort(long long n, void* temp, size_t temp_bytes, cudaStream_t stream);
+};
 
 // lrf_export.cu
 cudaError_t launch_ray_opacity(const float* w, long long n, int S, long long n_views, const float* blend,

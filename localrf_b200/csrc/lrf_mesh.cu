@@ -5,20 +5,20 @@
 // brick of the lattice.  lrf_mesh_cells runs the 256-case table over the brick's cells: each cut edge is claimed once
 // in an open-addressing table keyed by its lower lattice point and axis, and stores its vertex; each triangle is
 // appended with the slots of its edges.  lrf_mesh_extract sorts the edges by key and the triangles by (cell, index in
-// the case) with CUB's radix sort, so the mesh comes out in one canonical order whatever the brick size, the brick
-// order or the thread scheduling.  lrf_mesh_normals takes the normals from central differences of A.
+// the case) with a radix sort, so the mesh comes out in one canonical order whatever the brick size, the brick
+// order or the thread scheduling.  lrf_mesh_normals takes the normals from central differences of A.  The edge
+// table's conventions are lrf_table.cuh's; the sort is KeySlotSort.
 //
 // The lattice points and vertices are written with explicit round-to-nearest fp32 operations (no FMA contraction), so
 // a numpy float32 restatement reproduces them bit for bit.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <cub/device/device_radix_sort.cuh>
-
 #include "../../include/localrf_b200.h"
 #include "lrf_device.cuh"
 #include "lrf_launch.cuh"
 #include "lrf_launchers.cuh"
+#include "lrf_table.cuh"
 
 namespace lrf {
 
@@ -26,7 +26,6 @@ namespace {
 
 constexpr int MC_THREADS = 256;
 constexpr int KEY_HALF = 1 << 19;       // lattice indices lie in [-2^19, 2^19): 20 bits per axis
-constexpr unsigned long long NO_KEY = ~0ull;
 
 // The widely published 256-case triangle table (three edges per triangle, -1 after the last).  Bit c of the case is
 // set when corner c is inside; corners 0-3 are (0,0,0), (1,0,0), (1,1,0), (0,1,0) and 4-7 the same at z = 1.  The
@@ -214,38 +213,6 @@ __global__ void __launch_bounds__(MC_THREADS) mesh_lattice_kernel(const __grid_c
   values[e] = mesh_value(S, p);
 }
 
-// splitmix64's finaliser: the probe start of a key
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
-  x ^= x >> 27; x *= 0x94d049bb133111ebull;
-  return x ^ (x >> 31);
-}
-
-__device__ __forceinline__ unsigned long long claimed(const LrfMeshTable& t) {
-  return *reinterpret_cast<volatile unsigned long long*>(t.stats);
-}
-
-// The slot of edge `key`; the caller that claims it stores v there.  -1 once the table holds more than capacity / 2.
-__device__ __forceinline__ int edge_slot(const LrfMeshTable& t, unsigned long long key, const float* v) {
-  const unsigned long long half = (unsigned long long)t.capacity >> 1, mask = (unsigned long long)t.capacity - 1;
-  const unsigned long long tag = key + 1;
-  unsigned long long slot = mix64(key) & mask;
-  for (long long probe = 0; probe < t.capacity; ++probe, slot = (slot + 1) & mask) {
-    unsigned long long cur = __ldcg(t.keys + slot);          // a slot, once claimed, never changes
-    if (cur == 0) {
-      cur = atomicCAS(t.keys + slot, 0ull, tag);
-      if (cur == 0) {
-        if (atomicAdd(t.stats, 1ull) >= half) return -1;   // more than capacity / 2 vertices: overflow
-        t.verts[3 * slot] = v[0]; t.verts[3 * slot + 1] = v[1]; t.verts[3 * slot + 2] = v[2];
-        return (int)slot;
-      }
-    }
-    if (cur == tag) return (int)slot;
-    if (claimed(t) > half) return -1;
-  }
-  return -1;
-}
-
 // slot[e] by selects, so the array stays in registers
 __device__ __forceinline__ int pick(const int (&slot)[12], int e) {
   int r = -1;
@@ -254,13 +221,14 @@ __device__ __forceinline__ int pick(const int (&slot)[12], int e) {
   return r;
 }
 
-// One thread per cell of the brick: its case, the vertices of its cut edges, its triangles.
+// One thread per cell of the brick: its case, the vertices of its cut edges, its triangles.  The edge table's claim
+// counter is stats[0]; the thread that claims an edge's slot stores its vertex there.
 __global__ void __launch_bounds__(MC_THREADS) mesh_cells_kernel(const __grid_constant__ MeshSceneDev S, int3 lo,
                                                                 int3 d, const float* __restrict__ values,
                                                                 const LrfMeshTable t) {
   const int nx = d.x - 1, ny = d.y - 1, nz = d.z - 1;
   const long long e = (long long)blockIdx.x * MC_THREADS + threadIdx.x;
-  if (e >= (long long)nx * ny * nz || claimed(t) > ((unsigned long long)t.capacity >> 1)) return;
+  if (e >= (long long)nx * ny * nz || claim_count(t.stats) > ((unsigned long long)t.capacity >> 1)) return;
   const int cz = (int)(e % nz), cy = (int)((e / nz) % ny), cx = (int)(e / ((long long)nz * ny));
   float v[8];
   int cube = 0;
@@ -286,7 +254,9 @@ __global__ void __launch_bounds__(MC_THREADS) mesh_cells_kernel(const __grid_con
       const unsigned long long key = ((unsigned long long)(i[0] + KEY_HALF) << 42) |
                                      ((unsigned long long)(i[1] + KEY_HALF) << 22) |
                                      ((unsigned long long)(i[2] + KEY_HALF) << 2) | (unsigned long long)axis;
-      slot[ed] = edge_slot(t, key, p);
+      slot[ed] = find_or_claim(t.keys, t.capacity, t.stats, key, [&](unsigned long long s, bool claimed) {
+        if (claimed) { t.verts[3 * s] = p[0]; t.verts[3 * s + 1] = p[1]; t.verts[3 * s + 2] = p[2]; }
+      });
     }
   }
   const unsigned long long ck = ((unsigned long long)(g[0] + KEY_HALF) << 40) |
@@ -371,12 +341,11 @@ __global__ void __launch_bounds__(MC_THREADS) mesh_normals_kernel(const __grid_c
   owner[i] = mesh_owner(S, x, y, norm);
 }
 
-// The extract's scratch: the edge keys and slots, the vertex rank of each slot, the triangle keys and ids (two buffers
-// of each sorted array, for CUB's double-buffered sort), then CUB's temporary storage for the larger of the two sorts.
-// With a null base only the size is computed.
+// The extract's scratch: the sort's buffers of the edge keys and slots, the vertex rank of each slot, the sort's
+// buffers of the triangle keys and ids, then the sorts' temporary storage, for the larger of the two.  With a null base
+// only the size is computed.
 struct MeshScratch {
-  cub::DoubleBuffer<unsigned long long> ekeys, tkeys;
-  cub::DoubleBuffer<unsigned int> slots, ids;
+  KeySlotSort edges, tris;
   int* rank;
   void* temp;
   size_t temp_bytes;
@@ -385,22 +354,12 @@ struct MeshScratch {
 
 cudaError_t mesh_scratch(void* base, long long cap, long long max_tri, MeshScratch& x) {
   ScratchCarver c(base);
-  unsigned long long* e0 = c.take<unsigned long long>(cap * 8, 256);
-  unsigned long long* e1 = c.take<unsigned long long>(cap * 8, 256);
-  unsigned int* s0 = c.take<unsigned int>(cap * 4, 256);
-  unsigned int* s1 = c.take<unsigned int>(cap * 4, 256);
+  x.edges.carve(c, cap);
   x.rank = c.take<int>(cap * 4, 256);
-  unsigned long long* t0 = c.take<unsigned long long>(max_tri * 8, 256);
-  unsigned long long* t1 = c.take<unsigned long long>(max_tri * 8, 256);
-  unsigned int* i0 = c.take<unsigned int>(max_tri * 4, 256);
-  unsigned int* i1 = c.take<unsigned int>(max_tri * 4, 256);
-  x.ekeys = cub::DoubleBuffer<unsigned long long>(e0, e1);
-  x.slots = cub::DoubleBuffer<unsigned int>(s0, s1);
-  x.tkeys = cub::DoubleBuffer<unsigned long long>(t0, t1);
-  x.ids = cub::DoubleBuffer<unsigned int>(i0, i1);
+  x.tris.carve(c, max_tri);
   size_t a = 0, b = 0;
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, a, x.ekeys, x.slots, (int)cap, 0, 64);
-  if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, b, x.tkeys, x.ids, (int)max_tri, 0, 64);
+  cudaError_t e = KeySlotSort::temp_bytes(cap, a);
+  if (e == cudaSuccess) e = KeySlotSort::temp_bytes(max_tri, b);
   x.temp_bytes = a > b ? a : b;
   x.temp = c.take(x.temp_bytes, 256);
   x.total = c.size(256);
@@ -437,19 +396,17 @@ cudaError_t launch_mesh_extract(const LrfMeshTable& t, float* xyz, int* faces, l
   MeshScratch x;
   cudaError_t e = mesh_scratch(scratch, t.capacity, t.max_triangles, x);
   if (e != cudaSuccess) return e;
-  edge_keys_kernel<<<blocks_of(t.capacity), MC_THREADS, 0, stream>>>(t, x.ekeys.Current(), x.slots.Current());
+  edge_keys_kernel<<<blocks_of(t.capacity), MC_THREADS, 0, stream>>>(t, x.edges.keys(), x.edges.slots());
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  e = cub::DeviceRadixSort::SortPairs(x.temp, x.temp_bytes, x.ekeys, x.slots, (int)t.capacity, 0, 64, stream);
-  if (e != cudaSuccess) return e;
-  vertex_write_kernel<<<blocks_of(t.capacity), MC_THREADS, 0, stream>>>(t, x.ekeys.Current(), x.slots.Current(), xyz,
+  if ((e = x.edges.sort(t.capacity, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  vertex_write_kernel<<<blocks_of(t.capacity), MC_THREADS, 0, stream>>>(t, x.edges.keys(), x.edges.slots(), xyz,
                                                                         x.rank, counts);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  tri_keys_kernel<<<blocks_of(t.max_triangles), MC_THREADS, 0, stream>>>(t, x.tkeys.Current(), x.ids.Current());
+  tri_keys_kernel<<<blocks_of(t.max_triangles), MC_THREADS, 0, stream>>>(t, x.tris.keys(), x.tris.slots());
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  e = cub::DeviceRadixSort::SortPairs(x.temp, x.temp_bytes, x.tkeys, x.ids, (int)t.max_triangles, 0, 64, stream);
-  if (e != cudaSuccess) return e;
-  face_write_kernel<<<blocks_of(t.max_triangles), MC_THREADS, 0, stream>>>(t, x.tkeys.Current(), x.ids.Current(),
-                                                                           x.rank, faces, counts);
+  if ((e = x.tris.sort(t.max_triangles, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  face_write_kernel<<<blocks_of(t.max_triangles), MC_THREADS, 0, stream>>>(t, x.tris.keys(), x.tris.slots(), x.rank,
+                                                                           faces, counts);
   return cudaGetLastError();
 }
 

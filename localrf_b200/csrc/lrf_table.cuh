@@ -1,0 +1,57 @@
+// lrf_table.cuh -- the open-addressing table of the geometry exports (LrfVoxelTable of lrf_export.cu, LrfMeshTable of
+// lrf_mesh.cu), keyed by 64-bit integers below ~0.
+//
+// Slot i of `keys` holds tag = key + 1, 0 while empty; a slot, once claimed by CAS, never changes.  A key's probe
+// starts at probe_start(key) & (capacity - 1) and steps by one slot, wrapping from the last to 0.  A claim counter
+// counts the claims, and the table holds at most capacity / 2 keys: the claim that finds the counter there or above
+// is an overflow, as is every probe that starts or continues once it is past.  The extracts sort the tables by key,
+// with NO_KEY (sorted last) for the slots they leave out (lrf_launchers.cuh, KeySlotSort).
+#pragma once
+#include <cuda_runtime.h>
+
+namespace lrf {
+
+constexpr unsigned long long NO_KEY = ~0ull;
+
+// splitmix64's finaliser: the probe start of a key
+__device__ __forceinline__ unsigned long long probe_start(unsigned long long x) {
+  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27; x *= 0x94d049bb133111ebull;
+  return x ^ (x >> 31);
+}
+
+// the claims so far (a volatile read: other threads add to the counter while the table fills)
+__device__ __forceinline__ unsigned long long claim_count(const unsigned long long* counter) {
+  return *reinterpret_cast<const volatile unsigned long long*>(counter);
+}
+
+// The slot of `key` (capacity is at most 2^30), claimed when no slot holds it yet -> -1 once the table has
+// overflowed.  Before it returns a slot it calls on_slot(slot, claimed), claimed when this call made the claim.  The
+// caller's work at the slot sits in the probe loop that way, where the compiler keeps it on the claim and find paths
+// without a join.
+template <typename OnSlot>
+__device__ __forceinline__ int find_or_claim(unsigned long long* keys, long long capacity, unsigned long long* counter,
+                                             unsigned long long key, OnSlot on_slot) {
+  const unsigned long long half = (unsigned long long)capacity >> 1, mask = (unsigned long long)capacity - 1;
+  const unsigned long long tag = key + 1;
+  unsigned long long slot = probe_start(key) & mask;
+  for (long long probe = 0; probe < capacity; ++probe, slot = (slot + 1) & mask) {
+    unsigned long long cur = __ldcg(keys + slot);
+    if (cur == 0) {
+      cur = atomicCAS(keys + slot, 0ull, tag);
+      if (cur == 0) {
+        if (atomicAdd(counter, 1ull) >= half) return -1;   // more than capacity / 2 keys: overflow
+        on_slot(slot, true);
+        return (int)slot;
+      }
+    }
+    if (cur == tag) {
+      on_slot(slot, false);
+      return (int)slot;
+    }
+    if (claim_count(counter) > half) return -1;
+  }
+  return -1;
+}
+
+}  // namespace lrf

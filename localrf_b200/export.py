@@ -30,6 +30,53 @@ from .tensorf import _stream
 _TABLE_WORDS = 8          # per slot: the key, then count, sum f_x, f_y, f_z, sum r, g, b
 
 
+def _cuda_device(local_tensorfs):
+    dev = local_tensorfs.blending_weights.device
+    if dev.type != "cuda":
+        raise RuntimeError("localrf_b200: the scene model is on the CPU; the export runs only on a CUDA device")
+    return dev
+
+
+def _table_capacity(capacity):
+    """`capacity` of an export's open-addressing table (csrc/lrf_table.cuh): a power of two in [2, 2^30]."""
+    capacity = int(capacity)
+    if capacity < 2 or capacity > 1 << 30 or capacity & (capacity - 1):
+        raise ValueError("capacity must be a power of two in [2, 2^30]")
+    return capacity
+
+
+def _extract_scratch(nbytes, what, dev):
+    """The scratch block of an extract, `nbytes` from its *_extract_scratch_bytes (0: the size query failed)."""
+    if nbytes == 0:
+        raise RuntimeError(f"localrf_b200: the {what}'s scratch size could not be determined")
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev)
+
+
+def _voxel_table(capacity, voxel_size, origin, dev):
+    """A zeroed LrfVoxelTable in one int64 device block: keys [capacity], sums [capacity][7], stats [4] (kept,
+    out of range, occupied, and the voxel count lrf_voxel_extract writes) -> (struct, block)."""
+    store = torch.zeros(_TABLE_WORDS * capacity + 4, dtype=torch.int64, device=dev)
+    table = _lib.LrfVoxelTable(capacity=capacity, voxel_size=float(voxel_size), keys=store.data_ptr(),
+                               sums=store.data_ptr() + 8 * capacity, stats=store.data_ptr() + 8 * _TABLE_WORDS * capacity)
+    table.origin[:] = [float(v) for v in origin]
+    return table, store
+
+
+def _mesh_table(capacity, max_triangles, dev):
+    """A zeroed LrfMeshTable in one int64 device block: edge keys [capacity], vertices [capacity][3] float32,
+    triangle keys [max_triangles], triangle slots [max_triangles][3] int32, stats [2], then two words for the counts
+    lrf_mesh_extract writes -> (struct, block)."""
+    words = capacity + (3 * capacity + 1) // 2 + max_triangles + (3 * max_triangles + 1) // 2
+    store = torch.zeros(words + 4, dtype=torch.int64, device=dev)
+    base = store.data_ptr()
+    keys_at, verts_at = base, base + 8 * capacity
+    tri_keys_at = verts_at + 8 * ((3 * capacity + 1) // 2)
+    tri_slots_at = tri_keys_at + 8 * max_triangles
+    table = _lib.LrfMeshTable(capacity=capacity, max_triangles=max_triangles, keys=keys_at, verts=verts_at,
+                              tri_keys=tri_keys_at, tri_slots=tri_slots_at, stats=base + 8 * words)
+    return table, store
+
+
 def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 / 256, origin=(0, 0, 0), min_acc=0.5,
                 max_norm=1.0, min_count=1, capacity=1 << 24, weights_budget=256 << 20, _frames=None):
     """Renders every view of `view_ids` (default: every frame of r_c2w, each with its own pose and blending row) at
@@ -50,9 +97,7 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
 
     `_frames`, when a list, receives (view, first ray, rgb, depth, acc, directions) of every chunk (tests)."""
     lt = local_tensorfs
-    dev = lt.blending_weights.device
-    if dev.type != "cuda":
-        raise RuntimeError("localrf_b200: the scene model is on the CPU; the export runs only on a CUDA device")
+    dev = _cuda_device(lt)
     views = list(range(len(lt.r_c2w))) if view_ids is None else [int(v) for v in view_ids]
     tests = {int(v) for v in test_ids}
     if not tests <= set(views):
@@ -66,16 +111,11 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
         raise ValueError(f"weights_budget must hold one ray's weights ({4 * S} bytes)")
     n = W * H
     per_chunk = min(per_chunk, n)
-    capacity = int(capacity)
-    if capacity < 2 or capacity > 1 << 30 or capacity & (capacity - 1):
-        raise ValueError("capacity must be a power of two in [2, 2^30]")
+    capacity = _table_capacity(capacity)
     lib = _lib.lib()
 
-    store = torch.zeros(_TABLE_WORDS * capacity + 4, dtype=torch.int64, device=dev)
-    table = _lib.LrfVoxelTable(capacity=capacity, voxel_size=float(voxel_size), keys=store.data_ptr(),
-                               sums=store.data_ptr() + 8 * capacity, stats=store.data_ptr() + 8 * _TABLE_WORDS * capacity)
-    table.origin[:] = [float(v) for v in origin]
-    stats = store[_TABLE_WORDS * capacity:]
+    table, store = _voxel_table(capacity, voxel_size, origin, dev)
+    stats = store[-4:]
     n_fields = len(lt.tensorfs)
     w2rf = torch.stack([w.detach().to(dev, torch.float32) for w in lt.world2rf]).contiguous()
     blend_rows = lt.blending_weights.detach().to(dev, torch.float32).contiguous()
@@ -102,9 +142,7 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
                 if _frames is not None:
                     _frames.append((v, lo, rgb, depth, acc, dirs))
         scratch_bytes = lib.lrf_voxel_extract_scratch_bytes(capacity)
-        if scratch_bytes == 0:
-            raise RuntimeError("localrf_b200: the voxel extract's scratch size could not be determined")
-        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
+        scratch = _extract_scratch(scratch_bytes, "voxel extract", dev)
         xyz = torch.empty(capacity, 3, dtype=torch.float32, device=dev)
         rgb8 = torch.empty(capacity, 3, dtype=torch.uint8, device=dev)
         count = torch.empty(capacity, dtype=torch.int32, device=dev)
@@ -151,15 +189,11 @@ def mesh(local_tensorfs, voxel_size=1 / 128, level=0.005, origin=(0, 0, 0), max_
     the surface head-on (viewdirs = -normal, (0, 0, -1) where the normal is 0), without exposure, floor(255 c + 0.5).
     The only host reads are world2rf and the stepSizes at the start and the counts at the end."""
     lt = local_tensorfs
-    dev = lt.blending_weights.device
-    if dev.type != "cuda":
-        raise RuntimeError("localrf_b200: the scene model is on the CPU; the export runs only on a CUDA device")
+    dev = _cuda_device(lt)
     n_fields = len(lt.tensorfs)
     if n_fields > _lib.MESH_MAX_FIELDS:
         raise NotImplementedError(f"localrf_b200: the mesh export is built for at most {_lib.MESH_MAX_FIELDS} fields")
-    capacity, max_triangles, brick = int(capacity), int(max_triangles), int(_brick)
-    if capacity < 2 or capacity > 1 << 30 or capacity & (capacity - 1):
-        raise ValueError("capacity must be a power of two in [2, 2^30]")
+    capacity, max_triangles, brick = _table_capacity(capacity), int(max_triangles), int(_brick)
     if max_triangles < 1 or max_triangles >= 1 << 31:
         raise ValueError("max_triangles must be in [1, 2^31)")
     if brick < 1:
@@ -179,16 +213,8 @@ def mesh(local_tensorfs, voxel_size=1 / 128, level=0.005, origin=(0, 0, 0), max_
     if bricks and (min(min(b) for b in bricks) < -key_lim or max(max(b) for b in bricks) + brick >= key_lim):
         raise ValueError("the lattice indices exceed [-2^19, 2^19): raise `voxel_size` or move `origin`")
 
-    # one device block: table keys, vertices, triangle keys and slots, stats (2) and counts (2)
-    words = capacity + (3 * capacity + 1) // 2 + max_triangles + (3 * max_triangles + 1) // 2
-    store = torch.zeros(words + 4, dtype=torch.int64, device=dev)
-    base = store.data_ptr()
-    keys_at, verts_at = base, base + 8 * capacity
-    tri_keys_at = verts_at + 8 * ((3 * capacity + 1) // 2)
-    tri_slots_at = tri_keys_at + 8 * max_triangles
-    tail = store[words:]
-    table = _lib.LrfMeshTable(capacity=capacity, max_triangles=max_triangles, keys=keys_at, verts=verts_at,
-                              tri_keys=tri_keys_at, tri_slots=tri_slots_at, stats=tail.data_ptr())
+    table, store = _mesh_table(capacity, max_triangles, dev)
+    tail = store[-4:]                                             # stats (2) and counts (2)
     values = torch.empty((brick + 1) ** 3, dtype=torch.float32, device=dev)
     dims = (C.c_int32 * 3)(brick + 1, brick + 1, brick + 1)
     with torch.no_grad(), torch.cuda.device(dev):
@@ -198,9 +224,7 @@ def mesh(local_tensorfs, voxel_size=1 / 128, level=0.005, origin=(0, 0, 0), max_
             _lib.check(lib.lrf_mesh_lattice(C.byref(scene), lo, dims, values.data_ptr(), stream))
             _lib.check(lib.lrf_mesh_cells(C.byref(scene), lo, dims, values.data_ptr(), C.byref(table), stream))
         scratch_bytes = lib.lrf_mesh_extract_scratch_bytes(capacity, max_triangles)
-        if scratch_bytes == 0:
-            raise RuntimeError("localrf_b200: the mesh extract's scratch size could not be determined")
-        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
+        scratch = _extract_scratch(scratch_bytes, "mesh extract", dev)
         xyz = torch.empty(capacity // 2, 3, dtype=torch.float32, device=dev)
         faces = torch.empty(max_triangles, 3, dtype=torch.int32, device=dev)
         _lib.check(lib.lrf_mesh_extract(C.byref(table), xyz.data_ptr(), faces.data_ptr(), tail.data_ptr() + 16,

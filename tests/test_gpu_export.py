@@ -14,20 +14,12 @@ import torch
 import export_oracle as eo
 import localrf_b200 as L
 from localrf_b200 import _lib
-from localrf_b200.export import point_cloud
+from localrf_b200.export import _voxel_table, point_cloud
 
 pytestmark = pytest.mark.gpu
 
 PAD = 64
 CANARY_F = -12345.5
-
-
-def _table(cap, voxel_size, origin):
-    store = torch.zeros(8 * cap + 4, dtype=torch.int64, device="cuda")
-    t = _lib.LrfVoxelTable(capacity=cap, voxel_size=voxel_size, keys=store.data_ptr(), sums=store.data_ptr() + 8 * cap,
-                           stats=store.data_ptr() + 64 * cap)
-    t.origin[:] = list(origin)
-    return t, store
 
 
 def _padded(n, cols, dtype, fill):
@@ -136,7 +128,7 @@ CASES = {   # (rays per frame, frames, fields, voxel_size, origin, max_norm, cap
 @pytest.mark.parametrize("case", list(CASES))
 def test_frame_points_and_extract_vs_oracle(case):
     n, frames, F, vs, origin, max_norm, cap, mc = CASES[case]
-    t, store = _table(cap, vs, origin)
+    t, store = _voxel_table(cap, vs, origin, "cuda")
     table = eo.new_table()
     for fr in range(frames):
         rgb, depth, acc, dirs, c2w, w2rf, blend = _random_rays(n, 10 * fr + F, F)

@@ -16,8 +16,8 @@ import torch
 import export_oracle as eo
 import localrf_b200 as L
 from localrf_b200 import _lib
-from localrf_b200.export import point_cloud
-from test_gpu_export import CANARY_F, PAD, _extract, _frame_points, _padded, _rot, _table
+from localrf_b200.export import _voxel_table, point_cloud
+from test_gpu_export import CANARY_F, PAD, _extract, _frame_points, _padded, _rot
 
 pytestmark = pytest.mark.gpu
 
@@ -133,7 +133,7 @@ def _on_device(rgb, depth, acc, dirs, c2w=EYE, w2rf=((0, 0, 0),), blend=None, mi
     args = [np.ascontiguousarray(a, np.float32) for a in (rgb, depth, acc, dirs, c2w)]
     w2 = np.asarray(w2rf, np.float32).reshape(-1, 3)
     bl = None if blend is None else np.asarray(blend, np.float32)
-    t, store = _table(cap, vs, origin)
+    t, store = _voxel_table(cap, vs, origin, "cuda")
     _frame_points(t, *args, w2, bl, min_acc, max_norm)
     table = eo.new_table()
     eo.frame_points(table, *args, w2, bl, min_acc, max_norm, vs, origin)
@@ -288,7 +288,7 @@ def test_exactly_half_and_one_past(cap):
     p = _centres(k, vs)
     rgb = _rgb(half + 1, cap)
     for m in (half, half + 1):
-        t, store = _table(cap, vs, (0, 0, 0))
+        t, store = _voxel_table(cap, vs, (0, 0, 0), "cuda")
         _frame_points(t, rgb[:m], np.ones(m, np.float32), np.ones(m, np.float32), p[:m], EYE,
                       np.zeros((1, 3), np.float32), None, 0.5, np.inf)
         xyz, rgb8, count, stats = _extract(t, store, 1)
@@ -310,7 +310,7 @@ def test_overflow_in_a_later_frame():
     half = cap // 2
     k = _distinct_voxels(half + 1, 5)
     p, rgb = _centres(k, vs), _rgb(half + 1, 5)
-    t, store = _table(cap, vs, (0, 0, 0))
+    t, store = _voxel_table(cap, vs, (0, 0, 0), "cuda")
     one = lambda a, b: _frame_points(t, rgb[a:b], np.ones(b - a, np.float32), np.ones(b - a, np.float32), p[a:b], EYE,
                                      np.zeros((1, 3), np.float32), None, 0.5, np.inf)
     one(0, half)
@@ -344,7 +344,7 @@ def test_forced_collisions_and_wrap_around(cap):
     rep = np.concatenate([rep[0::3], rep[1::3], rep[2::3]])
     p, rgb = _centres(rep, vs), _rgb(len(rep), cap)
     n = len(rep)
-    t, store = _table(cap, vs, (0, 0, 0))
+    t, store = _voxel_table(cap, vs, (0, 0, 0), "cuda")
     _frame_points(t, rgb, np.ones(n, np.float32), np.ones(n, np.float32), p, EYE, np.zeros((1, 3), np.float32), None,
                   0.5, np.inf)
     assert _occupied_slots(store, cap) == want_slots
@@ -366,7 +366,7 @@ def test_contention_past_2e24_points(voxels):
     n, vs = 1 << 22, 1 / 16
     rng = np.random.default_rng(voxels)
     org = np.array([0.01, -0.02, 0.03])
-    t, store = _table(1024, vs, org)
+    t, store = _voxel_table(1024, vs, org, "cuda")
     table = eo.new_table()
     centres = org + (np.array([[4, -3, 1], [4, -3, 2]]) + 0.5) * vs
     frames = 4 * voxels + 1
@@ -389,7 +389,7 @@ def test_contention_past_2e24_points(voxels):
 def _written(cap, slots, vs=0.25, origin=(0.5, -1.0, 2.0)):
     """A table whose slot i holds key `key` and sums `sums` for each (i, key, sums) of `slots`, and the same voxels
     as a restatement table."""
-    t, store = _table(cap, vs, origin)
+    t, store = _voxel_table(cap, vs, origin, "cuda")
     words = np.zeros(8 * cap + 4, np.uint64)
     table = eo.new_table()
     for i, key, sums in slots:

@@ -12,7 +12,7 @@ import localrf_b200 as L
 import mesh_oracle as mo
 import render64 as r64
 from localrf_b200 import _lib
-from localrf_b200.export import mesh
+from localrf_b200.export import _mesh_table, mesh
 from localrf_b200.ray_utils import contract
 
 pytestmark = pytest.mark.gpu
@@ -99,17 +99,6 @@ def test_lattice_matches_float64(variant):
     assert (got[owner == -1] == 0).all()
 
 
-def _table(capacity, max_tri, dev="cuda"):
-    words = capacity + (3 * capacity + 1) // 2 + max_tri + (3 * max_tri + 1) // 2
-    store = torch.zeros(words + 2, dtype=torch.int64, device=dev)
-    b = store.data_ptr()
-    verts = b + 8 * capacity
-    tk = verts + 8 * ((3 * capacity + 1) // 2)
-    t = _lib.LrfMeshTable(capacity=capacity, max_triangles=max_tri, keys=b, verts=verts, tri_keys=tk,
-                          tri_slots=tk + 8 * max_tri, stats=b + 8 * words)
-    return t, store
-
-
 def _extract(t):
     lib = _lib.lib()
     nb = lib.lrf_mesh_extract_scratch_bytes(t.capacity, t.max_triangles)
@@ -150,12 +139,12 @@ def test_cells_and_extract_equal_the_restatement(seed):
     s, keep = _scene_struct(lt, [[0, 0, 0]], voxel, origin, level=level)
     want = mo.mesh_lattice(v, lo, level, origin, voxel)
     assert len(want[1]) > 5000
-    t, store = _table(1 << 16, 1 << 16)
+    t, store = _mesh_table(1 << 16, 1 << 16, "cuda")
     vt = torch.from_numpy(v).cuda().reshape(-1).contiguous()
     _cells(s, lo, dims, vt, t)
     got = _extract(t)
     assert np.array_equal(got[0].view(np.uint32), want[0].view(np.uint32)) and np.array_equal(got[1], want[1])
-    t2, store2 = _table(1 << 16, 1 << 16)
+    t2, store2 = _mesh_table(1 << 16, 1 << 16, "cuda")
     for x0, x1 in ((0, 11), (10, 21)):
         for y0, y1 in ((0, 8), (7, 15), (14, 22)):
             for z0, z1 in ((0, 12), (11, 23)):
