@@ -159,9 +159,12 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
 
 def _mesh_bricks(w2rf, voxel_size, origin, max_norm, brick):
     """The bricks (lattice index of the lower corner, multiples of `brick` cells) whose cells meet some field's max_norm
-    cube, widened by one lattice step so that a surface cut by the cube's boundary closes outside it."""
+    cube, widened by one lattice step so that a surface cut by the cube's boundary closes outside it.  A field whose
+    world2rf has a NaN or infinite component owns no point (the owner rule of lrf_mesh_*), so it adds no brick."""
     out = set()
     for w in w2rf:
+        if not all(math.isfinite(x) for x in w):
+            continue
         lo, hi = [], []
         for a in range(3):
             lo.append(math.floor((-w[a] - max_norm - origin[a]) / voxel_size) - 1)
@@ -180,7 +183,8 @@ def mesh(local_tensorfs, voxel_size=1 / 128, level=0.005, origin=(0, 0, 0), max_
     contracted local position, and A = 0 beyond `max_norm` of every centre.  Marching cubes runs over the cells of the
     bricks (`_brick` cells per axis, tests only) that meet some field's cube.  The table holds at most capacity / 2
     vertices (`capacity` a power of two) and `max_triangles` triangles; a larger mesh raises RuntimeError naming the
-    parameter to raise.  The default level is the one TensoRF's mesh export passes with getDenseAlpha.
+    parameter to raise (`capacity` first when both overflow).  A field whose world2rf is not finite owns no point;
+    with no finite one the mesh is empty.  The default level is the one TensoRF's mesh export passes with getDenseAlpha.
 
     -> dict(xyz [V,3] float32, normals [V,3] float32 (outward: -grad A / |grad A|, central differences of half a
     voxel; 0 where the gradient vanishes), rgb [V,3] uint8, faces [T,3] int32 (counter-clockwise seen from outside)),

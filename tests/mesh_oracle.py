@@ -3,7 +3,9 @@ applied to given lattice values, and a float64 restatement of the scalar field A
 TEST INFRASTRUCTURE: nothing under localrf_b200/ imports it.
 
 The cells and extract stages are restated bit for bit: the same fp32 round-to-nearest vertex arithmetic, the same edge
-and triangle keys, the same sort orders.  This file keeps its own copy of the 256-case triangle table."""
+and triangle keys, the same sort orders.  This file keeps its own copy of the 256-case triangle table.  cells_np /
+extract_np restate the same stages with array operations, for lattices of up to ~10^7 cells; owner32 restates the
+owner rule in float32 and probe_slots the edge table's occupied slots."""
 import numpy as np
 import torch
 import torch.nn.functional as Fn
@@ -202,6 +204,127 @@ def merge(parts):
 def mesh_lattice(values, lo, level, origin, voxel_size):
     """cells + extract of one brick -> (xyz, faces)."""
     return extract(*cells(values, lo, level, origin, voxel_size))
+
+
+# ---- the same restatement, vectorised ----------------------------------------------------------------------------
+# TRI_TABLE as a [256, 16] array (-1 after the last edge), and per edge its lower corner's offset and its axis
+TRI_NP = np.array([r + [-1] * (16 - len(r)) for r in TRI_TABLE], np.int8)
+EDGE_OFF = np.array([np.minimum(CORNERS[a], CORNERS[b]) for a, b in EDGES], np.int32)
+EDGE_AXIS = np.array([int(np.argmax(np.abs(np.subtract(CORNERS[b], CORNERS[a])))) for a, b in EDGES], np.int32)
+WINDING = np.array([0, 2, 1], np.int32)                  # (e0, e2, e1): the outward winding
+SLAB_CELLS = 1 << 20                                     # cells per x-slab of cells_parts
+
+
+def _keys_np(g, shifts):
+    """Keys of lattice indices g [..., 3] (each in [-2^19, 2^19)): (g_a + 2^19) << shifts[a], or-ed -> uint64."""
+    out = np.zeros(g.shape[:-1], np.uint64)
+    for a in range(3):
+        out |= (g[..., a].astype(np.int64) + HALF).astype(np.uint64) << np.uint64(shifts[a])
+    return out
+
+
+def cells_parts(values, lo, level, origin, voxel_size):
+    """cells() vectorised, one x-slab of cells at a time so its memory stays bounded.  -> (edge keys [E] uint64,
+    vertices [E, 3] float32, triangle sort keys [T] uint64, triangle edge keys [T, 3] uint64); an edge may appear
+    once per slab, every time with the same vertex bits."""
+    v = np.asarray(values, np.float32)
+    d = v.shape
+    ny, nz = d[1] - 1, d[2] - 1
+    lvl, vs = np.float32(level), np.float32(voxel_size)
+    org = np.asarray(origin, np.float32)
+    lo = np.asarray(lo, np.int32)
+    step = max(1, SLAB_CELLS // max(1, ny * nz))
+    ek, ev, tk, te = [], [], [], []
+    for x0 in range(0, d[0] - 1, step):
+        x1 = min(x0 + step, d[0] - 1)
+        ins = v[x0:x1 + 1] >= lvl                                       # NaN is outside
+        idx = np.zeros((x1 - x0, ny, nz), np.uint8)
+        for c, (ox, oy, oz) in enumerate(CORNERS):
+            idx |= ins[ox:ox + x1 - x0, oy:oy + ny, oz:oz + nz].astype(np.uint8) << np.uint8(c)
+        cell = np.stack(np.nonzero((idx != 0) & (idx != 255)), 1).astype(np.int32)
+        if len(cell) == 0:
+            continue
+        case = idx[cell[:, 0], cell[:, 1], cell[:, 2]]
+        cell[:, 0] += x0
+        del idx, ins
+        tri = TRI_NP[case]
+        ci, k = np.nonzero(tri[:, 0:15:3] >= 0)
+        e = tri[ci[:, None], 3 * k[:, None] + WINDING].astype(np.int32)  # [T, 3] the edges, outward winding
+        del tri
+        pt = cell[ci][:, None, :] + EDGE_OFF[e]                           # [T, 3, 3] lower points in the brick
+        axis = EDGE_AXIS[e]
+        keys = _keys_np(pt + lo, (42, 22, 2)) | axis.astype(np.uint64)
+        tk.append((_keys_np(cell[ci] + lo, (40, 20, 0)) << np.uint64(3)) | k.astype(np.uint64))
+        te.append(keys)
+        uk, first = np.unique(keys.reshape(-1), return_index=True)
+        lp, ax = pt.reshape(-1, 3)[first], axis.reshape(-1)[first]
+        del pt, axis, e
+        r = np.arange(len(ax))
+        hp = lp.copy()
+        hp[r, ax] += 1
+        va, vb = v[lp[:, 0], lp[:, 1], lp[:, 2]], v[hp[:, 0], hp[:, 1], hp[:, 2]]
+        with np.errstate(all="ignore"):
+            t = (lvl - va) / (vb - va)
+        t = np.where(np.isfinite(t), np.clip(t, np.float32(0), np.float32(1)), np.float32(0)).astype(np.float32)
+        gl = lp + lo
+        xyz = (org[None] + gl.astype(np.float32) * vs).astype(np.float32)
+        pa = xyz[r, ax]
+        pb = (org[ax] + (gl[r, ax] + 1).astype(np.float32) * vs).astype(np.float32)
+        xyz[r, ax] = pa + t * (pb - pa)
+        ek.append(uk)
+        ev.append(xyz)
+    cat = lambda parts, shape, dt: np.concatenate(parts) if parts else np.zeros(shape, dt)
+    return (cat(ek, (0,), np.uint64), cat(ev, (0, 3), np.float32), cat(tk, (0,), np.uint64),
+            cat(te, (0, 3), np.uint64))
+
+
+def extract_np(parts):
+    """extract() of the concatenation of cells_parts() of one or more bricks (merge(), then extract(), vectorised):
+    each edge key's first vertex, in ascending key order, and the triangles in ascending sort-key order as vertex
+    ranks.  -> (xyz [V, 3] float32, faces [T, 3] int32)."""
+    keys = np.concatenate([p[0] for p in parts])
+    uk, first = np.unique(keys, return_index=True)
+    del keys
+    xyz = np.concatenate([p[1] for p in parts])[first]
+    tk = np.concatenate([p[2] for p in parts])
+    order = np.argsort(tk, kind="stable")
+    del tk
+    te = np.concatenate([p[3] for p in parts])
+    faces = np.empty((len(order), 3), np.int32)
+    for i in range(0, len(order), 1 << 22):
+        faces[i:i + (1 << 22)] = np.searchsorted(uk, te[order[i:i + (1 << 22)]])
+    return xyz, faces
+
+
+def cells_np(values, lo, level, origin, voxel_size):
+    """mesh_lattice vectorised: the same (xyz, faces), bit for bit."""
+    return extract_np([cells_parts(values, lo, level, origin, voxel_size)])
+
+
+# ---- the owner rule and the table's slots ------------------------------------------------------------------------
+def owner32(xyz, w2rf):
+    """The owner rule of lrf_mesh_* in float32: per field k, y = float32(p) + float32(w_k) per axis; a field with a NaN
+    component of y is skipped, the smallest max |y_a| wins strictly (exact ties to the lowest k, +inf never wins).
+    -> (owner [M] int32, -1 when no field has a finite norm; its norm [M] float32, +inf there)."""
+    p = np.asarray(xyz, np.float32).reshape(-1, 3)
+    w = np.asarray(w2rf, np.float32).reshape(-1, 3)
+    owner = np.full(len(p), -1, np.int32)
+    best = np.full(len(p), np.inf, np.float32)
+    for k in range(len(w)):
+        y = p + w[k]
+        with np.errstate(invalid="ignore"):
+            n = np.abs(y).max(1)
+            win = ~np.isnan(y).any(1) & (n < best)
+        owner[win] = k
+        best[win] = n[win]
+    return owner, best
+
+
+def probe_slots(keys, capacity):
+    """The occupied slots of the edge table (csrc/lrf_table.cuh: linear probing from mix64(key) & (capacity - 1),
+    wrapping to 0) after the distinct `keys` are claimed, in any order."""
+    import export_oracle as eo
+    return eo.probe_table(keys, capacity)
 
 
 # ---- checks of a mesh --------------------------------------------------------------------------------------------

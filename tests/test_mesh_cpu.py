@@ -242,3 +242,15 @@ def test_brick_table_and_output_refusals():
     s.fields = fields
     steps[0] = 0.0
     _err(L.lrf_mesh_lattice(C.byref(s), lo, d, FAKE, None), "step_size")
+
+
+def test_mesh_bricks_skip_non_finite_world2rf_rows():
+    """A world2rf row with a NaN or infinite component owns no lattice point, so it adds no brick; with no finite row
+    there is none."""
+    from localrf_b200.export import _mesh_bricks
+    args = (0.25, [0.0, 0.5, -0.5], 1.0, 4)
+    want = _mesh_bricks([[0.0, 0.0, 0.0], [0.5, -0.25, 0.0]], *args)
+    assert len(want) > 8
+    rows = [[math.nan, 0.0, 0.0], [0.0, math.inf, 0.0], [0.0, 0.0, -math.inf], [math.nan] * 3]
+    assert _mesh_bricks([rows[0], [0.0, 0.0, 0.0], rows[1], [0.5, -0.25, 0.0], rows[2], rows[3]], *args) == want
+    assert _mesh_bricks(rows, *args) == []
