@@ -143,7 +143,10 @@ typedef struct LrfOutputs {
    * until all local flags have reached wait_seq (the peers are done with the buffer about to be overwritten;
    * 0 = no wait); the LAST CTA to finish release-stores signal_seq into slot `rank` of every peer's array,
    * after all pixel stores of the launch.  With wait_seq = signal_seq - lag (lag >= 1) this replaces
-   * lrf_peer_signal_wait altogether: a step costs no extra launch. */
+   * lrf_peer_signal_wait altogether: a step costs no extra launch.
+   * These fields are checked for every batch, n_rays = 0 included (LRF_ERR_INVALID before any device work).  An
+   * empty batch stores no pixels; with signal_seq > 0 it publishes the step as above and waits for nothing
+   * (wait_seq is checked, not waited on). */
   unsigned long long *peer_flags[16];
   int32_t rank;
   unsigned long long signal_seq, wait_seq;

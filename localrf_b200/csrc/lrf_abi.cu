@@ -459,6 +459,29 @@ int check_plane(const void* p, int32_t ws, int32_t hs, int64_t stride, int per_p
   return LRF_OK;
 }
 
+// the fused pixel exchange fields of lrf_render's outputs, for every batch: an empty one still publishes its step
+int check_exchange(const LrfOutputs* o) {
+  if (o->n_peers < 0 || o->n_peers > LRF_MAX_PEERS) return fail(LRF_ERR_INVALID, "n_peers out of range");
+  if (o->n_peers > 0) {
+    if (!o->pix) return fail(LRF_ERR_INVALID, "the fused pixel exchange needs the interleaved `pix` output");
+    if (o->mc_pix) {
+      if ((uintptr_t)o->mc_pix & 15) return fail(LRF_ERR_INVALID, "mc_pix must be 16-byte aligned");
+    } else {
+      for (int p = 0; p < o->n_peers; ++p)
+        if (!o->peer_pix[p] || ((uintptr_t)o->peer_pix[p] & 15))
+          return fail(LRF_ERR_INVALID, "peer_pix pointers must be non-NULL and 16-byte aligned");
+    }
+  }
+  if (o->signal_seq) {
+    if (o->n_peers < 1 || o->rank < 0 || o->rank >= o->n_peers || o->wait_seq > o->signal_seq)
+      return fail(LRF_ERR_INVALID, "in-kernel signalling needs n_peers >= 1, 0 <= rank < n_peers, wait_seq <= signal_seq");
+    for (int p = 0; p < o->n_peers; ++p)
+      if (!o->peer_flags[p] || ((uintptr_t)o->peer_flags[p] & 7))
+        return fail(LRF_ERR_INVALID, "peer_flags pointers must be non-NULL and 8-byte aligned");
+  }
+  return LRF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -525,15 +548,12 @@ int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const
   if ((F.fea_pe || F.view_pe) && F.grid16)
     return fail(LRF_ERR_UNSUPPORTED, "bf16 grid storage is built for fields without positional encodings");
   if (b->n_rays < 0) return fail(LRF_ERR_INVALID, "n_rays < 0");
+  if ((rc = check_exchange(o)) != LRF_OK) return rc;
   if (b->n_rays == 0) {
-    // nothing to render; a rank with an empty shard must still publish its step to the peers
-    if (o->signal_seq && o->n_peers >= 1 && o->rank >= 0 && o->rank < o->n_peers) {
-      for (int p = 0; p < o->n_peers; ++p)
-        if (!o->peer_flags[p]) return fail(LRF_ERR_INVALID, "peer_flags pointer is NULL");
-      return cuda_status(lrf::launch_peer_barrier(o->peer_flags, o->rank, o->n_peers, o->signal_seq, 0ull,
-                                                  (cudaStream_t)stream), "peer_barrier_kernel");
-    }
-    return LRF_OK;
+    // nothing to render; a rank with an empty shard must still publish its step to the peers (and waits for none)
+    if (!o->signal_seq) return LRF_OK;
+    return cuda_status(lrf::launch_peer_barrier(o->peer_flags, o->rank, o->n_peers, o->signal_seq, 0ull,
+                                                (cudaStream_t)stream), "peer_barrier_kernel");
   }
   if (!o->pix && (!o->rgb || !o->depth)) return fail(LRF_ERR_INVALID, "rgb/depth output is NULL");
   lrf::BatchDev B;
@@ -553,31 +573,16 @@ int lrf_render(const LrfField* f, const void* prepared, const LrfBatch* b, const
   B.dirs = b->rays ? nullptr : o->directions;
   B.ij = b->rays ? nullptr : reinterpret_cast<long long*>(o->ij);
   B.stats = o->stats;
-  if (o->n_peers < 0 || o->n_peers > LRF_MAX_PEERS) return fail(LRF_ERR_INVALID, "n_peers out of range");
-  B.n_peers = o->n_peers;
+  B.n_peers = o->n_peers;                                            // (checked by check_exchange above)
   B.mc_pix = nullptr;
   if (o->n_peers > 0) {
-    if (!o->pix) return fail(LRF_ERR_INVALID, "the fused pixel exchange needs the interleaved `pix` output");
-    if (o->mc_pix) {
-      if ((uintptr_t)o->mc_pix & 15) return fail(LRF_ERR_INVALID, "mc_pix must be 16-byte aligned");
-      B.mc_pix = o->mc_pix;
-    } else {
-      for (int p = 0; p < o->n_peers; ++p) {
-        if (!o->peer_pix[p] || ((uintptr_t)o->peer_pix[p] & 15))
-          return fail(LRF_ERR_INVALID, "peer_pix pointers must be non-NULL and 16-byte aligned");
-        B.peer_pix[p] = o->peer_pix[p];
-      }
-    }
+    if (o->mc_pix) B.mc_pix = o->mc_pix;
+    else
+      for (int p = 0; p < o->n_peers; ++p) B.peer_pix[p] = o->peer_pix[p];
   }
   B.signal_seq = 0; B.wait_seq = 0; B.rank = 0;
   if (o->signal_seq) {
-    if (o->n_peers < 1 || o->rank < 0 || o->rank >= o->n_peers || o->wait_seq > o->signal_seq)
-      return fail(LRF_ERR_INVALID, "in-kernel signalling needs n_peers >= 1, 0 <= rank < n_peers, wait_seq <= signal_seq");
-    for (int p = 0; p < o->n_peers; ++p) {
-      if (!o->peer_flags[p] || ((uintptr_t)o->peer_flags[p] & 7))
-        return fail(LRF_ERR_INVALID, "peer_flags pointers must be non-NULL and 8-byte aligned");
-      B.peer_flags[p] = o->peer_flags[p];
-    }
+    for (int p = 0; p < o->n_peers; ++p) B.peer_flags[p] = o->peer_flags[p];
     B.signal_seq = o->signal_seq; B.wait_seq = o->wait_seq; B.rank = o->rank;
   }
   DevInfo d;

@@ -36,22 +36,24 @@ def shard_bounds(n_rays, rank, world, align=8):
 
 def shard_views(view_ids, n_rays, rank, world):
     """Shard of a training-style batch (rays grouped by view): whole views per rank, so the
-    kernel's view indexing (ray // rays_per_view) stays valid inside the shard."""
-    n_views = view_ids.shape[0]
+    kernel's view indexing (ray // rays_per_view) stays valid inside the shard.  -> (v_lo, v_hi, lo, hi)"""
+    n_views = len(view_ids)
     per_view = n_rays // n_views
     v_lo, v_hi = shard_bounds(n_views, rank, world, align=1)
     return v_lo, v_hi, v_lo * per_view, v_hi * per_view
 
 
-def gather_pixels(rgb, depth, n_total, group=None):
+def gather_pixels(rgb, depth, n_total, group=None, bounds=None):
     """One all-gather of the rendered pixels: local [n_local,3] + [n_local] -> [n_total,3], [n_total].
 
-    Shards may differ in length by one aligned block, so every rank pads to the largest shard."""
+    `bounds` = every rank's shard [lo, hi), in rank order, contiguous over [0, n_total) (default: shard_bounds).
+    Shards may differ in length, so every rank pads to the largest shard."""
     world = dist.get_world_size(group)
     if world == 1:
         return rgb, depth
     rank = dist.get_rank(group)
-    bounds = [shard_bounds(n_total, r, world) for r in range(world)]
+    if bounds is None:
+        bounds = [shard_bounds(n_total, r, world) for r in range(world)]
     width = max(hi - lo for lo, hi in bounds)
     pix = torch.zeros(width, 4, dtype=rgb.dtype, device=rgb.device)
     n_local = bounds[rank][1] - bounds[rank][0]
@@ -190,20 +192,29 @@ class PixelExchange:
 
 
 def render_sharded(local_tensorfs, ray_ids, view_ids, W, H, group=None, exchange=None, **kw):
-    """LocalTensorfs.forward with the rays of an eval batch (single view) sharded over the ranks;
-    every rank returns the full (rgb, depth).  With a `PixelExchange` the pixels are exchanged by the
-    render kernel itself (returned tensors are views of the exchange buffer, valid until the step
-    after next); without one, by one NCCL all-gather."""
+    """LocalTensorfs.forward with the rays of an eval batch sharded over the ranks; every rank returns the
+    full (rgb, depth).  A single-view batch is sharded by `shard_bounds`, a multi-view one (rays grouped by
+    view) by whole views (`shard_views`), since the kernel takes a ray's view from its position in the
+    launch.  With a `PixelExchange` the pixels are exchanged by the render kernel itself (returned tensors
+    are views of the exchange buffer, valid until the step after next); without one, by one NCCL all-gather."""
     world = dist.get_world_size(group)
     rank = dist.get_rank(group)
     n = ray_ids.shape[0]
-    lo, hi = shard_bounds(n, rank, world)
+    if len(view_ids) > 1:
+        parts = [shard_views(view_ids, n, r, world) for r in range(world)]
+        bounds = [(lo, hi) for _, _, lo, hi in parts]
+        v_lo, v_hi = parts[rank][:2]
+        views = view_ids[v_lo:v_hi]
+    else:
+        bounds = [shard_bounds(n, r, world) for r in range(world)]
+        views = view_ids
+    lo, hi = bounds[rank]
     if exchange is None:
-        rgb, depth, _, _ = local_tensorfs(ray_ids[lo:hi], view_ids, W, H, **kw)
-        return gather_pixels(rgb, depth, n, group)
+        rgb, depth, _, _ = local_tensorfs(ray_ids[lo:hi], views, W, H, **kw)
+        return gather_pixels(rgb, depth, n, group, bounds)
     if n > exchange.max_rays:
         raise ValueError(f"batch of {n} rays exceeds the exchange buffer ({exchange.max_rays})")
-    local_tensorfs(ray_ids[lo:hi], view_ids, W, H, exchange=(exchange, lo), **kw)   # (an empty shard only signals)
+    local_tensorfs(ray_ids[lo:hi], views, W, H, exchange=(exchange, lo), **kw)   # (an empty shard only signals)
     full = exchange.gathered(n)
     return full[:, :3], full[:, 3]
 

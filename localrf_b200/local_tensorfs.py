@@ -626,10 +626,20 @@ class LocalTensorfs(torch.nn.Module):
                 blend = blending_weights.detach().to(dev, torch.float32).contiguous()
                 active = torch.nonzero(blend.sum(dim=0))[:, 0].tolist()
             if len(active) == 0:
+                if exchange is not None:
+                    # (before anything is enqueued: the exchange's step count does not advance; ranks sharding
+                    # one view hold the same blending row, so they all raise at this step)
+                    raise NotImplementedError("exchange= needs a field that renders the batch's views")
                 print("****** No valid RF")
                 i, j = ids2pixel(W, H, ray_ids)
                 ones = torch.ones_like(ray_ids).float()
-                return torch.ones([n, 3], device=dev), ones, torch.zeros(n, 3, device=dev), torch.stack([i, j], -1)
+                if out is None:
+                    return torch.ones([n, 3], device=dev), ones, torch.zeros(n, 3, device=dev), torch.stack([i, j], -1)
+                rgbs, depth = self._alloc_outputs(n, dev, None, out)[1:3]
+                with torch.cuda.device(dev):            # in stream order, like the kernel's stores (out may be pinned)
+                    rgbs.copy_(torch.ones(n, 3, device=dev), non_blocking=True)
+                    depth.copy_(torch.ones(n, device=dev), non_blocking=True)
+                return rgbs, depth, torch.zeros(n, 3, device=dev), torch.stack([i, j], -1)
 
             if world2rf is None:
                 world2rf = self.world2rf

@@ -37,15 +37,20 @@ def _fake_render(ids):
     return torch.stack([torch.sin(x), torch.cos(x), x / 1000.0], -1), torch.sqrt(x + 1.0)
 
 
-def _worker(rank, world, port, n, q):
+def _worker(rank, world, port, n, q, n_views=1):
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         ids = torch.arange(n)
-        lo, hi = shard_bounds(n, rank, world)
+        bounds = None
+        if n_views > 1:                              # whole views per rank: shards of any length, empty ones included
+            bounds = [shard_views(torch.arange(n_views), n, r, world)[2:] for r in range(world)]
+            lo, hi = bounds[rank]
+        else:
+            lo, hi = shard_bounds(n, rank, world)
         rgb, depth = _fake_render(ids[lo:hi])
-        full_rgb, full_depth = gather_pixels(rgb, depth, n)
+        full_rgb, full_depth = gather_pixels(rgb, depth, n, bounds=bounds)
         ref_rgb, ref_depth = _fake_render(ids)
         ok = torch.equal(full_rgb, ref_rgb) and torch.equal(full_depth, ref_depth)
         q.put((rank, bool(ok)))
@@ -53,21 +58,38 @@ def _worker(rank, world, port, n, q):
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("n", [4096, 1001])
-def test_gather_pixels_equals_single_process(n):
-    world = 2
+def _run_gather(n, world, n_views):
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
         port = s.getsockname()[1]
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, n, q)) for r in range(world)]
+    procs = [ctx.Process(target=_worker, args=(r, world, port, n, q, n_views)) for r in range(world)]
     for p in procs:
         p.start()
     results = [q.get(timeout=120) for _ in range(world)]
     for p in procs:
         p.join(timeout=60)
-    assert sorted(results) == [(0, True), (1, True)]
+    return sorted(results)
+
+
+@pytest.mark.parametrize("n", [4096, 1001])
+def test_gather_pixels_equals_single_process(n):
+    assert _run_gather(n, 2, 1) == [(0, True), (1, True)]
+
+
+@pytest.mark.parametrize("n,world,n_views", [(300, 2, 3), (4096, 3, 16), (74, 3, 2)])
+def test_gather_pixels_whole_view_shards(n, world, n_views):
+    """Whole-view shards of a multi-view batch (shard_views, the bounds handed to gather_pixels): 200 + 100 rays,
+    6 + 5 + 5 views of 256, and 37 + 37 + 0 rays (a rank without a view)."""
+    assert _run_gather(n, world, n_views) == [(r, True) for r in range(world)]
+
+
+def test_shard_views_uneven_and_empty():
+    """Views that do not divide evenly give the first ranks one view more; more ranks than views leave the last
+    ones empty, at the end of the batch; a list of view ids shards like a tensor."""
+    assert [shard_views(torch.arange(3), 300, r, 2) for r in range(2)] == [(0, 2, 0, 200), (2, 3, 200, 300)]
+    assert [shard_views([4, 9], 74, r, 3) for r in range(3)] == [(0, 1, 0, 37), (1, 2, 37, 74), (2, 2, 74, 74)]
 
 
 def _grad_worker(rank, world, port, q):
