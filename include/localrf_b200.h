@@ -158,8 +158,9 @@ const char *lrf_last_error(void);
 /* sizeof() of the ABI structs as this library was compiled: 0 LrfField, 1 LrfBatch, 2 LrfOutputs,
  * 3 LrfGradients, 4 LrfLossBatch, 5 LrfLossGrads, 6 LrfAdamTensor, 7 LrfCameraGrads, 8 LrfFrameStore,
  * 9 LrfRayGather, 10 LrfPanelFrame, 11 LrfIngestFrame, 12 LrfPointFrame, 13 LrfVoxelTable, 14 LrfMeshScene,
- * 15 LrfMeshTable (0 for any other index).  Bindings compare these with their own mirrors at load
- * time, so a stale library or a drifted mirror fails loudly instead of mis-reading arguments. */
+ * 15 LrfMeshTable, 17 LrfColourFrame (0 for any other index; 16 is left unused and stays 0, as libraries
+ * before LrfColourFrame answered).  Bindings compare these with their own mirrors at load time, so a stale library
+ * or a drifted mirror fails loudly instead of mis-reading arguments. */
 size_t lrf_sizeof(int32_t which);
 
 /* Device bytes of the per-field "prepared" block (folded / re-laid-out MLP weights) of a field without
@@ -673,6 +674,50 @@ size_t lrf_voxel_extract_scratch_bytes(int64_t capacity);
  * and scratch that is NULL, not 256-byte aligned or smaller than lrf_voxel_extract_scratch_bytes(capacity). */
 int lrf_voxel_extract(const LrfVoxelTable *table, int64_t min_count, float *xyz, uint8_t *rgb, int32_t *count,
                       int64_t *n_voxels, void *scratch, size_t scratch_bytes, lrf_stream_t stream);
+
+/* ---- colours from the frames: points projected into the rendered views that see them, blended on the device -------
+ * One rendered view and its photo, all in device memory. */
+typedef struct LrfColourFrame {
+  int32_t W, H;                /* >= 1, W H < 2^31 */
+  int32_t fov360;              /* nonzero: equirectangular (get_ray_directions_360), else pinhole */
+  const float *intrinsics;     /* [3] focal, cx, cy, as LrfBatch.intrinsics (not read for fov360) */
+  const float *cam2world;      /* [3][4] the view's camera */
+  const float *depth;          /* [H W] the view's eval render (LrfOutputs.depth) */
+  const float *acc;            /* [H W] its blended opacity (lrf_ray_opacity) */
+  const float *image;          /* [H][W][3] the frame, fp32 RGB */
+  float min_acc;               /* a pixel counts when acc >= min_acc (not NaN) ... */
+  float depth_tol;             /* ... and |d_v - s| <= depth_tol s (> 0, finite) ... */
+  float min_cos;               /* ... and, with normals, w >= min_cos (in (0, 1]) */
+} LrfColourFrame;
+
+/* Adds one view's pixels to the points that view sees.  Per point p (xyz [n][3]), fp32 round to nearest in this order,
+ * no FMA, with R = cam2world[:, :3], t = cam2world[:, 3]:
+ *   1. c_b = (R_0b (p_0 - t_0) + R_1b (p_1 - t_1)) + R_2b (p_2 - t_2).
+ *   2. pinhole (needs c_2 < 0): d_v = -c_2, i = floor(c_0 / d_v f + cx), j = floor(-c_1 / d_v f + cy); the pixel must
+ *      lie in [0, W) x [0, H).  d_v is the planar depth, which the render's depth is for get_ray_directions_lean's
+ *      z = -1 directions.
+ *   3. fov360 (inverts get_ray_directions_360): d_v = r = sqrt((c_0 c_0 + c_1 c_1) + c_2 c_2) (needs 0 < r < inf),
+ *      phi = asinf(clamp(c_1 / r, -1, 1)), theta = atan2f(c_0, c_2), j = floor((phi + pi/2) H / pi) clamped to
+ *      [0, H - 1], i = floor((theta - pi) W / (2 pi)) mod W (fp32 pi; asinf and atan2f are CUDA's, within their ulp
+ *      bounds).  d_v is the range, since those directions are unit vectors.
+ *   4. depth test at k = j W + i: a = acc[k], s = depth[k] / a; the pixel counts only if a >= min_acc, a > 0, s is
+ *      finite, s > 0 and |d_v - s| <= depth_tol s.
+ *   5. weight: w = 1 when normals is NULL; else w = ((n_0 e_0 + n_1 e_1) + n_2 e_2) / sqrt((e_0 e_0 + e_1 e_1) + e_2 e_2)
+ *      with e = t - p, and the point needs w >= min_cos (a zero normal never passes).
+ *   6. a pixel with a non-finite channel adds nothing; else q = (uint32)(min(w, 1) 2^16), c24_ch =
+ *      (uint32)(clamp(image[k][ch], 0, 1) 2^24) and sums[p] += {1, q, q c24_r, q c24_g, q c24_b} (atomics).
+ * The sums are integers, so they are bitwise the same whatever the frame order or thread scheduling; w is capped at 1
+ * so that each view adds at most 2^40 to a sum.  Zero sums [n][5] before the first view.  One launch, one thread per
+ * point, no host synchronisation.  LRF_ERR_INVALID before any device work for a NULL frame, xyz, sums or frame
+ * pointer (normals may be NULL), n < 0 or n >= 2^31, W or H < 1 or W H >= 2^31, sums not 8-byte aligned, a NaN
+ * min_acc, a depth_tol that is not > 0 and finite, and a min_cos outside (0, 1]. */
+int lrf_frame_colours(const LrfColourFrame *frame, const float *xyz, const float *normals, int64_t n,
+                      unsigned long long *sums, lrf_stream_t stream);
+/* Per point of sums [n][5]: count[p] = sums[p][0] (the views that coloured it; int32, saturated) and rgb[p][ch] =
+ * (uint8)floor(sum q c24_ch / (sum q 2^24) 255 + 0.5) in fp64, rounded once; rgb is 0 where sum q is 0 (count 0
+ * included).  rgb [n][3] and count [n] are device memory.  One launch, no atomics.  LRF_ERR_INVALID before any device
+ * work for a NULL sums, rgb or count, n < 0 or n >= 2^31, and sums not 8-byte aligned. */
+int lrf_colour_extract(const unsigned long long *sums, int64_t n, uint8_t *rgb, int32_t *count, lrf_stream_t stream);
 
 /* ---- mesh export: marching cubes over the fields' density on a world-space lattice, on the device -----------------
  * Lattice point i = (ix, iy, iz) sits at p_a = origin_a + i_a voxel_size (fp32, round to nearest).  The scalar field at

@@ -118,6 +118,12 @@ class LrfMeshTable(C.Structure):
                 ("tri_keys", _vp), ("tri_slots", _vp), ("stats", _vp)]
 
 
+class LrfColourFrame(C.Structure):
+    _fields_ = [("W", C.c_int32), ("H", C.c_int32), ("fov360", C.c_int32), ("intrinsics", _vp), ("cam2world", _vp),
+                ("depth", _vp), ("acc", _vp), ("image", _vp), ("min_acc", C.c_float), ("depth_tol", C.c_float),
+                ("min_cos", C.c_float)]
+
+
 MESH_MAX_FIELDS = 64
 
 
@@ -171,7 +177,7 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_test_panels_scratch_bytes", "lrf_test_panels", "lrf_ingest_scratch_bytes", "lrf_ingest_frame",
            "lrf_resize_linear", "lrf_ray_opacity", "lrf_frame_points", "lrf_voxel_extract_scratch_bytes",
            "lrf_voxel_extract", "lrf_mesh_lattice", "lrf_mesh_cells", "lrf_mesh_extract_scratch_bytes",
-           "lrf_mesh_extract", "lrf_mesh_normals"]
+           "lrf_mesh_extract", "lrf_mesh_normals", "lrf_frame_colours", "lrf_colour_extract"]
 
 
 def _stale():
@@ -224,9 +230,10 @@ def lib():
                            "rebuild it (python -c 'import localrf_b200; localrf_b200.build(force=True)')")
     L.lrf_sizeof.restype = C.c_size_t
     L.lrf_sizeof.argtypes = [C.c_int32]
-    for which, mirror in enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
-                                     LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather, LrfPanelFrame,
-                                     LrfIngestFrame, LrfPointFrame, LrfVoxelTable, LrfMeshScene, LrfMeshTable)):
+    mirrors = list(enumerate((LrfField, LrfBatch, LrfOutputs, LrfGradients, LrfLossBatch, LrfLossGrads,
+                              LrfAdamTensor, LrfCameraGrads, LrfFrameStore, LrfRayGather, LrfPanelFrame,
+                              LrfIngestFrame, LrfPointFrame, LrfVoxelTable, LrfMeshScene, LrfMeshTable)))
+    for which, mirror in mirrors + [(17, LrfColourFrame)]:
         if L.lrf_sizeof(which) != C.sizeof(mirror):
             raise RuntimeError(f"localrf_b200: struct {mirror.__name__} is {L.lrf_sizeof(which)} bytes in "
                                f"{LIB_PATH} but {C.sizeof(mirror)} in the ctypes mirror -- stale build")
@@ -297,6 +304,8 @@ def lib():
     L.lrf_mesh_extract_scratch_bytes.argtypes = [C.c_int64, C.c_int64]
     L.lrf_mesh_extract.argtypes = [C.POINTER(LrfMeshTable), _vp, _vp, _vp, _vp, C.c_size_t, _vp]
     L.lrf_mesh_normals.argtypes = [C.POINTER(LrfMeshScene), _vp, C.c_int64, _vp, _vp, _vp]
+    L.lrf_frame_colours.argtypes = [C.POINTER(LrfColourFrame), _vp, _vp, C.c_int64, _vp, _vp]
+    L.lrf_colour_extract.argtypes = [_vp, C.c_int64, _vp, _vp, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

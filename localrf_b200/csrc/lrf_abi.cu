@@ -506,6 +506,7 @@ size_t lrf_sizeof(int32_t which) {
     case 13: return sizeof(LrfVoxelTable);
     case 14: return sizeof(LrfMeshScene);
     case 15: return sizeof(LrfMeshTable);
+    case 17: return sizeof(LrfColourFrame);
     default: return 0;
   }
 }
@@ -950,6 +951,38 @@ int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uin
   if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_voxel_extract(*t, min_count, xyz, rgb, (int*)count, (long long*)n_voxels, scratch,
                                                (cudaStream_t)stream), "voxel_extract");
+}
+
+// the point count and sums of lrf_frame_colours and lrf_colour_extract
+int check_colour_sums(const unsigned long long* sums, int64_t n) {
+  if (n < 0 || n > 2147483647LL) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
+  if (!sums || ((uintptr_t)sums & 7)) return fail(LRF_ERR_INVALID, "sums must be non-NULL and 8-byte aligned");
+  return LRF_OK;
+}
+
+int lrf_frame_colours(const LrfColourFrame* f, const float* xyz, const float* normals, int64_t n,
+                      unsigned long long* sums, lrf_stream_t stream) {
+  if (!f) return fail(LRF_ERR_INVALID, "frame is NULL");
+  int rc = check_colour_sums(sums, n);
+  if (rc != LRF_OK) return rc;
+  if (!xyz) return fail(LRF_ERR_INVALID, "xyz is NULL");
+  if (f->W < 1 || f->H < 1 || (int64_t)f->W * f->H > 2147483647LL)
+    return fail(LRF_ERR_INVALID, "W and H must be >= 1 with W H < 2^31");
+  if (!f->intrinsics || !f->cam2world || !f->depth || !f->acc || !f->image)
+    return fail(LRF_ERR_INVALID, "intrinsics / cam2world / depth / acc / image of the frame is NULL");
+  if (std::isnan(f->min_acc)) return fail(LRF_ERR_INVALID, "min_acc is NaN");
+  if (!positive_finite(f->depth_tol)) return fail(LRF_ERR_INVALID, "depth_tol must be > 0 and finite");
+  if (!(f->min_cos > 0.0f && f->min_cos <= 1.0f)) return fail(LRF_ERR_INVALID, "min_cos must lie in (0, 1]");
+  return cuda_status(lrf::launch_frame_colours(*f, xyz, normals, n, sums, (cudaStream_t)stream),
+                     "frame_colours_kernel");
+}
+
+int lrf_colour_extract(const unsigned long long* sums, int64_t n, uint8_t* rgb, int32_t* count, lrf_stream_t stream) {
+  const int rc = check_colour_sums(sums, n);
+  if (rc != LRF_OK) return rc;
+  if (!rgb || !count) return fail(LRF_ERR_INVALID, "rgb / count is NULL");
+  return cuda_status(lrf::launch_colour_extract(sums, n, rgb, (int*)count, (cudaStream_t)stream),
+                     "colour_extract_kernel");
 }
 
 // (the scene's device view is ~17 KB: static storage per host thread rather than stack)

@@ -11,6 +11,10 @@
 // The back-projection and the key are written with explicit round-to-nearest fp32 operations in a fixed order (no
 // FMA contraction), so a numpy float32 restatement reproduces them bit for bit; the per-voxel means are fp64, rounded
 // once.
+//
+// lrf_frame_colours / lrf_colour_extract colour given points (a mesh's vertices, a cloud's points) from the video's
+// frames: each point is projected into one rendered view, tested against the view's expected depth, and the frame's
+// pixel is added to the point's integer sums; the blend is fp64, rounded once.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -27,6 +31,7 @@ constexpr int OP_RAYS = 128;           // rays per CTA of ray_opacity_kernel (on
 constexpr int OP_TILE = 32;            // samples per tile staged through shared memory
 constexpr int PT_THREADS = 256;
 constexpr int EX_THREADS = 256;
+constexpr int CO_THREADS = 256;
 constexpr int KEY_BITS = 21;           // per axis: keys in [-2^20, 2^20), 63 bits in all
 constexpr float KEY_LIM = 1048576.0f;  // 2^20
 
@@ -123,6 +128,88 @@ __global__ void __launch_bounds__(PT_THREADS) frame_points_kernel(const LrfPoint
   });
 }
 
+// One thread per point: the pixel of the view that sees it, the depth test against the view's rendered depth, then
+// the integer sums of lrf_frame_colours (include/localrf_b200.h, which states every operation).  Each point is one
+// thread's, so the atomics never contend; they keep the sums exact when frames of one table run on several streams.
+__global__ void __launch_bounds__(CO_THREADS) frame_colours_kernel(const LrfColourFrame f, const float* __restrict__ xyz,
+                                                                   const float* __restrict__ normals, long long n,
+                                                                   unsigned long long* sums) {
+  const long long p = (long long)blockIdx.x * CO_THREADS + threadIdx.x;
+  if (p >= n) return;
+  const float* M = f.cam2world;
+  float x[3], e[3], c[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    x[a] = xyz[3 * p + a];
+    e[a] = __fsub_rn(x[a], M[4 * a + 3]);
+  }
+#pragma unroll
+  for (int b = 0; b < 3; ++b)
+    c[b] = __fadd_rn(__fadd_rn(__fmul_rn(M[b], e[0]), __fmul_rn(M[4 + b], e[1])), __fmul_rn(M[8 + b], e[2]));
+  long long i, j;
+  float dv;
+  if (f.fov360) {
+    dv = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(c[0], c[0]), __fmul_rn(c[1], c[1])), __fmul_rn(c[2], c[2])));
+    if (!(dv > 0.0f) || !isfinite(dv)) return;
+    const float pi = 3.14159265358979323846f;
+    const float phi = asinf(fminf(fmaxf(__fdiv_rn(c[1], dv), -1.0f), 1.0f));
+    const float theta = atan2f(c[0], c[2]);               // both finite, so are the quotients below
+    j = (long long)floorf(__fdiv_rn(__fmul_rn(__fadd_rn(phi, pi / 2.0f), (float)f.H), pi));
+    j = j < 0 ? 0 : (j > f.H - 1 ? f.H - 1 : j);
+    i = (long long)floorf(__fdiv_rn(__fmul_rn(__fsub_rn(theta, pi), (float)f.W), __fmul_rn(2.0f, pi))) % f.W;
+    if (i < 0) i += f.W;
+  } else {
+    if (!(c[2] < 0.0f)) return;
+    dv = -c[2];
+    const float* K = f.intrinsics;
+    const float u = floorf(__fadd_rn(__fmul_rn(__fdiv_rn(c[0], dv), K[0]), K[1]));
+    const float v = floorf(__fadd_rn(__fmul_rn(__fdiv_rn(-c[1], dv), K[0]), K[2]));
+    if (!(u >= 0.0f && (double)u < (double)f.W && v >= 0.0f && (double)v < (double)f.H)) return;
+    i = (long long)u;
+    j = (long long)v;
+  }
+  const long long k = j * f.W + i;
+  const float acc = f.acc[k];
+  const float s = __fdiv_rn(f.depth[k], acc);
+  if (!(acc >= f.min_acc && acc > 0.0f && isfinite(s) && s > 0.0f &&
+        fabsf(__fsub_rn(dv, s)) <= __fmul_rn(f.depth_tol, s)))
+    return;
+  float w = 1.0f;
+  if (normals) {
+    float t[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) t[a] = __fsub_rn(M[4 * a + 3], x[a]);
+    const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(t[0], t[0]), __fmul_rn(t[1], t[1])), __fmul_rn(t[2], t[2])));
+    const float* nv = normals + 3 * p;
+    w = __fdiv_rn(__fadd_rn(__fadd_rn(__fmul_rn(nv[0], t[0]), __fmul_rn(nv[1], t[1])), __fmul_rn(nv[2], t[2])), len);
+    if (!(w >= f.min_cos)) return;
+  }
+  const float* px = f.image + 3 * k;
+  const float r = px[0], g = px[1], b = px[2];
+  if (!isfinite(r) || !isfinite(g) || !isfinite(b)) return;
+  const unsigned long long q = __float2uint_rz(__fmul_rn(fminf(w, 1.0f), 65536.0f));
+  unsigned long long* v = sums + 5 * p;
+  atomicAdd(v, 1ull);
+  atomicAdd(v + 1, q);
+  atomicAdd(v + 2, q * __float2uint_rz(__fmul_rn(fminf(fmaxf(r, 0.0f), 1.0f), 16777216.0f)));
+  atomicAdd(v + 3, q * __float2uint_rz(__fmul_rn(fminf(fmaxf(g, 0.0f), 1.0f), 16777216.0f)));
+  atomicAdd(v + 4, q * __float2uint_rz(__fmul_rn(fminf(fmaxf(b, 0.0f), 1.0f), 16777216.0f)));
+}
+
+__global__ void __launch_bounds__(CO_THREADS) colour_extract_kernel(const unsigned long long* __restrict__ sums,
+                                                                    long long n, unsigned char* rgb, int* count) {
+  const long long p = (long long)blockIdx.x * CO_THREADS + threadIdx.x;
+  if (p >= n) return;
+  const unsigned long long* v = sums + 5 * p;
+  const unsigned long long views = v[0], q = v[1];
+  count[p] = views < 2147483647ull ? (int)views : 2147483647;
+  const double den = __dmul_rn(__ull2double_rn(q), 16777216.0);
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+    rgb[3 * p + a] = q == 0 ? 0 : (unsigned char)floor(__dadd_rn(__dmul_rn(__ddiv_rn(__ull2double_rn(v[2 + a]), den),
+                                                                            255.0), 0.5));
+}
+
 // sort input: the key of every slot holding at least min_count points, NO_KEY (sorted last) for the others
 __global__ void __launch_bounds__(EX_THREADS) voxel_keys_kernel(const LrfVoxelTable t, unsigned long long min_count,
                                                                 unsigned long long* keys, unsigned int* slots) {
@@ -191,6 +278,21 @@ cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, 
   if (f.n_rays == 0) return cudaSuccess;
   const unsigned blocks = (unsigned)((f.n_rays + PT_THREADS - 1) / PT_THREADS);
   frame_points_kernel<<<blocks, PT_THREADS, 0, stream>>>(f, t);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_frame_colours(const LrfColourFrame& f, const float* xyz, const float* normals, long long n,
+                                 unsigned long long* sums, cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  frame_colours_kernel<<<(unsigned)((n + CO_THREADS - 1) / CO_THREADS), CO_THREADS, 0, stream>>>(f, xyz, normals, n,
+                                                                                               sums);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_colour_extract(const unsigned long long* sums, long long n, unsigned char* rgb, int* count,
+                                  cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  colour_extract_kernel<<<(unsigned)((n + CO_THREADS - 1) / CO_THREADS), CO_THREADS, 0, stream>>>(sums, n, rgb, count);
   return cudaGetLastError();
 }
 

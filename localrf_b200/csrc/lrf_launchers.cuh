@@ -136,6 +136,10 @@ cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, 
 cudaError_t voxel_extract_scratch_bytes(long long cap, size_t& bytes);
 cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, float* xyz, unsigned char* rgb,
                                  int* count, long long* n_out, void* scratch, cudaStream_t stream);
+cudaError_t launch_frame_colours(const LrfColourFrame& f, const float* xyz, const float* normals, long long n,
+                                 unsigned long long* sums, cudaStream_t stream);
+cudaError_t launch_colour_extract(const unsigned long long* sums, long long n, unsigned char* rgb, int* count,
+                                  cudaStream_t stream);
 
 // lrf_mesh.cu
 cudaError_t launch_mesh_lattice(const MeshSceneDev& S, const int* lo, const int* dims, float* values,

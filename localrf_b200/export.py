@@ -16,9 +16,17 @@ read from the field whose centre is nearest, so overlapping fields give one surf
 
     m = mesh(local_tensorfs)
     write_ply("mesh.ply", m["xyz"], m["rgb"], faces=m["faces"], normals=m["normals"])
+
+Colours of any such points from the video's own frames: each point projected into the rendered views that see it,
+tested against the view's rendered depth, and the frame's pixels blended on the device as integer sums
+(include/localrf_b200.h, lrf_frame_colours / lrf_colour_extract):
+
+    fc = frame_colours(local_tensorfs, m["xyz"], frames, normals=m["normals"])
+    rgb = torch.where(fc["count"][:, None] > 0, fc["rgb"], m["rgb"])
 """
 import ctypes as C
 import math
+import operator
 
 import numpy as np
 import torch
@@ -77,6 +85,37 @@ def _mesh_table(capacity, max_triangles, dev):
     return table, store
 
 
+def _chunk_rays(lt, weights_budget, dev):
+    """(S, rays per chunk): S the longest eval distance table of the fields (`TensorBase.sample_table`, the weights
+    each ray's render writes), and the most rays whose weights fit in `weights_budget` bytes (ValueError below one)."""
+    S = max(rf.sample_table(False, -1, dev).numel() for rf in lt.tensorfs)
+    per_chunk = int(weights_budget) // (4 * S)
+    if per_chunk < 1:
+        raise ValueError(f"weights_budget must hold one ray's weights ({4 * S} bytes)")
+    return S, per_chunk
+
+
+def _render_view(lt, v, W, H, test, per_chunk, ids, weights, dev, frame=None):
+    """The eval render of view `v` at W x H (forward's render with its per-sample weights into `weights`, then
+    lrf_ray_opacity's blended opacity) in chunks of at most `per_chunk` rays, ray r = ids[r] (`ids` an int64 arange of
+    at least W H on `dev`).  Yields (first ray, plan, rgb, depth, acc, directions) per chunk: fresh tensors, or rows of
+    frame = (rgb [W H, 3], depth [W H], acc [W H]) when given.  Yields nothing when no field renders the view."""
+    n = W * H
+    for lo in range(0, n, per_chunk):
+        m = min(per_chunk, n - lo)
+        plan = lt._eval_plan(v, m, W, H, test, dev)
+        if plan is None:
+            return
+        if frame is None:
+            outs = lt._alloc_outputs(m, dev, None, None)
+            acc = torch.empty(m, dtype=torch.float32, device=dev)
+        else:
+            outs = lt._alloc_outputs(m, dev, None, (frame[0][lo:lo + m], frame[1][lo:lo + m]))
+            acc = frame[2][lo:lo + m]
+        rgb, depth, dirs, _ = lt._run_weights(plan, ids.data_ptr() + 8 * lo, outs, weights, acc)
+        yield lo, plan, rgb, depth, acc, dirs
+
+
 def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 / 256, origin=(0, 0, 0), min_acc=0.5,
                 max_norm=1.0, min_count=1, capacity=1 << 24, weights_budget=256 << 20, _frames=None):
     """Renders every view of `view_ids` (default: every frame of r_c2w, each with its own pose and blending row) at
@@ -105,10 +144,7 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
     W, H = int(W), int(H)
     if W < 1 or H < 1:
         raise ValueError(f"W and H must be >= 1 (got W={W}, H={H})")
-    S = max(rf.sample_table(False, -1, dev).numel() for rf in lt.tensorfs)
-    per_chunk = int(weights_budget) // (4 * S)
-    if per_chunk < 1:
-        raise ValueError(f"weights_budget must hold one ray's weights ({4 * S} bytes)")
+    S, per_chunk = _chunk_rays(lt, weights_budget, dev)
     n = W * H
     per_chunk = min(per_chunk, n)
     capacity = _table_capacity(capacity)
@@ -125,14 +161,8 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
     with torch.no_grad(), torch.cuda.device(dev):
         stream = _stream(dev)
         for v in views:
-            for lo in range(0, n, per_chunk):
-                m = min(per_chunk, n - lo)
-                plan = lt._eval_plan(v, m, W, H, v in tests, dev)
-                if plan is None:
-                    break
-                outs = lt._alloc_outputs(m, dev, None, None)
-                acc = torch.empty(m, dtype=torch.float32, device=dev)
-                rgb, depth, dirs, _ = lt._run_weights(plan, ids.data_ptr() + 8 * lo, outs, weights, acc)
+            for lo, plan, rgb, depth, acc, dirs in _render_view(lt, v, W, H, v in tests, per_chunk, ids, weights, dev):
+                m = acc.numel()
                 f = _lib.LrfPointFrame(n_rays=m, rgb=rgb.data_ptr(), depth=depth.data_ptr(), acc=acc.data_ptr(),
                                        directions=dirs.data_ptr(), cam2world=plan.keep[0].data_ptr(),
                                        world2rf=w2rf.data_ptr(), blend=blend_rows[v].data_ptr(), n_fields=n_fields,
@@ -266,6 +296,111 @@ def _mesh_colours(lt, xyz, normals, owner, w2rf):
         c = rf.renderModule(None, view[sel], rf.compute_appfeature(x), bool(lt.is_refining))
         rgb[sel] = torch.floor(255 * c + 0.5).clamp(0, 255).to(torch.uint8)
     return rgb
+
+
+def _points_arg(a, name, dev):
+    """`a` ([P, 3] float32, a tensor on any device or a numpy array, P < 2^31) as a contiguous tensor on `dev`."""
+    t = torch.from_numpy(a) if isinstance(a, np.ndarray) else a
+    if not torch.is_tensor(t) or t.dtype != torch.float32 or t.dim() != 2 or t.shape[1] != 3 or t.shape[0] >= 1 << 31:
+        raise ValueError(f"{name} must be a [P, 3] float32 tensor or array with P < 2^31")
+    return t.detach().to(dev).contiguous()
+
+
+def _frame_image(image, dev):
+    """A frame's image ([h, w, 3] float32: a numpy array, a pinned tensor or a tensor on `dev`) as a contiguous tensor
+    on `dev`, enqueued on the current stream without blocking: arrays are staged through pinned memory (the caching
+    host allocator keeps each staging block until its copy has run)."""
+    host = isinstance(image, np.ndarray)
+    shape = image.shape if host or torch.is_tensor(image) else None
+    dtype_ok = (image.dtype == np.float32) if host else (torch.is_tensor(image) and image.dtype == torch.float32)
+    if (not dtype_ok or len(shape) != 3 or shape[2] != 3 or shape[0] < 1 or shape[1] < 1
+            or shape[0] * shape[1] >= 1 << 31):
+        raise ValueError("each frame's image must be [h, w, 3] float32 (a numpy array or a tensor) with w h < 2^31")
+    if host:
+        staged = torch.empty(shape, dtype=torch.float32, pin_memory=True)
+        staged.numpy()[...] = image
+        return staged.to(dev, non_blocking=True)
+    if image.is_cuda:
+        if image.device != dev:
+            raise ValueError(f"a CUDA image must be on the scene's device ({dev})")
+        return image.contiguous()
+    if not image.is_pinned():
+        raise ValueError("a host tensor image must be pinned (page-locked); pass a numpy array to have it staged")
+    return image.to(dev, non_blocking=True).contiguous()
+
+
+def frame_colours(local_tensorfs, xyz, frames, normals=None, min_acc=0.5, depth_tol=0.02, min_cos=0.1,
+                  weights_budget=256 << 20):
+    """Colours of the points `xyz` [P, 3] (world frame of get_cam2world(): a mesh's vertices, a cloud's points) from the
+    video's frames.  `frames` is an iterable of (view, image): `view` indexes r_c2w and `image` is that frame's photo,
+    [h, w, 3] float32 RGB in [0, 1] (a numpy array, a pinned tensor or a CUDA tensor).  Each view renders through the
+    eval path at its image's size (focal(w) and center(w, h) as forward scales them), in chunks of at most
+    weights_budget / (4 S) rays as in point_cloud, and each point it sees takes the pixel it projects to
+    (lrf_frame_colours): the point must lie within `depth_tol` (relative) of the pixel's normalised expected depth
+    depth / acc, and the pixel's acc must be >= `min_acc`.  With `normals` [P, 3] a view's pixel is weighted by the
+    cosine between the normal and the direction to the camera, and a view with cosine below `min_cos` does not count;
+    without them every view that passes the depth test weighs 1.  Views no field renders add nothing.
+
+    -> dict(rgb [P,3] uint8 (the weighted mean of the pixels, floor(255 c + 0.5); 0 where no view counted),
+    count [P] int32 (the views that coloured each point), n_rays (rays rendered)); rgb and count are CUDA tensors,
+    bitwise the same whatever the frame order.  A malformed xyz or normals or an option out of range raises ValueError
+    before any launch; each (view, image) pair is checked before its view renders, and a malformed one (a view outside
+    r_c2w, an image of the wrong shape, type or device) raises ValueError.  Nothing is read back from the device; host
+    images do not block the loop."""
+    lt = local_tensorfs
+    dev = _cuda_device(lt)
+    xyz = _points_arg(xyz, "xyz", dev)
+    P = xyz.shape[0]
+    if normals is not None:
+        normals = _points_arg(normals, "normals", dev)
+        if normals.shape[0] != P:
+            raise ValueError("normals must have one row per point of xyz")
+    min_acc, depth_tol, min_cos = float(min_acc), float(depth_tol), float(min_cos)
+    if math.isnan(min_acc):
+        raise ValueError("min_acc must not be NaN")
+    if not (depth_tol > 0 and math.isfinite(depth_tol)):
+        raise ValueError("depth_tol must be > 0 and finite")
+    if not 0 < min_cos <= 1:
+        raise ValueError("min_cos must lie in (0, 1]")
+    S, per_chunk = _chunk_rays(lt, weights_budget, dev)
+    n_views = len(lt.r_c2w)
+    fov360 = int(lt.fov == 360)
+    lib = _lib.lib()
+    sums = torch.zeros(P, 5, dtype=torch.int64, device=dev)
+    ids = torch.empty(0, dtype=torch.int64, device=dev)
+    weights = torch.empty(0, dtype=torch.float32, device=dev)
+    n_rays = 0
+    with torch.no_grad(), torch.cuda.device(dev):
+        stream = _stream(dev)
+        for view, image in frames:
+            view = operator.index(view)
+            if not 0 <= view < n_views:
+                raise ValueError(f"view {view} lies outside r_c2w (0 <= view < {n_views})")
+            image = _frame_image(image, dev)
+            h, w = image.shape[0], image.shape[1]
+            n = w * h
+            chunk = min(per_chunk, n)
+            if ids.numel() < n:
+                ids = torch.arange(n, dtype=torch.int64, device=dev)
+            if weights.numel() < chunk * S:
+                weights = torch.empty(chunk * S, dtype=torch.float32, device=dev)
+            rendered = tuple(torch.empty(shape, dtype=torch.float32, device=dev) for shape in ((n, 3), n, n))
+            plan = None
+            for _, plan, *_ in _render_view(lt, view, w, h, False, chunk, ids, weights, dev, rendered):
+                pass
+            if plan is None:
+                continue
+            n_rays += n
+            f = _lib.LrfColourFrame(W=w, H=h, fov360=fov360, intrinsics=plan.keep[1].data_ptr(),
+                                    cam2world=plan.keep[0].data_ptr(), depth=rendered[1].data_ptr(),
+                                    acc=rendered[2].data_ptr(), image=image.data_ptr(), min_acc=min_acc,
+                                    depth_tol=depth_tol, min_cos=min_cos)
+            n_ptr = None if normals is None else normals.data_ptr()
+            _lib.check(lib.lrf_frame_colours(C.byref(f), xyz.data_ptr(), n_ptr, P, sums.data_ptr(), stream))
+        rgb = torch.empty(P, 3, dtype=torch.uint8, device=dev)
+        count = torch.empty(P, dtype=torch.int32, device=dev)
+        _lib.check(lib.lrf_colour_extract(sums.data_ptr(), P, rgb.data_ptr(), count.data_ptr(), stream))
+    return dict(rgb=rgb, count=count, n_rays=n_rays)
 
 
 def write_ply(path, xyz, rgb, faces=None, normals=None):
