@@ -704,7 +704,8 @@ typedef struct LrfColourFrame {
  *      finite, s > 0 and |d_v - s| <= depth_tol s.
  *   5. weight: w = 1 when normals is NULL; else w = ((n_0 e_0 + n_1 e_1) + n_2 e_2) / sqrt((e_0 e_0 + e_1 e_1) + e_2 e_2)
  *      with e = t - p, and the point needs w >= min_cos (a zero normal never passes).
- *   6. a pixel with a non-finite channel adds nothing; else q = (uint32)(min(w, 1) 2^16), c24_ch =
+ *   6. a pixel with a non-finite channel adds nothing; else q = (uint32)(min(w, 1) 2^16), and a view with q = 0
+ *      (w < 2^-16, possible when min_cos is that small) adds nothing either, the count included; else c24_ch =
  *      (uint32)(clamp(image[k][ch], 0, 1) 2^24) and sums[p] += {1, q, q c24_r, q c24_g, q c24_b} (atomics).
  * The sums are integers, so they are bitwise the same whatever the frame order or thread scheduling; w is capped at 1
  * so that each view adds at most 2^40 to a sum.  Zero sums [n][5] before the first view.  One launch, one thread per
@@ -713,9 +714,10 @@ typedef struct LrfColourFrame {
  * min_acc, a depth_tol that is not > 0 and finite, and a min_cos outside (0, 1]. */
 int lrf_frame_colours(const LrfColourFrame *frame, const float *xyz, const float *normals, int64_t n,
                       unsigned long long *sums, lrf_stream_t stream);
-/* Per point of sums [n][5]: count[p] = sums[p][0] (the views that coloured it; int32, saturated) and rgb[p][ch] =
- * (uint8)floor(sum q c24_ch / (sum q 2^24) 255 + 0.5) in fp64, rounded once; rgb is 0 where sum q is 0 (count 0
- * included).  rgb [n][3] and count [n] are device memory.  One launch, no atomics.  LRF_ERR_INVALID before any device
+/* Per point of sums [n][5], with Q = sum q and S_ch = sum q c24_ch: count[p] = sums[p][0] (the views that gave the point
+ * a positive weight; int32, saturated) and rgb[p][ch] = floor(255 S_ch / (Q 2^24) + 1/2) exactly, computed as the
+ * integer quotient (510 S_ch + Q 2^24) / (Q 2^25) in 128 bits.  It is at most 255 for sums lrf_frame_colours adds
+ * (S_ch <= Q 2^24) and saturates at 255 for larger hand-written S_ch; rgb is 0 where Q is 0 (count 0 included).  rgb [n][3] and count [n] are device memory.  One launch, no atomics.  LRF_ERR_INVALID before any device
  * work for a NULL sums, rgb or count, n < 0 or n >= 2^31, and sums not 8-byte aligned. */
 int lrf_colour_extract(const unsigned long long *sums, int64_t n, uint8_t *rgb, int32_t *count, lrf_stream_t stream);
 

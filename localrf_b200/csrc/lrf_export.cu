@@ -14,7 +14,7 @@
 //
 // lrf_frame_colours / lrf_colour_extract colour given points (a mesh's vertices, a cloud's points) from the video's
 // frames: each point is projected into one rendered view, tested against the view's expected depth, and the frame's
-// pixel is added to the point's integer sums; the blend is fp64, rounded once.
+// pixel is added to the point's integer sums; the blend is an exact integer quotient of those sums.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -188,6 +188,7 @@ __global__ void __launch_bounds__(CO_THREADS) frame_colours_kernel(const LrfColo
   const float r = px[0], g = px[1], b = px[2];
   if (!isfinite(r) || !isfinite(g) || !isfinite(b)) return;
   const unsigned long long q = __float2uint_rz(__fmul_rn(fminf(w, 1.0f), 65536.0f));
+  if (q == 0) return;                                     // w < 2^-16 (min_cos that small): no weight, no count
   unsigned long long* v = sums + 5 * p;
   atomicAdd(v, 1ull);
   atomicAdd(v + 1, q);
@@ -203,11 +204,14 @@ __global__ void __launch_bounds__(CO_THREADS) colour_extract_kernel(const unsign
   const unsigned long long* v = sums + 5 * p;
   const unsigned long long views = v[0], q = v[1];
   count[p] = views < 2147483647ull ? (int)views : 2147483647;
-  const double den = __dmul_rn(__ull2double_rn(q), 16777216.0);
+  // rgb = floor(255 S / (Q 2^24) + 1/2) exactly: (510 S + Q 2^24) / (Q 2^25) in 128-bit integers (510 S < 2^73,
+  // Q 2^25 < 2^89); at most 255 when S <= Q 2^24, as every view's sums are, and saturated for sums written otherwise
 #pragma unroll
-  for (int a = 0; a < 3; ++a)
-    rgb[3 * p + a] = q == 0 ? 0 : (unsigned char)floor(__dadd_rn(__dmul_rn(__ddiv_rn(__ull2double_rn(v[2 + a]), den),
-                                                                            255.0), 0.5));
+  for (int a = 0; a < 3; ++a) {
+    unsigned __int128 c = 0;
+    if (q != 0) c = ((unsigned __int128)v[2 + a] * 510u + ((unsigned __int128)q << 24)) / ((unsigned __int128)q << 25);
+    rgb[3 * p + a] = (unsigned char)(c < 255u ? c : 255u);
+  }
 }
 
 // sort input: the key of every slot holding at least min_count points, NO_KEY (sorted last) for the others

@@ -341,12 +341,13 @@ def frame_colours(local_tensorfs, xyz, frames, normals=None, min_acc=0.5, depth_
     cosine between the normal and the direction to the camera, and a view with cosine below `min_cos` does not count;
     without them every view that passes the depth test weighs 1.  Views no field renders add nothing.
 
-    -> dict(rgb [P,3] uint8 (the weighted mean of the pixels, floor(255 c + 0.5); 0 where no view counted),
-    count [P] int32 (the views that coloured each point), n_rays (rays rendered)); rgb and count are CUDA tensors,
+    -> dict(rgb [P,3] uint8 (the weighted mean of the pixels, floor(255 c + 0.5), exact; 0 where no view counted),
+    count [P] int32 (the views that gave each point a positive weight), n_rays (rays rendered)); rgb and count are CUDA tensors,
     bitwise the same whatever the frame order.  A malformed xyz or normals or an option out of range raises ValueError
     before any launch; each (view, image) pair is checked before its view renders, and a malformed one (a view outside
-    r_c2w, an image of the wrong shape, type or device) raises ValueError.  Nothing is read back from the device; host
-    images do not block the loop."""
+    r_c2w, an image of the wrong shape, type or device) raises ValueError.  With no points (P = 0) the pairs are
+    checked but nothing renders (n_rays 0).  Nothing is read back from the device; host images do not block the
+    loop."""
     lt = local_tensorfs
     dev = _cuda_device(lt)
     xyz = _points_arg(xyz, "xyz", dev)
@@ -377,6 +378,8 @@ def frame_colours(local_tensorfs, xyz, frames, normals=None, min_acc=0.5, depth_
             if not 0 <= view < n_views:
                 raise ValueError(f"view {view} lies outside r_c2w (0 <= view < {n_views})")
             image = _frame_image(image, dev)
+            if P == 0:                                   # nothing to colour: the pair is checked, nothing renders
+                continue
             h, w = image.shape[0], image.shape[1]
             n = w * h
             chunk = min(per_chunk, n)
@@ -399,7 +402,8 @@ def frame_colours(local_tensorfs, xyz, frames, normals=None, min_acc=0.5, depth_
             _lib.check(lib.lrf_frame_colours(C.byref(f), xyz.data_ptr(), n_ptr, P, sums.data_ptr(), stream))
         rgb = torch.empty(P, 3, dtype=torch.uint8, device=dev)
         count = torch.empty(P, dtype=torch.int32, device=dev)
-        _lib.check(lib.lrf_colour_extract(sums.data_ptr(), P, rgb.data_ptr(), count.data_ptr(), stream))
+        if P:
+            _lib.check(lib.lrf_colour_extract(sums.data_ptr(), P, rgb.data_ptr(), count.data_ptr(), stream))
     return dict(rgb=rgb, count=count, n_rays=n_rays)
 
 
