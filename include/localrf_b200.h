@@ -789,6 +789,50 @@ int lrf_mesh_extract(const LrfMeshTable *table, float *xyz, int32_t *faces, int6
 int lrf_mesh_normals(const LrfMeshScene *scene, const float *xyz, int64_t n, float *normals, int32_t *owner,
                      lrf_stream_t stream);
 
+/* ---- connected components of an exported mesh or point cloud, to keep its large parts (floaters removed) ----------
+ * Union-find on the device with index-ordered hooking: the label of a vertex (or point) is the lowest index of its
+ * component, and sizes are integer sums, so labels and sizes are bitwise the same whatever the thread scheduling, the
+ * triangle order or the order of the indices within a triangle.  label [n] int32 and size [n] int64 are device
+ * memory; size[v] is the component's size where label[v] = v and 0 at every other v.  The entries write every
+ * output, stats included (nothing to zero first), and never synchronise the host. */
+
+/* Components of a mesh: each triangle of faces [n_triangles][3] joins its three vertices (a repeated index is legal).
+ * A triangle with an index outside [0, n_vertices) is skipped, never dereferenced, and counted in stats[0] (device,
+ * [1]).  size = the triangles of each component (a vertex no triangle uses is a component of size 0).
+ * LRF_ERR_INVALID before any device work for n_triangles or n_vertices outside [0, 2^31), NULL faces with
+ * n_triangles > 0, NULL label or size with n_vertices > 0, NULL stats, and misaligned arrays. */
+int lrf_mesh_components(const int32_t *faces, int64_t n_triangles, int64_t n_vertices, int32_t *label, int64_t *size,
+                        int64_t *stats, lrf_stream_t stream);
+/* Components of a point cloud xyz [n][3]: points in the same cell or in cells that share a face, edge or corner are
+ * connected.  A point's cell is k_a = floor((x_a - origin_a) / cell_size) (fp32, round to nearest, as
+ * lrf_frame_points' voxels), keyed (k_x + 2^20) << 42 | (k_y + 2^20) << 21 | (k_z + 2^20) in an open-addressing table
+ * keys [capacity] / first [capacity] (device scratch, contents irrelevant) that holds at most capacity / 2 cells.  A
+ * point that is not finite or whose k_a lies outside [-2^20, 2^20) stays alone and is counted in stats[1]; stats[0]
+ * counts the claimed cells, and stats[0] > capacity / 2 means the table overflowed and the outputs are incomplete.
+ * stats (device, [2]).  size = the points of each component.  LRF_ERR_INVALID before any device work for n outside
+ * [0, 2^31), NULL xyz with n > 0, a NULL or non-finite origin (host [3]), a cell_size that is not > 0 and finite, a
+ * capacity that is not a power of two in [2, 2^30], NULL or misaligned keys / first, and the output checks of
+ * lrf_mesh_components. */
+int lrf_point_components(const float *xyz, int64_t n, const float origin[3], float cell_size, unsigned long long *keys,
+                         int32_t *first, int64_t capacity, int32_t *label, int64_t *size, int64_t *stats,
+                         lrf_stream_t stream);
+/* Device scratch bytes of lrf_components_select (256-byte aligned); 0 for n outside [0, 2^31) or when the device
+ * cannot be queried. */
+size_t lrf_components_select_scratch_bytes(int64_t n);
+/* Ranks and selects the components label / size (as lrf_*_components write them) describe.  The components are ranked
+ * by size descending, ties by label ascending; rank i keeps its component when size >= min_size and, unless keep is
+ * 0, i < keep.  Device outputs: sizes_sorted [n] rows [0, counts[2]) the size of every component in rank order;
+ * new_index [n] -1 for a vertex of a dropped component, else its position among the kept vertices in their original
+ * order; rank [n] rows [0, counts[0]) the rank of each kept vertex's component, in that order; counts [4] the kept
+ * vertices, kept components, all components and the sum of the kept sizes.  Sizes above 2^31 - 1 rank as 2^31 - 1,
+ * and a vertex whose label is not a root in [0, n) is dropped.  Two CUB radix sorts and integer atomics: bitwise
+ * repeatable.  With n = 0 only counts (zeros) is written and scratch is not read.
+ * LRF_ERR_INVALID before any device work for n outside [0, 2^31), keep or min_size < 0, NULL or misaligned arrays,
+ * and scratch that is NULL, not 256-byte aligned or smaller than lrf_components_select_scratch_bytes(n). */
+int lrf_components_select(const int32_t *label, const int64_t *size, int64_t n, int64_t keep, int64_t min_size,
+                          int32_t *new_index, int32_t *rank, int64_t *sizes_sorted, int64_t *counts, void *scratch,
+                          size_t scratch_bytes, lrf_stream_t stream);
+
 /* fp32 -> bfloat16 (round to nearest even), n elements: the 16-bit copy of a channel-last plane / line
  * tensor for LrfField.grid_dtype = LRF_GRID_BF16.  dst must be 16-byte aligned when used as a grid. */
 int lrf_pack_bf16(const float *src, void *dst, int64_t n, lrf_stream_t stream);

@@ -12,7 +12,7 @@ _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_CSRC, "liblrf_b200.so")
 SOURCES = ["lrf_render.cu", "lrf_aux.cu", "lrf_grad.cu", "lrf_backward.cu", "lrf_sched.cu", "lrf_metrics.cu",
            "lrf_losses.cu", "lrf_optim.cu", "lrf_train.cu", "lrf_data.cu", "lrf_panels.cu", "lrf_ingest.cu",
-           "lrf_table.cu", "lrf_export.cu", "lrf_mesh.cu", "lrf_abi.cu"]
+           "lrf_table.cu", "lrf_export.cu", "lrf_mesh.cu", "lrf_components.cu", "lrf_abi.cu"]
 HEADERS = ["lrf_common.cuh", "lrf_device.cuh", "lrf_launch.cuh", "lrf_launchers.cuh", "lrf_reproject.cuh",
            "lrf_select.cuh", "lrf_table.cuh", os.path.join("..", "..", "include", "localrf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -177,7 +177,8 @@ EXPORTS = ["lrf_version", "lrf_sizeof", "lrf_last_error", "lrf_prepared_bytes", 
            "lrf_test_panels_scratch_bytes", "lrf_test_panels", "lrf_ingest_scratch_bytes", "lrf_ingest_frame",
            "lrf_resize_linear", "lrf_ray_opacity", "lrf_frame_points", "lrf_voxel_extract_scratch_bytes",
            "lrf_voxel_extract", "lrf_mesh_lattice", "lrf_mesh_cells", "lrf_mesh_extract_scratch_bytes",
-           "lrf_mesh_extract", "lrf_mesh_normals", "lrf_frame_colours", "lrf_colour_extract"]
+           "lrf_mesh_extract", "lrf_mesh_normals", "lrf_frame_colours", "lrf_colour_extract", "lrf_mesh_components",
+           "lrf_point_components", "lrf_components_select_scratch_bytes", "lrf_components_select"]
 
 
 def _stale():
@@ -306,6 +307,13 @@ def lib():
     L.lrf_mesh_normals.argtypes = [C.POINTER(LrfMeshScene), _vp, C.c_int64, _vp, _vp, _vp]
     L.lrf_frame_colours.argtypes = [C.POINTER(LrfColourFrame), _vp, _vp, C.c_int64, _vp, _vp]
     L.lrf_colour_extract.argtypes = [_vp, C.c_int64, _vp, _vp, _vp]
+    L.lrf_mesh_components.argtypes = [_vp, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp]
+    L.lrf_point_components.argtypes = [_vp, C.c_int64, C.c_float * 3, C.c_float, _vp, _vp, C.c_int64, _vp, _vp, _vp,
+                                       _vp]
+    L.lrf_components_select_scratch_bytes.restype = C.c_size_t
+    L.lrf_components_select_scratch_bytes.argtypes = [C.c_int64]
+    L.lrf_components_select.argtypes = [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp, _vp,
+                                        C.c_size_t, _vp]
     L.lrf_peer_barrier.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, _vp]
     L.lrf_peer_signal_wait.argtypes = [C.POINTER(_vp), C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _vp]
     for name in EXPORTS:

@@ -482,6 +482,18 @@ int check_exchange(const LrfOutputs* o) {
   return LRF_OK;
 }
 
+// a count of the lrf_*_components entries: [0, 2^31)
+bool count_ok(int64_t n) { return n >= 0 && n <= 2147483647LL; }
+
+// the label and size outputs of lrf_mesh_components / lrf_point_components and their stats
+int check_component_outputs(int64_t n, const int32_t* label, const int64_t* size, const int64_t* stats) {
+  if (n > 0 && (!label || !size)) return fail(LRF_ERR_INVALID, "label / size is NULL");
+  if (!stats) return fail(LRF_ERR_INVALID, "stats is NULL");
+  if (((uintptr_t)label & 3) || (((uintptr_t)size | (uintptr_t)stats) & 7))
+    return fail(LRF_ERR_INVALID, "label must be 4-byte and size / stats 8-byte aligned");
+  return LRF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1038,6 +1050,70 @@ int lrf_mesh_normals(const LrfMeshScene* scene, const float* xyz, int64_t n, flo
   if (n > 0 && (!xyz || !normals || !owner)) return fail(LRF_ERR_INVALID, "xyz / normals / owner is NULL");
   return cuda_status(lrf::launch_mesh_normals(S, xyz, n, normals, (int*)owner, (cudaStream_t)stream),
                      "mesh_normals_kernel");
+}
+
+int lrf_mesh_components(const int32_t* faces, int64_t n_triangles, int64_t n_vertices, int32_t* label, int64_t* size,
+                        int64_t* stats, lrf_stream_t stream) {
+  if (!count_ok(n_triangles) || !count_ok(n_vertices))
+    return fail(LRF_ERR_INVALID, "n_triangles and n_vertices must lie in [0, 2^31)");
+  if (n_triangles > 0 && (!faces || ((uintptr_t)faces & 3)))
+    return fail(LRF_ERR_INVALID, "faces must be non-NULL and 4-byte aligned");
+  const int rc = check_component_outputs(n_vertices, label, size, stats);
+  if (rc != LRF_OK) return rc;
+  return cuda_status(lrf::launch_mesh_components((const int*)faces, n_triangles, n_vertices, (int*)label,
+                                                 (unsigned long long*)size, (unsigned long long*)stats,
+                                                 (cudaStream_t)stream), "mesh_components");
+}
+
+int lrf_point_components(const float* xyz, int64_t n, const float origin[3], float cell_size, unsigned long long* keys,
+                         int32_t* first, int64_t capacity, int32_t* label, int64_t* size, int64_t* stats,
+                         lrf_stream_t stream) {
+  if (!count_ok(n)) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
+  if (n > 0 && (!xyz || ((uintptr_t)xyz & 3))) return fail(LRF_ERR_INVALID, "xyz must be non-NULL and 4-byte aligned");
+  if (!origin) return fail(LRF_ERR_INVALID, "origin is NULL");
+  if (!std::isfinite(origin[0]) || !std::isfinite(origin[1]) || !std::isfinite(origin[2]))
+    return fail(LRF_ERR_INVALID, "origin must be finite");
+  if (!positive_finite(cell_size)) return fail(LRF_ERR_INVALID, "cell_size must be > 0 and finite");
+  if (!table_capacity_ok(capacity)) return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  if (!keys || !first || ((uintptr_t)keys & 7) || ((uintptr_t)first & 3))
+    return fail(LRF_ERR_INVALID, "keys must be non-NULL and 8-byte aligned, first non-NULL and 4-byte aligned");
+  const int rc = check_component_outputs(n, label, size, stats);
+  if (rc != LRF_OK) return rc;
+  return cuda_status(lrf::launch_point_components(xyz, n, origin, cell_size, keys, (int*)first, capacity, (int*)label,
+                                                  (unsigned long long*)size, (unsigned long long*)stats,
+                                                  (cudaStream_t)stream), "point_components");
+}
+
+size_t lrf_components_select_scratch_bytes(int64_t n) {
+  if (!count_ok(n)) return 0;
+  size_t bytes = 0;
+  return lrf::components_select_scratch_bytes(n, bytes) == cudaSuccess ? bytes : 0;
+}
+
+int lrf_components_select(const int32_t* label, const int64_t* size, int64_t n, int64_t keep, int64_t min_size,
+                          int32_t* new_index, int32_t* rank, int64_t* sizes_sorted, int64_t* counts, void* scratch,
+                          size_t scratch_bytes, lrf_stream_t stream) {
+  if (!count_ok(n)) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
+  if (keep < 0 || min_size < 0) return fail(LRF_ERR_INVALID, "keep and min_size must be >= 0");
+  if (!counts || ((uintptr_t)counts & 7)) return fail(LRF_ERR_INVALID, "counts must be non-NULL and 8-byte aligned");
+  if (n > 0) {
+    if (!label || !size || !new_index || !rank || !sizes_sorted)
+      return fail(LRF_ERR_INVALID, "label / size / new_index / rank / sizes_sorted is NULL");
+    if ((((uintptr_t)label | (uintptr_t)new_index | (uintptr_t)rank) & 3) ||
+        (((uintptr_t)size | (uintptr_t)sizes_sorted) & 7))
+      return fail(LRF_ERR_INVALID, "the 32-bit arrays must be 4-byte and the 64-bit arrays 8-byte aligned");
+    const char* too_small = "scratch_bytes is smaller than lrf_components_select_scratch_bytes(n)";
+    if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
+    if (scratch_bytes < lrf::components_select_buffer_bytes(n)) return fail(LRF_ERR_INVALID, "%s", too_small);
+    const int rc = check_extract_scratch(
+        scratch, scratch_bytes, [&](size_t& need) { return lrf::components_select_scratch_bytes(n, need); },
+        "components_select (sort size)", too_small);
+    if (rc != LRF_OK) return rc;
+  }
+  return cuda_status(lrf::launch_components_select((const int*)label, (const unsigned long long*)size, n, keep,
+                                                   min_size, (int*)new_index, (int*)rank, (long long*)sizes_sorted,
+                                                   (long long*)counts, scratch, (cudaStream_t)stream),
+                     "components_select");
 }
 
 size_t lrf_test_panels_scratch_bytes(int32_t W, int32_t H) {

@@ -152,4 +152,17 @@ cudaError_t launch_mesh_extract(const LrfMeshTable& t, float* xyz, int* faces, l
 cudaError_t launch_mesh_normals(const MeshSceneDev& S, const float* xyz, long long n, float* normals, int* owner,
                                 cudaStream_t stream);
 
+// lrf_components.cu
+cudaError_t launch_mesh_components(const int* faces, long long T, long long V, int* label, unsigned long long* size,
+                                   unsigned long long* stats, cudaStream_t stream);
+cudaError_t launch_point_components(const float* xyz, long long n, const float* origin, float cell_size,
+                                    unsigned long long* keys, int* first, long long cap, int* label,
+                                    unsigned long long* size, unsigned long long* stats, cudaStream_t stream);
+// the select's scratch without the sort's temporary storage (known without a device: a lower bound of the whole)
+size_t components_select_buffer_bytes(long long n);
+cudaError_t components_select_scratch_bytes(long long n, size_t& bytes);
+cudaError_t launch_components_select(const int* label, const unsigned long long* size, long long n, long long keep,
+                                     long long min_size, int* new_index, int* rank, long long* sizes_sorted,
+                                     long long* counts, void* scratch, cudaStream_t stream);
+
 }  // namespace lrf

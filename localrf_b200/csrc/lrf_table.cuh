@@ -1,5 +1,5 @@
 // lrf_table.cuh -- the open-addressing table of the geometry exports (LrfVoxelTable of lrf_export.cu, LrfMeshTable of
-// lrf_mesh.cu), keyed by 64-bit integers below ~0.
+// lrf_mesh.cu, the cell table of lrf_components.cu), keyed by 64-bit integers below ~0.
 //
 // Slot i of `keys` holds tag = key + 1, 0 while empty; a slot, once claimed by CAS, never changes.  A key's probe
 // starts at probe_start(key) & (capacity - 1) and steps by one slot, wrapping from the last to 0.  A claim counter
@@ -50,6 +50,19 @@ __device__ __forceinline__ int find_or_claim(unsigned long long* keys, long long
       return (int)slot;
     }
     if (claim_count(counter) > half) return -1;
+  }
+  return -1;
+}
+
+// The slot holding `key` in a table no thread is claiming in -> -1 when none holds it.  The table is at most half
+// full, so an empty slot ends every probe for an absent key.
+__device__ __forceinline__ int find_slot(const unsigned long long* keys, long long capacity, unsigned long long key) {
+  const unsigned long long mask = (unsigned long long)capacity - 1, tag = key + 1;
+  unsigned long long slot = probe_start(key) & mask;
+  for (long long probe = 0; probe < capacity; ++probe, slot = (slot + 1) & mask) {
+    const unsigned long long cur = __ldg(keys + slot);
+    if (cur == tag) return (int)slot;
+    if (cur == 0) return -1;
   }
   return -1;
 }

@@ -23,6 +23,12 @@ tested against the view's rendered depth, and the frame's pixels blended on the 
 
     fc = frame_colours(local_tensorfs, m["xyz"], frames, normals=m["normals"])
     rgb = torch.where(fc["count"][:, None] > 0, fc["rgb"], m["rgb"])
+
+Floaters removed: the mesh's or cloud's connected components found on the device (include/localrf_b200.h,
+lrf_mesh_components / lrf_point_components / lrf_components_select), and only the large ones kept:
+
+    clean = keep_components(m, keep=1)                                   # mesh: size = triangles
+    clean = keep_components(cloud, min_size=50, cell_size=1 / 256)       # cloud: size = points
 """
 import ctypes as C
 import math
@@ -405,6 +411,115 @@ def frame_colours(local_tensorfs, xyz, frames, normals=None, min_acc=0.5, depth_
         if P:
             _lib.check(lib.lrf_colour_extract(sums.data_ptr(), P, rgb.data_ptr(), count.data_ptr(), stream))
     return dict(rgb=rgb, count=count, n_rays=n_rays)
+
+
+def _rows_at(pos, n):
+    """The rows r with pos[r] >= 0 ordered by pos (each of 0 .. n - 1 taken once), as int64 [n] on pos's device,
+    without a host read: row r is scattered to slot pos[r], the others to a spare slot past the end."""
+    m = pos.numel()
+    rows = torch.empty(m + 1, dtype=torch.int64, device=pos.device)
+    rows.scatter_(0, torch.where(pos >= 0, pos.long(), m), torch.arange(m, dtype=torch.int64, device=pos.device))
+    return rows[:n]
+
+
+def keep_components(geometry, keep=0, min_size=0, cell_size=None, origin=(0, 0, 0), capacity=None):
+    """The large connected parts of an exported mesh or point cloud: `geometry` is a dict as mesh() or point_cloud()
+    returns it.  With `faces`, two vertices are connected when a triangle joins them and a component's size is its
+    triangles.  Without, `cell_size` is required: each point falls in the cell floor((xyz - origin) / cell_size) (as
+    point_cloud's voxels, so cell_size = its voxel_size connects neighbouring voxels), points in the same or adjacent
+    cells (the 26 around a cell) are connected, and a component's size is its points; a point that is not finite or
+    whose cell index lies outside [-2^20, 2^20) is a component of its own.  The components are ranked by size
+    (descending, ties to the one holding the lowest row), and those with size >= `min_size` are kept, only the `keep`
+    largest of them unless keep is 0.
+
+    keep=1 keeps the largest part alone: every part of the scene not connected to it goes, separate real objects as
+    well as floaters.  Use `min_size` to drop only small debris.
+
+    -> a dict with the same keys: every tensor entry but `faces` (one row per vertex: xyz, normals, rgb, count) holds
+    the kept rows in their original order, `faces` the kept triangles in their original order with their vertex
+    indices renumbered, and other entries are copied; plus component ([V'] int32: the rank of each kept row's
+    component, 0 the largest) and sizes ([K] int64: the size of every component, kept or not, in rank order).  The
+    input is not modified.  The cell table of a cloud holds capacity / 2 cells (`capacity` a power of two; default the
+    smallest holding one cell per point, up to 2^30): more raises RuntimeError naming `capacity`.  A malformed dict
+    or option raises ValueError before any launch; a face index outside [0, V) raises ValueError.  The only host read
+    is the counts at the end."""
+    if not isinstance(geometry, dict) or "xyz" not in geometry:
+        raise ValueError("geometry must be a dict as mesh() or point_cloud() returns it, with an `xyz` entry")
+    xyz = geometry["xyz"]
+    if (not torch.is_tensor(xyz) or not xyz.is_cuda or xyz.dtype != torch.float32 or xyz.dim() != 2
+            or xyz.shape[1] != 3 or xyz.shape[0] >= 1 << 31):
+        raise ValueError("geometry['xyz'] must be a [V, 3] float32 CUDA tensor with V < 2^31")
+    dev, V = xyz.device, xyz.shape[0]
+    for k, v in geometry.items():
+        if k not in ("faces", "sizes") and torch.is_tensor(v) and (v.dim() < 1 or v.shape[0] != V or v.device != dev):
+            raise ValueError(f"geometry[{k!r}] must have one row per vertex of xyz, on its device")
+    keep, min_size = operator.index(keep), operator.index(min_size)
+    if keep < 0 or min_size < 0:
+        raise ValueError("keep and min_size must be >= 0")
+    faces = geometry.get("faces")
+    if faces is not None:
+        if cell_size is not None:
+            raise ValueError("cell_size is for a point cloud; a mesh is connected by its faces")
+        if (not torch.is_tensor(faces) or faces.device != dev or faces.dtype != torch.int32 or faces.dim() != 2
+                or faces.shape[1] != 3 or faces.shape[0] >= 1 << 31):
+            raise ValueError("geometry['faces'] must be a [T, 3] int32 tensor on the device of xyz with T < 2^31")
+        faces = faces.contiguous()
+    else:
+        if cell_size is None:
+            raise ValueError("a point cloud (a dict without `faces`) needs cell_size")
+        cell_size = float(cell_size)
+        if not (cell_size > 0 and math.isfinite(cell_size)):
+            raise ValueError("cell_size must be > 0 and finite")
+        origin = [float(v) for v in origin]
+        if len(origin) != 3 or not all(math.isfinite(v) for v in origin):
+            raise ValueError("origin must be three finite numbers")
+        if capacity is None:
+            capacity = min(max(2, 1 << (2 * V - 1).bit_length()), 1 << 30)
+        capacity = _table_capacity(capacity)
+    lib = _lib.lib()
+    with torch.no_grad(), torch.cuda.device(dev):
+        stream = _stream(dev)
+        xyz = xyz.contiguous()
+        label = torch.empty(V, dtype=torch.int32, device=dev)
+        size = torch.empty(V, dtype=torch.int64, device=dev)
+        tail = torch.zeros(6, dtype=torch.int64, device=dev)         # counts (4), stats (2)
+        if faces is not None:
+            _lib.check(lib.lrf_mesh_components(faces.data_ptr(), faces.shape[0], V, label.data_ptr(), size.data_ptr(),
+                                               tail.data_ptr() + 32, stream))
+        else:
+            keys = torch.empty(capacity, dtype=torch.int64, device=dev)
+            first = torch.empty(capacity, dtype=torch.int32, device=dev)
+            _lib.check(lib.lrf_point_components(xyz.data_ptr(), V, (C.c_float * 3)(*origin), cell_size, keys.data_ptr(),
+                                                first.data_ptr(), capacity, label.data_ptr(), size.data_ptr(),
+                                                tail.data_ptr() + 32, stream))
+            del keys, first
+        scratch_bytes = lib.lrf_components_select_scratch_bytes(V) if V else 0
+        scratch = _extract_scratch(scratch_bytes, "component select", dev) if V else None
+        new_index = torch.empty(V, dtype=torch.int32, device=dev)
+        rank = torch.empty(V, dtype=torch.int32, device=dev)
+        sizes = torch.empty(V, dtype=torch.int64, device=dev)
+        _lib.check(lib.lrf_components_select(label.data_ptr(), size.data_ptr(), V, keep, min_size, new_index.data_ptr(),
+                                             rank.data_ptr(), sizes.data_ptr(), tail.data_ptr(),
+                                             None if scratch is None else scratch.data_ptr(), scratch_bytes, stream))
+        del scratch
+        n_rows, _, n_comp, kept_size, stat0, _ = tail.tolist()
+        if faces is not None and stat0:
+            raise ValueError(f"geometry['faces'] has {stat0} triangles with a vertex index outside [0, {V})")
+        if faces is None and stat0 > capacity // 2:
+            raise RuntimeError(f"localrf_b200: the cloud has more cells than the table holds (capacity / 2 = "
+                               f"{capacity // 2}); raise `capacity` or `cell_size`")
+        rows = _rows_at(new_index, n_rows)
+        out = {}
+        for k, v in geometry.items():
+            if k == "faces":
+                remapped = new_index[faces.long()]
+                kept = remapped[:, 0] >= 0
+                out[k] = remapped[_rows_at(torch.where(kept, torch.cumsum(kept, 0) - 1, -1), kept_size)]
+            elif k != "sizes":
+                out[k] = v[rows] if torch.is_tensor(v) else v
+        out["component"] = rank[:n_rows].clone()
+        out["sizes"] = sizes[:n_comp].clone()
+    return out
 
 
 def write_ply(path, xyz, rgb, faces=None, normals=None):
