@@ -240,9 +240,12 @@ int check_views(long long n_rays, long long n_views, bool allow_empty) {
                                            : "n_rays must be a positive multiple of n_views");
 }
 
-// the ray count of a kernel that indexes rays with 32-bit integers
+// a count of items the kernels index with 32-bit integers: [0, 2^31)
+bool count_ok(int64_t n) { return n >= 0 && n <= 2147483647LL; }
+
+// the ray count of a kernel that indexes rays with 32-bit integers (the callers have refused negative counts)
 int check_31_bits(long long n_rays) {
-  return n_rays > 2147483647LL ? fail(LRF_ERR_INVALID, "n_rays must fit 31 bits") : LRF_OK;
+  return count_ok(n_rays) ? LRF_OK : fail(LRF_ERR_INVALID, "n_rays must fit 31 bits");
 }
 
 // validates a batch of n_rays >= 1 -- its split into views when `per_view`, n_rays < 2^31 when `fit_31`, and in
@@ -363,25 +366,38 @@ bool table_capacity_ok(int64_t capacity) {
   return capacity >= 2 && capacity <= (1LL << 30) && !(capacity & (capacity - 1));
 }
 
-// the scratch block of lrf_voxel_extract and lrf_mesh_extract: non-NULL and 256-byte aligned, then (the sort-size query
-// needs a device, so after those checks) at least the bytes need(bytes) reports; `where` names a failed query
-template <typename Need>
-int check_extract_scratch(const void* scratch, size_t bytes, Need need, const char* where, const char* too_small) {
+int check_capacity(int64_t capacity) {
+  return table_capacity_ok(capacity) ? LRF_OK : fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+}
+
+// the origin of an export's lattice or cell grid
+int check_origin(const float origin[3]) {
+  if (!std::isfinite(origin[0]) || !std::isfinite(origin[1]) || !std::isfinite(origin[2]))
+    return fail(LRF_ERR_INVALID, "origin must be finite");
+  return LRF_OK;
+}
+
+// an extract's scratch block: non-NULL and 256-byte aligned, at least its buffers (known without a device), then at
+// least the whole block (the sort-size query needs a device); `where` names a failed query
+int check_extract_scratch(const void* scratch, size_t bytes, const lrf::ExtractScratch& x, const char* where,
+                          const char* too_small) {
   if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
-  size_t n = 0;
-  const cudaError_t e = need(n);
+  size_t need = 0;
+  x.bytes(need, false);
+  if (bytes < need) return fail(LRF_ERR_INVALID, "%s", too_small);
+  const cudaError_t e = x.bytes(need, true);
   if (e != cudaSuccess) return cuda_fail(e, where);
-  if (bytes < n) return fail(LRF_ERR_INVALID, "%s", too_small);
+  if (bytes < need) return fail(LRF_ERR_INVALID, "%s", too_small);
   return LRF_OK;
 }
 
 // the voxel table of lrf_frame_points and lrf_voxel_extract
 int check_voxel_table(const LrfVoxelTable* t) {
   if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
-  if (!table_capacity_ok(t->capacity)) return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  int rc = check_capacity(t->capacity);
+  if (rc != LRF_OK) return rc;
   if (!(t->voxel_size > 0.0f) || !std::isfinite(t->voxel_size)) return fail(LRF_ERR_INVALID, "voxel_size must be > 0 and finite");
-  if (!std::isfinite(t->origin[0]) || !std::isfinite(t->origin[1]) || !std::isfinite(t->origin[2]))
-    return fail(LRF_ERR_INVALID, "origin must be finite");
+  if ((rc = check_origin(t->origin)) != LRF_OK) return rc;
   if (!t->keys || !t->sums || !t->stats) return fail(LRF_ERR_INVALID, "keys / sums / stats of the table is NULL");
   if (((uintptr_t)t->keys | (uintptr_t)t->sums | (uintptr_t)t->stats) & 7)
     return fail(LRF_ERR_INVALID, "keys / sums / stats of the table must be 8-byte aligned");
@@ -402,11 +418,10 @@ int make_mesh_scene(const LrfMeshScene* s, lrf::MeshSceneDev& S) {
   if (!positive_finite(s->voxel_size)) return fail(LRF_ERR_INVALID, "voxel_size must be > 0 and finite");
   if (!positive_finite(s->max_norm)) return fail(LRF_ERR_INVALID, "max_norm must be > 0 and finite");
   if (!positive_finite(s->level)) return fail(LRF_ERR_INVALID, "level must be > 0 and finite");
-  if (!std::isfinite(s->origin[0]) || !std::isfinite(s->origin[1]) || !std::isfinite(s->origin[2]))
-    return fail(LRF_ERR_INVALID, "origin must be finite");
+  int rc = check_origin(s->origin);
+  if (rc != LRF_OK) return rc;
   for (int k = 0; k < s->n_fields; ++k) {
-    const int rc = make_field(s->fields + k, false, false, nullptr, S.f[k]);
-    if (rc != LRF_OK) return rc;
+    if ((rc = make_field(s->fields + k, false, false, nullptr, S.f[k])) != LRF_OK) return rc;
     if (!positive_finite(s->step_size[k])) return fail(LRF_ERR_INVALID, "step_size must be > 0 and finite");
     S.length[k] = s->step_size[k];
   }
@@ -435,7 +450,8 @@ int check_brick(const int32_t lo[3], const int32_t dims[3]) {
 // the edge and triangle table of lrf_mesh_cells and lrf_mesh_extract
 int check_mesh_table(const LrfMeshTable* t) {
   if (!t) return fail(LRF_ERR_INVALID, "table is NULL");
-  if (!table_capacity_ok(t->capacity)) return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  const int rc = check_capacity(t->capacity);
+  if (rc != LRF_OK) return rc;
   if (t->max_triangles < 1 || t->max_triangles > 2147483647LL)
     return fail(LRF_ERR_INVALID, "max_triangles must be in [1, 2^31)");
   if (!t->keys || !t->verts || !t->tri_keys || !t->tri_slots || !t->stats)
@@ -481,9 +497,6 @@ int check_exchange(const LrfOutputs* o) {
   }
   return LRF_OK;
 }
-
-// a count of the lrf_*_components entries: [0, 2^31)
-bool count_ok(int64_t n) { return n >= 0 && n <= 2147483647LL; }
 
 // the label and size outputs of lrf_mesh_components / lrf_point_components and their stats
 int check_component_outputs(int64_t n, const int32_t* label, const int64_t* size, const int64_t* stats) {
@@ -936,7 +949,7 @@ int lrf_frame_points(const LrfPointFrame* f, const LrfVoxelTable* t, lrf_stream_
   if (!f) return fail(LRF_ERR_INVALID, "frame is NULL");
   int rc = check_voxel_table(t);
   if (rc != LRF_OK) return rc;
-  if (f->n_rays < 0 || f->n_rays > 2147483647LL) return fail(LRF_ERR_INVALID, "n_rays must lie in [0, 2^31)");
+  if (!count_ok(f->n_rays)) return fail(LRF_ERR_INVALID, "n_rays must lie in [0, 2^31)");
   if (f->n_fields < 1) return fail(LRF_ERR_INVALID, "n_fields must be >= 1");
   if (!f->rgb || !f->depth || !f->acc || !f->directions || !f->cam2world || !f->world2rf)
     return fail(LRF_ERR_INVALID, "rgb / depth / acc / directions / cam2world / world2rf of the frame is NULL");
@@ -947,7 +960,7 @@ int lrf_frame_points(const LrfPointFrame* f, const LrfVoxelTable* t, lrf_stream_
 size_t lrf_voxel_extract_scratch_bytes(int64_t capacity) {
   if (!table_capacity_ok(capacity)) return 0;
   size_t bytes = 0;
-  return lrf::voxel_extract_scratch_bytes(capacity, bytes) == cudaSuccess ? bytes : 0;
+  return lrf::voxel_extract_scratch(capacity).bytes(bytes, true) == cudaSuccess ? bytes : 0;
 }
 
 int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uint8_t* rgb, int32_t* count,
@@ -956,8 +969,7 @@ int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uin
   if (rc != LRF_OK) return rc;
   if (min_count < 1) return fail(LRF_ERR_INVALID, "min_count must be >= 1");
   if (!xyz || !rgb || !count || !n_voxels) return fail(LRF_ERR_INVALID, "xyz / rgb / count / n_voxels is NULL");
-  rc = check_extract_scratch(scratch, scratch_bytes,
-                             [&](size_t& need) { return lrf::voxel_extract_scratch_bytes(t->capacity, need); },
+  rc = check_extract_scratch(scratch, scratch_bytes, lrf::voxel_extract_scratch(t->capacity),
                              "voxel_extract (sort size)",
                              "scratch_bytes is smaller than lrf_voxel_extract_scratch_bytes(capacity)");
   if (rc != LRF_OK) return rc;
@@ -967,7 +979,7 @@ int lrf_voxel_extract(const LrfVoxelTable* t, int64_t min_count, float* xyz, uin
 
 // the point count and sums of lrf_frame_colours and lrf_colour_extract
 int check_colour_sums(const unsigned long long* sums, int64_t n) {
-  if (n < 0 || n > 2147483647LL) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
+  if (!count_ok(n)) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
   if (!sums || ((uintptr_t)sums & 7)) return fail(LRF_ERR_INVALID, "sums must be non-NULL and 8-byte aligned");
   return LRF_OK;
 }
@@ -1020,10 +1032,9 @@ int lrf_mesh_cells(const LrfMeshScene* scene, const int32_t lo[3], const int32_t
 }
 
 size_t lrf_mesh_extract_scratch_bytes(int64_t capacity, int64_t max_triangles) {
-  if (!table_capacity_ok(capacity)) return 0;
-  if (max_triangles < 1 || max_triangles > 2147483647LL) return 0;
+  if (!table_capacity_ok(capacity) || max_triangles < 1 || max_triangles > 2147483647LL) return 0;
   size_t bytes = 0;
-  return lrf::mesh_extract_scratch_bytes(capacity, max_triangles, bytes) == cudaSuccess ? bytes : 0;
+  return lrf::mesh_extract_scratch(capacity, max_triangles).bytes(bytes, true) == cudaSuccess ? bytes : 0;
 }
 
 int lrf_mesh_extract(const LrfMeshTable* table, float* xyz, int32_t* faces, int64_t* counts, void* scratch,
@@ -1031,11 +1042,9 @@ int lrf_mesh_extract(const LrfMeshTable* table, float* xyz, int32_t* faces, int6
   int rc = check_mesh_table(table);
   if (rc != LRF_OK) return rc;
   if (!xyz || !faces || !counts) return fail(LRF_ERR_INVALID, "xyz / faces / counts is NULL");
-  rc = check_extract_scratch(
-      scratch, scratch_bytes,
-      [&](size_t& need) { return lrf::mesh_extract_scratch_bytes(table->capacity, table->max_triangles, need); },
-      "mesh_extract (sort size)",
-      "scratch_bytes is smaller than lrf_mesh_extract_scratch_bytes(capacity, max_triangles)");
+  rc = check_extract_scratch(scratch, scratch_bytes, lrf::mesh_extract_scratch(table->capacity, table->max_triangles),
+                             "mesh_extract (sort size)",
+                             "scratch_bytes is smaller than lrf_mesh_extract_scratch_bytes(capacity, max_triangles)");
   if (rc != LRF_OK) return rc;
   return cuda_status(lrf::launch_mesh_extract(*table, xyz, (int*)faces, (long long*)counts, scratch,
                                               (cudaStream_t)stream), "mesh_extract");
@@ -1046,7 +1055,7 @@ int lrf_mesh_normals(const LrfMeshScene* scene, const float* xyz, int64_t n, flo
   static thread_local lrf::MeshSceneDev S;
   int rc = make_mesh_scene(scene, S);
   if (rc != LRF_OK) return rc;
-  if (n < 0 || n > 2147483647LL) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
+  if (!count_ok(n)) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
   if (n > 0 && (!xyz || !normals || !owner)) return fail(LRF_ERR_INVALID, "xyz / normals / owner is NULL");
   return cuda_status(lrf::launch_mesh_normals(S, xyz, n, normals, (int*)owner, (cudaStream_t)stream),
                      "mesh_normals_kernel");
@@ -1071,23 +1080,21 @@ int lrf_point_components(const float* xyz, int64_t n, const float origin[3], flo
   if (!count_ok(n)) return fail(LRF_ERR_INVALID, "n must lie in [0, 2^31)");
   if (n > 0 && (!xyz || ((uintptr_t)xyz & 3))) return fail(LRF_ERR_INVALID, "xyz must be non-NULL and 4-byte aligned");
   if (!origin) return fail(LRF_ERR_INVALID, "origin is NULL");
-  if (!std::isfinite(origin[0]) || !std::isfinite(origin[1]) || !std::isfinite(origin[2]))
-    return fail(LRF_ERR_INVALID, "origin must be finite");
+  int rc = check_origin(origin);
+  if (rc != LRF_OK) return rc;
   if (!positive_finite(cell_size)) return fail(LRF_ERR_INVALID, "cell_size must be > 0 and finite");
-  if (!table_capacity_ok(capacity)) return fail(LRF_ERR_INVALID, "capacity must be a power of two in [2, 2^30]");
+  if ((rc = check_capacity(capacity)) != LRF_OK) return rc;
   if (!keys || !first || ((uintptr_t)keys & 7) || ((uintptr_t)first & 3))
     return fail(LRF_ERR_INVALID, "keys must be non-NULL and 8-byte aligned, first non-NULL and 4-byte aligned");
-  const int rc = check_component_outputs(n, label, size, stats);
-  if (rc != LRF_OK) return rc;
+  if ((rc = check_component_outputs(n, label, size, stats)) != LRF_OK) return rc;
   return cuda_status(lrf::launch_point_components(xyz, n, origin, cell_size, keys, (int*)first, capacity, (int*)label,
                                                   (unsigned long long*)size, (unsigned long long*)stats,
                                                   (cudaStream_t)stream), "point_components");
 }
 
 size_t lrf_components_select_scratch_bytes(int64_t n) {
-  if (!count_ok(n)) return 0;
   size_t bytes = 0;
-  return lrf::components_select_scratch_bytes(n, bytes) == cudaSuccess ? bytes : 0;
+  return count_ok(n) && lrf::components_select_scratch(n).bytes(bytes, true) == cudaSuccess ? bytes : 0;
 }
 
 int lrf_components_select(const int32_t* label, const int64_t* size, int64_t n, int64_t keep, int64_t min_size,
@@ -1102,12 +1109,9 @@ int lrf_components_select(const int32_t* label, const int64_t* size, int64_t n, 
     if ((((uintptr_t)label | (uintptr_t)new_index | (uintptr_t)rank) & 3) ||
         (((uintptr_t)size | (uintptr_t)sizes_sorted) & 7))
       return fail(LRF_ERR_INVALID, "the 32-bit arrays must be 4-byte and the 64-bit arrays 8-byte aligned");
-    const char* too_small = "scratch_bytes is smaller than lrf_components_select_scratch_bytes(n)";
-    if (!scratch || ((uintptr_t)scratch & 255)) return fail(LRF_ERR_INVALID, "scratch is NULL or not 256-byte aligned");
-    if (scratch_bytes < lrf::components_select_buffer_bytes(n)) return fail(LRF_ERR_INVALID, "%s", too_small);
-    const int rc = check_extract_scratch(
-        scratch, scratch_bytes, [&](size_t& need) { return lrf::components_select_scratch_bytes(n, need); },
-        "components_select (sort size)", too_small);
+    const int rc = check_extract_scratch(scratch, scratch_bytes, lrf::components_select_scratch(n),
+                                         "components_select (sort size)",
+                                         "scratch_bytes is smaller than lrf_components_select_scratch_bytes(n)");
     if (rc != LRF_OK) return rc;
   }
   return cuda_status(lrf::launch_components_select((const int*)label, (const unsigned long long*)size, n, keep,

@@ -7,11 +7,11 @@
 // a component is its lowest index whatever order the threads run in.  Sizes are integer atomics at the root, so
 // labels and sizes are bitwise deterministic.
 //
-// Mesh: each triangle unites its three vertices.  Cloud: each point's cell, floor((x - origin) / cell_size) keyed as
-// lrf_frame_points keys its voxels, is claimed once in an lrf_table.cuh table whose slot keeps the cell's lowest point
-// (atomicMin); a point unites with the one its atomicMin replaced or lost to, so a cell's points form one set, and
-// each cell unites its lowest point with those of its 13 forward neighbours among the 26 (the neighbour relation is
-// symmetric, so that covers all 26).
+// Mesh: each triangle unites its three vertices.  Cloud: each point's cell, floor((x - origin) / cell_size) keyed by
+// cell_key as lrf_frame_points keys its voxels, is claimed once in an lrf_table.cuh table whose slot keeps the cell's
+// lowest point (atomicMin); a point unites with the one its atomicMin replaced or lost to, so a cell's points form one
+// set, and each cell unites its lowest point with those of its 13 forward neighbours among the 26 (the neighbour
+// relation is symmetric, so that covers all 26).
 //
 // lrf_components_select ranks the components by size (descending, ties by label) and compacts the kept vertices in
 // their original order, both with KeySlotSort.
@@ -28,12 +28,8 @@ namespace lrf {
 namespace {
 
 constexpr int CC_THREADS = 256;
-constexpr int KEY_BITS = 21;               // per axis: cells in [-2^20, 2^20), as lrf_frame_points' voxels
-constexpr float KEY_LIM = 1048576.0f;      // 2^20
 constexpr int NO_INDEX = 0x7fffffff;       // an empty cell's lowest point
 constexpr unsigned long long SIZE_MAX31 = 0x7fffffffull;
-
-unsigned int blocks_of(long long n) { return (unsigned int)((n + CC_THREADS - 1) / CC_THREADS); }
 
 // The root of v.  Path halving: v's parent becomes its grandparent (atomicMin, so a shortcut never raises a parent
 // another thread lowered), and the walk goes on from there.
@@ -144,14 +140,8 @@ __global__ void __launch_bounds__(CC_THREADS) point_cells_kernel(const float* __
   const long long p = (long long)blockIdx.x * CC_THREADS + threadIdx.x;
   bool in = false, out = false;
   unsigned long long key = 0;
-  if (p < n && claim_count(stats) <= ((unsigned long long)cap >> 1)) {
-    in = true;
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      const float k = floorf(__fdiv_rn(__fsub_rn(__ldg(xyz + 3 * p + a), g.origin[a]), g.cell));
-      in = in && k >= -KEY_LIM && k < KEY_LIM;                    // (false for NaN)
-      if (in) key = (key << KEY_BITS) | (unsigned long long)((int)k + (1 << 20));
-    }
+  if (p < n && !table_full(stats, cap)) {
+    in = cell_key(xyz + 3 * p, g.origin, g.cell, key, [](int, float, float) {});
     out = !in;
   }
   count_lanes(stats + 1, out);
@@ -167,20 +157,16 @@ __global__ void __launch_bounds__(CC_THREADS) cell_link_kernel(const unsigned lo
                                                                const int* __restrict__ first, long long cap,
                                                                const unsigned long long* stats, int* parent) {
   const long long s = (long long)blockIdx.x * CC_THREADS + threadIdx.x;
-  if (s >= cap || claim_count(stats) > ((unsigned long long)cap >> 1)) return;
+  if (s >= cap || table_full(stats, cap)) return;
   const unsigned long long tag = __ldg(keys + s);
   if (tag == 0) return;
   const int rep = __ldg(first + s);
-  const unsigned long long field = (1ull << KEY_BITS) - 1;
-  const int k[3] = {(int)(((tag - 1) >> (2 * KEY_BITS)) & field), (int)(((tag - 1) >> KEY_BITS) & field),
-                    (int)((tag - 1) & field)};
+  const int k[3] = {(int)cell_field(tag - 1, 0), (int)cell_field(tag - 1, 1), (int)cell_field(tag - 1, 2)};
   for (int o = 14; o < 27; ++o) {
     const int m[3] = {k[0] + o / 9 - 1, k[1] + (o / 3) % 3 - 1, k[2] + o % 3 - 1};
-    if ((unsigned)m[0] > (unsigned)field || (unsigned)m[1] > (unsigned)field || (unsigned)m[2] > (unsigned)field)
-      continue;
-    const unsigned long long nk = ((unsigned long long)m[0] << (2 * KEY_BITS)) |
-                                  ((unsigned long long)m[1] << KEY_BITS) | (unsigned long long)m[2];
-    const int ns = find_slot(keys, cap, nk);
+    const unsigned field = (unsigned)KEY_FIELD;
+    if ((unsigned)m[0] > field || (unsigned)m[1] > field || (unsigned)m[2] > field) continue;
+    const int ns = find_slot(keys, cap, cell_key_of(m));
     if (ns >= 0) unite(parent, rep, __ldg(first + ns));
   }
 }
@@ -257,91 +243,61 @@ __global__ void __launch_bounds__(CC_THREADS) kept_write_kernel(const unsigned l
   if (j + 1 == n || keys[j + 1] == NO_KEY) counts[0] = j + 1;
 }
 
-// The select's scratch: the sort's key and index buffers, the rank of each root, the sort's temporary storage.  With
-// a null base only the size is computed.
-struct SelectScratch {
-  KeySlotSort pairs;
-  int* comp_rank;
-  void* temp;
-  size_t temp_bytes;
-  size_t total;
-};
-
-cudaError_t select_scratch(void* base, long long n, SelectScratch& x) {
-  ScratchCarver c(base);
-  x.pairs.carve(c, n);
-  x.comp_rank = c.take<int>(n * 4, 256);
-  const cudaError_t e = KeySlotSort::temp_bytes(n, x.temp_bytes);
-  x.temp = c.take(x.temp_bytes, 256);
-  x.total = c.size(256);
-  return e;
-}
-
 }  // namespace
-
-size_t components_select_buffer_bytes(long long n) {
-  KeySlotSort pairs;
-  ScratchCarver c(nullptr);
-  pairs.carve(c, n);
-  c.take(n * 4, 256);
-  return c.size(256);
-}
 
 cudaError_t launch_mesh_components(const int* faces, long long T, long long V, int* label, unsigned long long* size,
                                    unsigned long long* stats, cudaStream_t stream) {
-  init_kernel<<<blocks_of(V > 1 ? V : 1), CC_THREADS, 0, stream>>>(label, size, V, nullptr, nullptr, 0, stats, 1);
+  init_kernel<<<item_ctas(V > 1 ? V : 1, CC_THREADS), CC_THREADS, 0, stream>>>(label, size, V, nullptr, nullptr, 0,
+                                                                               stats, 1);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || T == 0) return e;
-  mesh_link_kernel<<<blocks_of(T), CC_THREADS, 0, stream>>>(faces, T, (int)V, label, stats);
+  mesh_link_kernel<<<item_ctas(T, CC_THREADS), CC_THREADS, 0, stream>>>(faces, T, (int)V, label, stats);
   if ((e = cudaGetLastError()) != cudaSuccess || V == 0) return e;
-  label_kernel<<<blocks_of(V), CC_THREADS, 0, stream>>>(label, V, nullptr);
+  label_kernel<<<item_ctas(V, CC_THREADS), CC_THREADS, 0, stream>>>(label, V, nullptr);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  mesh_size_kernel<<<blocks_of(T), CC_THREADS, 0, stream>>>(faces, T, (int)V, label, size);
+  mesh_size_kernel<<<item_ctas(T, CC_THREADS), CC_THREADS, 0, stream>>>(faces, T, (int)V, label, size);
   return cudaGetLastError();
 }
 
 cudaError_t launch_point_components(const float* xyz, long long n, const float* origin, float cell_size,
                                     unsigned long long* keys, int* first, long long cap, int* label,
                                     unsigned long long* size, unsigned long long* stats, cudaStream_t stream) {
-  init_kernel<<<blocks_of(n > cap ? n : cap), CC_THREADS, 0, stream>>>(label, size, n, keys, first, cap, stats, 2);
+  init_kernel<<<item_ctas(n > cap ? n : cap, CC_THREADS), CC_THREADS, 0, stream>>>(label, size, n, keys, first, cap,
+                                                                                   stats, 2);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || n == 0) return e;
   const CellGrid g = {{origin[0], origin[1], origin[2]}, cell_size};
-  point_cells_kernel<<<blocks_of(n), CC_THREADS, 0, stream>>>(xyz, n, g, keys, first, cap, label, stats);
+  point_cells_kernel<<<item_ctas(n, CC_THREADS), CC_THREADS, 0, stream>>>(xyz, n, g, keys, first, cap, label, stats);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  cell_link_kernel<<<blocks_of(cap), CC_THREADS, 0, stream>>>(keys, first, cap, stats, label);
+  cell_link_kernel<<<item_ctas(cap, CC_THREADS), CC_THREADS, 0, stream>>>(keys, first, cap, stats, label);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  label_kernel<<<blocks_of(n), CC_THREADS, 0, stream>>>(label, n, size);
+  label_kernel<<<item_ctas(n, CC_THREADS), CC_THREADS, 0, stream>>>(label, n, size);
   return cudaGetLastError();
 }
 
-cudaError_t components_select_scratch_bytes(long long n, size_t& bytes) {
-  SelectScratch x;
-  const cudaError_t e = select_scratch(nullptr, n, x);
-  bytes = x.total;
-  return e;
-}
+// the sort's key and index buffers, the rank of each root, then the sort's temporary storage
+ExtractScratch components_select_scratch(long long n) { return ExtractScratch{n, n, 0}; }
 
 cudaError_t launch_components_select(const int* label, const unsigned long long* size, long long n, long long keep,
                                      long long min_size, int* new_index, int* rank, long long* sizes_sorted,
                                      long long* counts, void* scratch, cudaStream_t stream) {
   if (n == 0) return cudaMemsetAsync(counts, 0, 4 * sizeof(long long), stream);
-  SelectScratch x;
-  cudaError_t e = select_scratch(scratch, n, x);
+  ExtractScratch x = components_select_scratch(n);
+  cudaError_t e = x.carve(scratch);
   if (e != cudaSuccess) return e;
-  rank_keys_kernel<<<blocks_of(n), CC_THREADS, 0, stream>>>(label, size, n, x.pairs.keys(), x.pairs.slots(),
-                                                             x.comp_rank, counts);
+  const KeySlotSort& pairs = x.pairs[0];
+  int* comp_rank = x.index;
+  const unsigned blocks = item_ctas(n, CC_THREADS);
+  rank_keys_kernel<<<blocks, CC_THREADS, 0, stream>>>(label, size, n, pairs.keys(), pairs.slots(), comp_rank, counts);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  if ((e = x.pairs.sort(n, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
-  rank_write_kernel<<<blocks_of(n), CC_THREADS, 0, stream>>>(x.pairs.keys(), n, keep, min_size, x.comp_rank,
-                                                              sizes_sorted, counts);
+  if ((e = x.pairs[0].sort(n, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  rank_write_kernel<<<blocks, CC_THREADS, 0, stream>>>(pairs.keys(), n, keep, min_size, comp_rank, sizes_sorted,
+                                                       counts);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  kept_keys_kernel<<<blocks_of(n), CC_THREADS, 0, stream>>>(label, n, x.comp_rank, x.pairs.keys(), x.pairs.slots(),
-                                                             new_index);
+  kept_keys_kernel<<<blocks, CC_THREADS, 0, stream>>>(label, n, comp_rank, pairs.keys(), pairs.slots(), new_index);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  if ((e = x.pairs.sort(n, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
-  kept_write_kernel<<<blocks_of(n), CC_THREADS, 0, stream>>>(x.pairs.keys(), n, label, x.comp_rank, new_index, rank,
-                                                              counts);
+  if ((e = x.pairs[0].sort(n, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  kept_write_kernel<<<blocks, CC_THREADS, 0, stream>>>(pairs.keys(), n, label, comp_rank, new_index, rank, counts);
   return cudaGetLastError();
 }
 

@@ -32,8 +32,6 @@ constexpr int OP_TILE = 32;            // samples per tile staged through shared
 constexpr int PT_THREADS = 256;
 constexpr int EX_THREADS = 256;
 constexpr int CO_THREADS = 256;
-constexpr int KEY_BITS = 21;           // per axis: keys in [-2^20, 2^20), 63 bits in all
-constexpr float KEY_LIM = 1048576.0f;  // 2^20
 
 // One thread per ray sums its weights in sample order in fp64, from -0 (the identity of IEEE addition, so a row of -0
 // sums to -0 as np.cumsum does).  The [rays][S] rows are read a tile at a time, coalesced, into padded shared rows, so
@@ -66,11 +64,10 @@ __global__ void __launch_bounds__(OP_RAYS) ray_opacity_kernel(const float* __res
 // The table's claim counter is stats[2], the occupied slots.
 __global__ void __launch_bounds__(PT_THREADS) frame_points_kernel(const LrfPointFrame f, const LrfVoxelTable t) {
   const long long r = (long long)blockIdx.x * PT_THREADS + threadIdx.x;
-  const unsigned long long half = (unsigned long long)t.capacity >> 1;
   bool keep = false, out = false;
   unsigned long long key = 0, fs[3];
   unsigned int cs[3];
-  if (r < f.n_rays && claim_count(t.stats + 2) <= half) {
+  if (r < f.n_rays && !table_full(t.stats + 2, t.capacity)) {
     const float a = f.acc[r], d = f.depth[r];
     if (a >= f.min_acc && a > 0.0f && isfinite(d)) {
       const float s = __fdiv_rn(d, a);
@@ -90,21 +87,11 @@ __global__ void __launch_bounds__(PT_THREADS) frame_points_kernel(const LrfPoint
                  fabsf(__fadd_rn(p[2], o[2])) <= f.max_norm;
       }
       if (inside) {
-        bool in_range = true;
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          const float q = __fdiv_rn(__fsub_rn(p[i], t.origin[i]), t.voxel_size);
-          const float k = floorf(q);
-          in_range = in_range && k >= -KEY_LIM && k < KEY_LIM;
-          if (in_range) {
-            const float fr = __fsub_rn(q, k);
-            const unsigned long long u = __float2ull_rz(__fmul_rn(fr, 4294967296.0f));
-            fs[i] = u < 0xffffffffull ? u : 0xffffffffull;
-            key = (key << KEY_BITS) | (unsigned long long)((int)k + (1 << 20));
-          }
-        }
-        keep = in_range;
-        out = !in_range;
+        keep = cell_key(p, t.origin, t.voxel_size, key, [&](int i, float q, float k) {
+          const unsigned long long u = __float2ull_rz(__fmul_rn(__fsub_rn(q, k), 4294967296.0f));
+          fs[i] = u < 0xffffffffull ? u : 0xffffffffull;
+        });
+        out = !keep;
         if (keep)
 #pragma unroll
           for (int i = 0; i < 3; ++i)
@@ -241,7 +228,7 @@ __global__ void __launch_bounds__(EX_THREADS) voxel_write_kernel(const LrfVoxelT
   const double fden = __dmul_rn(cnt, 4294967296.0), cden = __dmul_rn(cnt, 16777216.0);
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
-    const long long k = (long long)((key >> (KEY_BITS * (2 - a))) & ((1ull << KEY_BITS) - 1)) - (1 << 20);
+    const long long k = (long long)cell_field(key, a) - (1 << 20);
     const double pos = __dadd_rn((double)k, __ddiv_rn(__ull2double_rn(v[1 + a]), fden));
     xyz[3 * i + a] = __double2float_rn(__dadd_rn((double)t.origin[a], __dmul_rn(pos, (double)t.voxel_size)));
     const double c = __dadd_rn(__dmul_rn(__ddiv_rn(__ull2double_rn(v[4 + a]), cden), 255.0), 0.5);
@@ -250,74 +237,51 @@ __global__ void __launch_bounds__(EX_THREADS) voxel_write_kernel(const LrfVoxelT
   count[i] = n < 2147483647ull ? (int)n : 2147483647;
 }
 
-// The extract's scratch: the sort's buffers of the slots' keys and indices, then the sort's temporary storage.  With a
-// null base only the size is computed.
-struct ExtractScratch {
-  KeySlotSort pairs;
-  void* temp;
-  size_t temp_bytes;
-  size_t total;
-};
-
-cudaError_t extract_scratch(void* base, long long cap, ExtractScratch& x) {
-  ScratchCarver c(base);
-  x.pairs.carve(c, cap);
-  const cudaError_t e = KeySlotSort::temp_bytes(cap, x.temp_bytes);
-  x.temp = c.take(x.temp_bytes, 256);
-  x.total = c.size(256);
-  return e;
-}
-
 }  // namespace
 
 cudaError_t launch_ray_opacity(const float* w, long long n, int S, long long n_views, const float* blend,
                                long long blend_stride, int accumulate, float* acc, cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
-  const unsigned blocks = (unsigned)((n + OP_RAYS - 1) / OP_RAYS);
-  ray_opacity_kernel<<<blocks, OP_RAYS, 0, stream>>>(w, n, S, n / n_views, blend, blend_stride, accumulate, acc);
+  ray_opacity_kernel<<<item_ctas(n, OP_RAYS), OP_RAYS, 0, stream>>>(w, n, S, n / n_views, blend, blend_stride,
+                                                                    accumulate, acc);
   return cudaGetLastError();
 }
 
 cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, cudaStream_t stream) {
   if (f.n_rays == 0) return cudaSuccess;
-  const unsigned blocks = (unsigned)((f.n_rays + PT_THREADS - 1) / PT_THREADS);
-  frame_points_kernel<<<blocks, PT_THREADS, 0, stream>>>(f, t);
+  frame_points_kernel<<<item_ctas(f.n_rays, PT_THREADS), PT_THREADS, 0, stream>>>(f, t);
   return cudaGetLastError();
 }
 
 cudaError_t launch_frame_colours(const LrfColourFrame& f, const float* xyz, const float* normals, long long n,
                                  unsigned long long* sums, cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
-  frame_colours_kernel<<<(unsigned)((n + CO_THREADS - 1) / CO_THREADS), CO_THREADS, 0, stream>>>(f, xyz, normals, n,
-                                                                                               sums);
+  frame_colours_kernel<<<item_ctas(n, CO_THREADS), CO_THREADS, 0, stream>>>(f, xyz, normals, n, sums);
   return cudaGetLastError();
 }
 
 cudaError_t launch_colour_extract(const unsigned long long* sums, long long n, unsigned char* rgb, int* count,
                                   cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
-  colour_extract_kernel<<<(unsigned)((n + CO_THREADS - 1) / CO_THREADS), CO_THREADS, 0, stream>>>(sums, n, rgb, count);
+  colour_extract_kernel<<<item_ctas(n, CO_THREADS), CO_THREADS, 0, stream>>>(sums, n, rgb, count);
   return cudaGetLastError();
 }
 
-cudaError_t voxel_extract_scratch_bytes(long long cap, size_t& bytes) {
-  ExtractScratch x;
-  const cudaError_t e = extract_scratch(nullptr, cap, x);
-  bytes = x.total;
-  return e;
-}
+// the sort's buffers of the slots' keys and indices, then its temporary storage
+ExtractScratch voxel_extract_scratch(long long cap) { return ExtractScratch{cap, 0, 0}; }
 
 cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, float* xyz, unsigned char* rgb,
                                  int* count, long long* n_out, void* scratch, cudaStream_t stream) {
-  ExtractScratch x;
-  cudaError_t e = extract_scratch(scratch, t.capacity, x);
+  ExtractScratch x = voxel_extract_scratch(t.capacity);
+  cudaError_t e = x.carve(scratch);
   if (e != cudaSuccess) return e;
-  const unsigned blocks = (unsigned)((t.capacity + EX_THREADS - 1) / EX_THREADS);
-  voxel_keys_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, (unsigned long long)min_count, x.pairs.keys(),
-                                                        x.pairs.slots());
+  const unsigned blocks = item_ctas(t.capacity, EX_THREADS);
+  voxel_keys_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, (unsigned long long)min_count, x.pairs[0].keys(),
+                                                        x.pairs[0].slots());
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  if ((e = x.pairs.sort(t.capacity, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
-  voxel_write_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, x.pairs.keys(), x.pairs.slots(), xyz, rgb, count, n_out);
+  if ((e = x.pairs[0].sort(t.capacity, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  voxel_write_kernel<<<blocks, EX_THREADS, 0, stream>>>(t, x.pairs[0].keys(), x.pairs[0].slots(), xyz, rgb, count,
+                                                         n_out);
   return cudaGetLastError();
 }
 

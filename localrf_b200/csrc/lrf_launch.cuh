@@ -1,6 +1,6 @@
 // lrf_launch.cuh -- the launch conventions the kernel files share: the fixed-order fp64 CTA sum, the CTA count of a
-// capped grid-stride launch, the carving of a caller's scratch block, and the one-time opt-in to large dynamic shared
-// memory and choice of the shared-memory carveout.
+// capped grid-stride launch and of a one-thread-per-item launch, the carving of a caller's scratch block, and the
+// one-time opt-in to large dynamic shared memory and choice of the shared-memory carveout.
 //
 // Not included from lrf_common.cuh or lrf_device.cuh: tests/host_emul compiles those with a host compiler.
 #pragma once
@@ -30,6 +30,9 @@ inline unsigned int cta_count(long long work, long long per_cta, int n_sms, int 
   const long long want = (work + per_cta - 1) / per_cta, cap = (long long)n_sms * per_sm;
   return (unsigned int)(want < 1 ? 1 : (want < cap ? want : cap));
 }
+
+// CTAs of `threads` for a kernel with one thread per item of n.  Not capped: these kernels do not loop.
+inline unsigned int item_ctas(long long n, int threads) { return (unsigned int)((n + threads - 1) / threads); }
 
 // Consecutive arrays in a caller's scratch block.  take(bytes, align) returns the next `bytes` from the first offset
 // that is a multiple of `align` (a power of two).  On a null base it only counts: the *_scratch_bytes functions and

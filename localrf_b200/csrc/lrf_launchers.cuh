@@ -2,8 +2,8 @@
 // scratch, prepared and shared-memory blocks, the ingest's resize rule and the extracts' sort.  Each defining file
 // includes this header, so the compiler checks every definition against the declaration its callers use.
 //
-// Declarations, and one small host-side struct (KeySlotSort: the sort's buffer pointers and their accessors); no
-// device code.
+// Declarations, and two small host-side structs (KeySlotSort: the sort's buffer pointers and their accessors;
+// ExtractScratch: an extract's scratch block); no device code.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -129,11 +129,26 @@ struct KeySlotSort {
   cudaError_t sort(long long n, void* temp, size_t temp_bytes, cudaStream_t stream);
 };
 
+// lrf_table.cu: an extract's scratch block, each array from a 256-byte boundary: the KeySlotSort buffers of n pairs,
+// `ints` 32-bit integers of the extract's own, the buffers of a second sort of n2 pairs (n2 = 0: none), then one
+// temporary storage sized for the larger sort.  The C ABI sizes and checks an extract's block with the launcher's.
+struct ExtractScratch {
+  long long n = 0, ints = 0, n2 = 0;
+  KeySlotSort pairs[2];
+  int* index = nullptr;                       // the `ints` integers
+  void* temp = nullptr;
+  size_t temp_bytes = 0;
+  // the whole block with `temp` (the sort-size query needs a device), else the buffers alone: a lower bound of the
+  // whole, known without a device
+  cudaError_t bytes(size_t& total, bool temp) const;
+  cudaError_t carve(void* base);              // points the arrays into `base`
+};
+
 // lrf_export.cu
 cudaError_t launch_ray_opacity(const float* w, long long n, int S, long long n_views, const float* blend,
                                long long blend_stride, int accumulate, float* acc, cudaStream_t stream);
 cudaError_t launch_frame_points(const LrfPointFrame& f, const LrfVoxelTable& t, cudaStream_t stream);
-cudaError_t voxel_extract_scratch_bytes(long long cap, size_t& bytes);
+ExtractScratch voxel_extract_scratch(long long cap);
 cudaError_t launch_voxel_extract(const LrfVoxelTable& t, long long min_count, float* xyz, unsigned char* rgb,
                                  int* count, long long* n_out, void* scratch, cudaStream_t stream);
 cudaError_t launch_frame_colours(const LrfColourFrame& f, const float* xyz, const float* normals, long long n,
@@ -146,7 +161,7 @@ cudaError_t launch_mesh_lattice(const MeshSceneDev& S, const int* lo, const int*
                                 cudaStream_t stream);
 cudaError_t launch_mesh_cells(const MeshSceneDev& S, const int* lo, const int* dims, const float* values,
                               const LrfMeshTable& t, cudaStream_t stream);
-cudaError_t mesh_extract_scratch_bytes(long long cap, long long max_tri, size_t& bytes);
+ExtractScratch mesh_extract_scratch(long long cap, long long max_tri);
 cudaError_t launch_mesh_extract(const LrfMeshTable& t, float* xyz, int* faces, long long* counts, void* scratch,
                                 cudaStream_t stream);
 cudaError_t launch_mesh_normals(const MeshSceneDev& S, const float* xyz, long long n, float* normals, int* owner,
@@ -158,9 +173,7 @@ cudaError_t launch_mesh_components(const int* faces, long long T, long long V, i
 cudaError_t launch_point_components(const float* xyz, long long n, const float* origin, float cell_size,
                                     unsigned long long* keys, int* first, long long cap, int* label,
                                     unsigned long long* size, unsigned long long* stats, cudaStream_t stream);
-// the select's scratch without the sort's temporary storage (known without a device: a lower bound of the whole)
-size_t components_select_buffer_bytes(long long n);
-cudaError_t components_select_scratch_bytes(long long n, size_t& bytes);
+ExtractScratch components_select_scratch(long long n);
 cudaError_t launch_components_select(const int* label, const unsigned long long* size, long long n, long long keep,
                                      long long min_size, int* new_index, int* rank, long long* sizes_sorted,
                                      long long* counts, void* scratch, cudaStream_t stream);

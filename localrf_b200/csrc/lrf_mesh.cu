@@ -228,7 +228,7 @@ __global__ void __launch_bounds__(MC_THREADS) mesh_cells_kernel(const __grid_con
                                                                 const LrfMeshTable t) {
   const int nx = d.x - 1, ny = d.y - 1, nz = d.z - 1;
   const long long e = (long long)blockIdx.x * MC_THREADS + threadIdx.x;
-  if (e >= (long long)nx * ny * nz || claim_count(t.stats) > ((unsigned long long)t.capacity >> 1)) return;
+  if (e >= (long long)nx * ny * nz || table_full(t.stats, t.capacity)) return;
   const int cz = (int)(e % nz), cy = (int)((e / nz) % ny), cx = (int)(e / ((long long)nz * ny));
   float v[8];
   int cube = 0;
@@ -341,79 +341,50 @@ __global__ void __launch_bounds__(MC_THREADS) mesh_normals_kernel(const __grid_c
   owner[i] = mesh_owner(S, x, y, norm);
 }
 
-// The extract's scratch: the sort's buffers of the edge keys and slots, the vertex rank of each slot, the sort's
-// buffers of the triangle keys and ids, then the sorts' temporary storage, for the larger of the two.  With a null base
-// only the size is computed.
-struct MeshScratch {
-  KeySlotSort edges, tris;
-  int* rank;
-  void* temp;
-  size_t temp_bytes;
-  size_t total;
-};
-
-cudaError_t mesh_scratch(void* base, long long cap, long long max_tri, MeshScratch& x) {
-  ScratchCarver c(base);
-  x.edges.carve(c, cap);
-  x.rank = c.take<int>(cap * 4, 256);
-  x.tris.carve(c, max_tri);
-  size_t a = 0, b = 0;
-  cudaError_t e = KeySlotSort::temp_bytes(cap, a);
-  if (e == cudaSuccess) e = KeySlotSort::temp_bytes(max_tri, b);
-  x.temp_bytes = a > b ? a : b;
-  x.temp = c.take(x.temp_bytes, 256);
-  x.total = c.size(256);
-  return e;
-}
-
-unsigned int blocks_of(long long n) { return (unsigned int)((n + MC_THREADS - 1) / MC_THREADS); }
-
 }  // namespace
 
 cudaError_t launch_mesh_lattice(const MeshSceneDev& S, const int* lo, const int* dims, float* values,
                                 cudaStream_t stream) {
-  mesh_lattice_kernel<<<blocks_of((long long)dims[0] * dims[1] * dims[2]), MC_THREADS, 0, stream>>>(
+  mesh_lattice_kernel<<<item_ctas((long long)dims[0] * dims[1] * dims[2], MC_THREADS), MC_THREADS, 0, stream>>>(
       S, make_int3(lo[0], lo[1], lo[2]), make_int3(dims[0], dims[1], dims[2]), values);
   return cudaGetLastError();
 }
 
 cudaError_t launch_mesh_cells(const MeshSceneDev& S, const int* lo, const int* dims, const float* values,
                               const LrfMeshTable& t, cudaStream_t stream) {
-  mesh_cells_kernel<<<blocks_of((long long)(dims[0] - 1) * (dims[1] - 1) * (dims[2] - 1)), MC_THREADS, 0, stream>>>(
+  const long long cells = (long long)(dims[0] - 1) * (dims[1] - 1) * (dims[2] - 1);
+  mesh_cells_kernel<<<item_ctas(cells, MC_THREADS), MC_THREADS, 0, stream>>>(
       S, make_int3(lo[0], lo[1], lo[2]), make_int3(dims[0], dims[1], dims[2]), values, t);
   return cudaGetLastError();
 }
 
-cudaError_t mesh_extract_scratch_bytes(long long cap, long long max_tri, size_t& bytes) {
-  MeshScratch x;
-  const cudaError_t e = mesh_scratch(nullptr, cap, max_tri, x);
-  bytes = x.total;
-  return e;
-}
+// the sort's buffers of the edge keys and slots, the vertex rank of each slot, the sort's buffers of the triangle keys
+// and ids, then the sorts' temporary storage
+ExtractScratch mesh_extract_scratch(long long cap, long long max_tri) { return ExtractScratch{cap, cap, max_tri}; }
 
 cudaError_t launch_mesh_extract(const LrfMeshTable& t, float* xyz, int* faces, long long* counts, void* scratch,
                                 cudaStream_t stream) {
-  MeshScratch x;
-  cudaError_t e = mesh_scratch(scratch, t.capacity, t.max_triangles, x);
+  ExtractScratch x = mesh_extract_scratch(t.capacity, t.max_triangles);
+  cudaError_t e = x.carve(scratch);
   if (e != cudaSuccess) return e;
-  edge_keys_kernel<<<blocks_of(t.capacity), MC_THREADS, 0, stream>>>(t, x.edges.keys(), x.edges.slots());
+  const KeySlotSort &edges = x.pairs[0], &tris = x.pairs[1];
+  const unsigned edge_ctas = item_ctas(t.capacity, MC_THREADS), tri_ctas = item_ctas(t.max_triangles, MC_THREADS);
+  edge_keys_kernel<<<edge_ctas, MC_THREADS, 0, stream>>>(t, edges.keys(), edges.slots());
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  if ((e = x.edges.sort(t.capacity, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
-  vertex_write_kernel<<<blocks_of(t.capacity), MC_THREADS, 0, stream>>>(t, x.edges.keys(), x.edges.slots(), xyz,
-                                                                        x.rank, counts);
+  if ((e = x.pairs[0].sort(t.capacity, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  vertex_write_kernel<<<edge_ctas, MC_THREADS, 0, stream>>>(t, edges.keys(), edges.slots(), xyz, x.index, counts);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  tri_keys_kernel<<<blocks_of(t.max_triangles), MC_THREADS, 0, stream>>>(t, x.tris.keys(), x.tris.slots());
+  tri_keys_kernel<<<tri_ctas, MC_THREADS, 0, stream>>>(t, tris.keys(), tris.slots());
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  if ((e = x.tris.sort(t.max_triangles, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
-  face_write_kernel<<<blocks_of(t.max_triangles), MC_THREADS, 0, stream>>>(t, x.tris.keys(), x.tris.slots(), x.rank,
-                                                                           faces, counts);
+  if ((e = x.pairs[1].sort(t.max_triangles, x.temp, x.temp_bytes, stream)) != cudaSuccess) return e;
+  face_write_kernel<<<tri_ctas, MC_THREADS, 0, stream>>>(t, tris.keys(), tris.slots(), x.index, faces, counts);
   return cudaGetLastError();
 }
 
 cudaError_t launch_mesh_normals(const MeshSceneDev& S, const float* xyz, long long n, float* normals, int* owner,
                                 cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
-  mesh_normals_kernel<<<blocks_of(n), MC_THREADS, 0, stream>>>(S, xyz, n, normals, owner);
+  mesh_normals_kernel<<<item_ctas(n, MC_THREADS), MC_THREADS, 0, stream>>>(S, xyz, n, normals, owner);
   return cudaGetLastError();
 }
 

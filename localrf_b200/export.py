@@ -41,9 +41,6 @@ from . import _lib
 from .ray_utils import contract
 from .tensorf import _stream
 
-_TABLE_WORDS = 8          # per slot: the key, then count, sum f_x, f_y, f_z, sum r, g, b
-
-
 def _cuda_device(local_tensorfs):
     dev = local_tensorfs.blending_weights.device
     if dev.type != "cuda":
@@ -66,29 +63,49 @@ def _extract_scratch(nbytes, what, dev):
     return torch.empty(nbytes, dtype=torch.uint8, device=dev)
 
 
+def _check_overflow(n, limit, what, param, size):
+    """RuntimeError when an export's table overflowed (n > limit, `what` with {} the limit), naming `param` to raise."""
+    if n > limit:
+        raise RuntimeError(f"localrf_b200: the {what.format(limit)}; raise `{param}` or `{size}`")
+
+
+# (stats, counts) at the end of each export's int64 block: the voxel table's stats (kept, out of range, occupied) and
+# lrf_voxel_extract's voxel count; the mesh table's (edge claims, triangles appended) and lrf_mesh_extract's vertex and
+# triangle counts; the components' stats and lrf_components_select's counts
+_VOXEL_TAIL, _MESH_TAIL, _COMPONENTS_TAIL = (3, 1), (2, 2), (2, 4)
+
+
+def _int64_block(dev, words):
+    """One zeroed int64 device block cut into consecutive views of `words` words each -> (block, views)."""
+    block = torch.zeros(sum(words), dtype=torch.int64, device=dev)
+    return block, block.split(words)
+
+
+def _tail(block, tail):
+    """The (stats, counts) `tail` at the end of `block` -> (both, to read with one .tolist(); stats; counts)."""
+    words = block[block.numel() - sum(tail):]
+    return words, words[:tail[0]], words[tail[0]:]
+
+
 def _voxel_table(capacity, voxel_size, origin, dev):
-    """A zeroed LrfVoxelTable in one int64 device block: keys [capacity], sums [capacity][7], stats [4] (kept,
-    out of range, occupied, and the voxel count lrf_voxel_extract writes) -> (struct, block)."""
-    store = torch.zeros(_TABLE_WORDS * capacity + 4, dtype=torch.int64, device=dev)
-    table = _lib.LrfVoxelTable(capacity=capacity, voxel_size=float(voxel_size), keys=store.data_ptr(),
-                               sums=store.data_ptr() + 8 * capacity, stats=store.data_ptr() + 8 * _TABLE_WORDS * capacity)
+    """A zeroed LrfVoxelTable in one int64 device block: keys [capacity], sums [capacity][7] (count, sum f_x, f_y,
+    f_z, sum r, g, b), then _VOXEL_TAIL -> (struct, block)."""
+    block, (keys, sums, stats, _) = _int64_block(dev, (capacity, 7 * capacity) + _VOXEL_TAIL)
+    table = _lib.LrfVoxelTable(capacity=capacity, voxel_size=float(voxel_size), keys=keys.data_ptr(),
+                               sums=sums.data_ptr(), stats=stats.data_ptr())
     table.origin[:] = [float(v) for v in origin]
-    return table, store
+    return table, block
 
 
 def _mesh_table(capacity, max_triangles, dev):
     """A zeroed LrfMeshTable in one int64 device block: edge keys [capacity], vertices [capacity][3] float32,
-    triangle keys [max_triangles], triangle slots [max_triangles][3] int32, stats [2], then two words for the counts
-    lrf_mesh_extract writes -> (struct, block)."""
-    words = capacity + (3 * capacity + 1) // 2 + max_triangles + (3 * max_triangles + 1) // 2
-    store = torch.zeros(words + 4, dtype=torch.int64, device=dev)
-    base = store.data_ptr()
-    keys_at, verts_at = base, base + 8 * capacity
-    tri_keys_at = verts_at + 8 * ((3 * capacity + 1) // 2)
-    tri_slots_at = tri_keys_at + 8 * max_triangles
-    table = _lib.LrfMeshTable(capacity=capacity, max_triangles=max_triangles, keys=keys_at, verts=verts_at,
-                              tri_keys=tri_keys_at, tri_slots=tri_slots_at, stats=base + 8 * words)
-    return table, store
+    triangle keys [max_triangles], triangle slots [max_triangles][3] int32, then _MESH_TAIL -> (struct, block)."""
+    words = (capacity, (3 * capacity + 1) // 2, max_triangles, (3 * max_triangles + 1) // 2) + _MESH_TAIL
+    block, views = _int64_block(dev, words)
+    keys, verts, tri_keys, tri_slots, stats, _ = (v.data_ptr() for v in views)
+    table = _lib.LrfMeshTable(capacity=capacity, max_triangles=max_triangles, keys=keys, verts=verts,
+                              tri_keys=tri_keys, tri_slots=tri_slots, stats=stats)
+    return table, block
 
 
 def _chunk_rays(lt, weights_budget, dev):
@@ -157,7 +174,7 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
     lib = _lib.lib()
 
     table, store = _voxel_table(capacity, voxel_size, origin, dev)
-    stats = store[-4:]
+    tail, _, counts = _tail(store, _VOXEL_TAIL)
     n_fields = len(lt.tensorfs)
     w2rf = torch.stack([w.detach().to(dev, torch.float32) for w in lt.world2rf]).contiguous()
     blend_rows = lt.blending_weights.detach().to(dev, torch.float32).contiguous()
@@ -183,12 +200,11 @@ def point_cloud(local_tensorfs, W, H, view_ids=None, test_ids=(), voxel_size=1 /
         rgb8 = torch.empty(capacity, 3, dtype=torch.uint8, device=dev)
         count = torch.empty(capacity, dtype=torch.int32, device=dev)
         _lib.check(lib.lrf_voxel_extract(C.byref(table), int(min_count), xyz.data_ptr(), rgb8.data_ptr(),
-                                         count.data_ptr(), stats.data_ptr() + 24, scratch.data_ptr(), scratch_bytes,
-                                         stream))
-        kept, out_of_range, occupied, P = stats.tolist()
-    if occupied > capacity // 2:
-        raise RuntimeError(f"localrf_b200: the scene has more voxels than the table holds (capacity / 2 = "
-                           f"{capacity // 2}); raise `capacity` or `voxel_size`")
+                                         count.data_ptr(), counts.data_ptr(), scratch.data_ptr(),
+                                         scratch_bytes, stream))
+        kept, out_of_range, occupied, P = tail.tolist()
+    _check_overflow(occupied, capacity // 2, "scene has more voxels than the table holds (capacity / 2 = {})",
+                    "capacity", "voxel_size")
     return dict(xyz=xyz[:P].clone(), rgb=rgb8[:P].clone(), count=count[:P].clone(), n_rays=n_rays, n_kept=kept,
                 n_out_of_range=out_of_range)
 
@@ -254,7 +270,7 @@ def mesh(local_tensorfs, voxel_size=1 / 128, level=0.005, origin=(0, 0, 0), max_
         raise ValueError("the lattice indices exceed [-2^19, 2^19): raise `voxel_size` or move `origin`")
 
     table, store = _mesh_table(capacity, max_triangles, dev)
-    tail = store[-4:]                                             # stats (2) and counts (2)
+    _, _, counts = _tail(store, _MESH_TAIL)
     values = torch.empty((brick + 1) ** 3, dtype=torch.float32, device=dev)
     dims = (C.c_int32 * 3)(brick + 1, brick + 1, brick + 1)
     with torch.no_grad(), torch.cuda.device(dev):
@@ -267,16 +283,14 @@ def mesh(local_tensorfs, voxel_size=1 / 128, level=0.005, origin=(0, 0, 0), max_
         scratch = _extract_scratch(scratch_bytes, "mesh extract", dev)
         xyz = torch.empty(capacity // 2, 3, dtype=torch.float32, device=dev)
         faces = torch.empty(max_triangles, 3, dtype=torch.int32, device=dev)
-        _lib.check(lib.lrf_mesh_extract(C.byref(table), xyz.data_ptr(), faces.data_ptr(), tail.data_ptr() + 16,
+        _lib.check(lib.lrf_mesh_extract(C.byref(table), xyz.data_ptr(), faces.data_ptr(), counts.data_ptr(),
                                         scratch.data_ptr(), scratch_bytes, stream))
         del scratch
-        n_vert, n_tri = tail[2:].tolist()
-        if n_vert > capacity // 2:
-            raise RuntimeError(f"localrf_b200: the mesh has more vertices than the table holds (capacity / 2 = "
-                               f"{capacity // 2}); raise `capacity` or `voxel_size`")
-        if n_tri > max_triangles:
-            raise RuntimeError(f"localrf_b200: the mesh has more than max_triangles = {max_triangles} triangles; "
-                               "raise `max_triangles` or `voxel_size`")
+        n_vert, n_tri = counts.tolist()
+        _check_overflow(n_vert, capacity // 2, "mesh has more vertices than the table holds (capacity / 2 = {})",
+                        "capacity", "voxel_size")
+        _check_overflow(n_tri, max_triangles, "mesh has more than max_triangles = {} triangles", "max_triangles",
+                        "voxel_size")
         xyz, faces = xyz[:n_vert].clone(), faces[:n_tri].clone()
         del store
         normals = torch.empty(n_vert, 3, dtype=torch.float32, device=dev)
@@ -482,16 +496,16 @@ def keep_components(geometry, keep=0, min_size=0, cell_size=None, origin=(0, 0, 
         xyz = xyz.contiguous()
         label = torch.empty(V, dtype=torch.int32, device=dev)
         size = torch.empty(V, dtype=torch.int64, device=dev)
-        tail = torch.zeros(6, dtype=torch.int64, device=dev)         # counts (4), stats (2)
+        tail, stats, counts = _tail(_int64_block(dev, _COMPONENTS_TAIL)[0], _COMPONENTS_TAIL)
         if faces is not None:
             _lib.check(lib.lrf_mesh_components(faces.data_ptr(), faces.shape[0], V, label.data_ptr(), size.data_ptr(),
-                                               tail.data_ptr() + 32, stream))
+                                               stats.data_ptr(), stream))
         else:
             keys = torch.empty(capacity, dtype=torch.int64, device=dev)
             first = torch.empty(capacity, dtype=torch.int32, device=dev)
             _lib.check(lib.lrf_point_components(xyz.data_ptr(), V, (C.c_float * 3)(*origin), cell_size, keys.data_ptr(),
                                                 first.data_ptr(), capacity, label.data_ptr(), size.data_ptr(),
-                                                tail.data_ptr() + 32, stream))
+                                                stats.data_ptr(), stream))
             del keys, first
         scratch_bytes = lib.lrf_components_select_scratch_bytes(V) if V else 0
         scratch = _extract_scratch(scratch_bytes, "component select", dev) if V else None
@@ -499,15 +513,15 @@ def keep_components(geometry, keep=0, min_size=0, cell_size=None, origin=(0, 0, 
         rank = torch.empty(V, dtype=torch.int32, device=dev)
         sizes = torch.empty(V, dtype=torch.int64, device=dev)
         _lib.check(lib.lrf_components_select(label.data_ptr(), size.data_ptr(), V, keep, min_size, new_index.data_ptr(),
-                                             rank.data_ptr(), sizes.data_ptr(), tail.data_ptr(),
+                                             rank.data_ptr(), sizes.data_ptr(), counts.data_ptr(),
                                              None if scratch is None else scratch.data_ptr(), scratch_bytes, stream))
         del scratch
-        n_rows, _, n_comp, kept_size, stat0, _ = tail.tolist()
+        stat0, _, n_rows, _, n_comp, kept_size = tail.tolist()
         if faces is not None and stat0:
             raise ValueError(f"geometry['faces'] has {stat0} triangles with a vertex index outside [0, {V})")
-        if faces is None and stat0 > capacity // 2:
-            raise RuntimeError(f"localrf_b200: the cloud has more cells than the table holds (capacity / 2 = "
-                               f"{capacity // 2}); raise `capacity` or `cell_size`")
+        if faces is None:
+            _check_overflow(stat0, capacity // 2, "cloud has more cells than the table holds (capacity / 2 = {})",
+                            "capacity", "cell_size")
         rows = _rows_at(new_index, n_rows)
         out = {}
         for k, v in geometry.items():
