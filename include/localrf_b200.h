@@ -824,9 +824,10 @@ size_t lrf_components_select_scratch_bytes(int64_t n);
  * 0, i < keep.  Device outputs: sizes_sorted [n] rows [0, counts[2]) the size of every component in rank order;
  * new_index [n] -1 for a vertex of a dropped component, else its position among the kept vertices in their original
  * order; rank [n] rows [0, counts[0]) the rank of each kept vertex's component, in that order; counts [4] the kept
- * vertices, kept components, all components and the sum of the kept sizes.  Sizes above 2^31 - 1 rank as 2^31 - 1,
- * and a vertex whose label is not a root in [0, n) is dropped.  Two CUB radix sorts and integer atomics: bitwise
- * repeatable.  With n = 0 only counts (zeros) is written and scratch is not read.
+ * vertices, kept components, all components and the sum of the kept sizes.  Sizes above 2^31 - 1 rank as 2^31 - 1
+ * and negative sizes as 0 (and are reported and summed so), and a vertex whose label is not a root in [0, n) is
+ * dropped.  Two CUB radix sorts and integer atomics: bitwise repeatable.  With n = 0 only counts (zeros) is written
+ * and scratch is not read.
  * LRF_ERR_INVALID before any device work for n outside [0, 2^31), keep or min_size < 0, NULL or misaligned arrays,
  * and scratch that is NULL, not 256-byte aligned or smaller than lrf_components_select_scratch_bytes(n). */
 int lrf_components_select(const int32_t *label, const int64_t *size, int64_t n, int64_t keep, int64_t min_size,

@@ -1114,7 +1114,7 @@ int lrf_components_select(const int32_t* label, const int64_t* size, int64_t n, 
                                          "scratch_bytes is smaller than lrf_components_select_scratch_bytes(n)");
     if (rc != LRF_OK) return rc;
   }
-  return cuda_status(lrf::launch_components_select((const int*)label, (const unsigned long long*)size, n, keep,
+  return cuda_status(lrf::launch_components_select((const int*)label, (const long long*)size, n, keep,
                                                    min_size, (int*)new_index, (int*)rank, (long long*)sizes_sorted,
                                                    (long long*)counts, scratch, (cudaStream_t)stream),
                      "components_select");

@@ -171,10 +171,10 @@ __global__ void __launch_bounds__(CC_THREADS) cell_link_kernel(const unsigned lo
   }
 }
 
-// sort input: the rank key (2^31 - 1 - size) << 31 | v at each root v (label[v] == v), NO_KEY (sorted last) at the
-// other vertices; comp_rank[v] = -1 and counts = 0 until the later launches write them
+// sort input: the rank key (2^31 - 1 - size) << 31 | v at each root v (label[v] == v), size clamped to [0, 2^31 - 1],
+// NO_KEY (sorted last) at the other vertices; comp_rank[v] = -1 and counts = 0 until the later launches write them
 __global__ void __launch_bounds__(CC_THREADS) rank_keys_kernel(const int* __restrict__ label,
-                                                               const unsigned long long* __restrict__ size, long long n,
+                                                               const long long* __restrict__ size, long long n,
                                                                unsigned long long* keys, unsigned int* slots,
                                                                int* comp_rank, long long* counts) {
   const long long v = (long long)blockIdx.x * CC_THREADS + threadIdx.x;
@@ -182,8 +182,9 @@ __global__ void __launch_bounds__(CC_THREADS) rank_keys_kernel(const int* __rest
   if (v >= n) return;
   unsigned long long key = NO_KEY;
   if (__ldg(label + v) == (int)v) {
-    const unsigned long long s = __ldg(size + v);
-    key = ((SIZE_MAX31 - (s < SIZE_MAX31 ? s : SIZE_MAX31)) << 31) | (unsigned long long)v;
+    const long long s = __ldg(size + v);
+    const unsigned long long c = s <= 0 ? 0 : s < (long long)SIZE_MAX31 ? (unsigned long long)s : SIZE_MAX31;
+    key = ((SIZE_MAX31 - c) << 31) | (unsigned long long)v;
   }
   keys[v] = key;
   slots[v] = (unsigned int)v;
@@ -278,7 +279,7 @@ cudaError_t launch_point_components(const float* xyz, long long n, const float* 
 // the sort's key and index buffers, the rank of each root, then the sort's temporary storage
 ExtractScratch components_select_scratch(long long n) { return ExtractScratch{n, n, 0}; }
 
-cudaError_t launch_components_select(const int* label, const unsigned long long* size, long long n, long long keep,
+cudaError_t launch_components_select(const int* label, const long long* size, long long n, long long keep,
                                      long long min_size, int* new_index, int* rank, long long* sizes_sorted,
                                      long long* counts, void* scratch, cudaStream_t stream) {
   if (n == 0) return cudaMemsetAsync(counts, 0, 4 * sizeof(long long), stream);

@@ -174,7 +174,7 @@ cudaError_t launch_point_components(const float* xyz, long long n, const float* 
                                     unsigned long long* keys, int* first, long long cap, int* label,
                                     unsigned long long* size, unsigned long long* stats, cudaStream_t stream);
 ExtractScratch components_select_scratch(long long n);
-cudaError_t launch_components_select(const int* label, const unsigned long long* size, long long n, long long keep,
+cudaError_t launch_components_select(const int* label, const long long* size, long long n, long long keep,
                                      long long min_size, int* new_index, int* rank, long long* sizes_sorted,
                                      long long* counts, void* scratch, cudaStream_t stream);
 

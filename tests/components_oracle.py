@@ -42,9 +42,69 @@ def cells(xyz, origin, cell_size):
         k = np.floor((x - np.asarray(origin, f32)) / f32(cell_size))
         ok = np.all((k >= -KEY_LIM) & (k < KEY_LIM), axis=1)
     ki = np.where(ok[:, None], k, 0).astype(np.int64)
-    u = (ki + KEY_LIM).astype(np.uint64)
-    key = (u[:, 0] << np.uint64(2 * KEY_BITS)) | (u[:, 1] << np.uint64(KEY_BITS)) | u[:, 2]
-    return ok, ki, key
+    return ok, ki, cell_keys(ki)
+
+
+def cell_keys(k):
+    """The keys of cells k [m, 3] (each k_a in [-2^20, 2^20)), as cell_key packs them."""
+    u = (np.asarray(k, np.int64).reshape(-1, 3) + KEY_LIM).astype(np.uint64)
+    return (u[:, 0] << np.uint64(2 * KEY_BITS)) | (u[:, 1] << np.uint64(KEY_BITS)) | u[:, 2]
+
+
+def probe_start(key):
+    """splitmix64's finaliser in uint64 arithmetic (wrapping products): the probe start of each key, as lrf_table.cuh's
+    probe_start."""
+    x = np.asarray(key, np.uint64)
+    with np.errstate(over="ignore"):
+        x = x ^ (x >> np.uint64(30))
+        x = x * np.uint64(0xbf58476d1ce4e5b9)
+        x = x ^ (x >> np.uint64(27))
+        x = x * np.uint64(0x94d049bb133111eb)
+        return x ^ (x >> np.uint64(31))
+
+
+def colliding_cells(capacity, slot, lo, hi):
+    """The cells k with lo <= k < hi (per axis) whose probe starts at `slot` of a table of `capacity`, in
+    lexicographic order, int64 [m, 3]."""
+    axes = [np.arange(a, b, dtype=np.int64) for a, b in zip(lo, hi)]
+    k = np.stack(np.meshgrid(*axes, indexing="ij"), -1).reshape(-1, 3)
+    return k[(probe_start(cell_keys(k)) & np.uint64(capacity - 1)) == np.uint64(slot)]
+
+
+def table_ok(keys, first, xyz, origin, cell_size, capacity):
+    """Checks the cell table keys / first [capacity] that lrf_point_components left for xyz: the tags are exactly the
+    keys of the in-range cells plus one, each once; first[slot] is the lowest point of the slot's cell, and
+    0x7fffffff at an empty slot; each key sits on its probe path, every slot from probe_start(key) & (capacity - 1) up
+    to its own (wrapping past the last) occupied.  -> True, or AssertionError naming what is wrong."""
+    tags = np.asarray(keys).view(np.uint64).reshape(-1)
+    first = np.asarray(first, np.int64).reshape(-1)
+    assert len(tags) == len(first) == capacity, "the table is not `capacity` slots"
+    ok, _, key = cells(xyz, origin, cell_size)
+    idx = np.nonzero(ok)[0]
+    uniq, inv = np.unique(key[idx], return_inverse=True)
+    low = np.full(len(uniq), len(ok), np.int64)
+    np.minimum.at(low, inv, idx)
+    occ = tags != 0
+    slots = np.nonzero(occ)[0]
+    held = tags[slots] - np.uint64(1)
+    order = np.argsort(held)
+    assert np.array_equal(held[order], uniq), "the table's keys are not the cells' keys, each once"
+    assert np.array_equal(first[slots[order]], low), "first[slot] is not the lowest point of the slot's cell"
+    assert (first[~occ] == 0x7fffffff).all(), "an empty slot's first is not 0x7fffffff"
+    if len(slots) == 0:
+        return True
+    assert not occ.all(), "no empty slot"
+    e0 = int(np.nonzero(~occ)[0][0])
+    j = np.arange(capacity)
+    rot = np.roll(occ, -(e0 + 1))                        # position j is slot (e0 + 1 + j) mod capacity
+    last_empty = np.maximum.accumulate(np.where(rot, -1, j))
+    run = j - last_empty - 1                             # occupied slots just before position j (itself excluded)
+    pos = (slots - e0 - 1) % capacity
+    start = (probe_start(held) & np.uint64(capacity - 1)).astype(np.int64)
+    dist = (slots - start) % capacity
+    bad = dist > run[pos]
+    assert not bad.any(), f"key {int(held[bad][0])} at slot {int(slots[bad][0])} is off its probe path"
+    return True
 
 
 def point_components(xyz, origin, cell_size):
@@ -64,8 +124,7 @@ def point_components(xyz, origin, cell_size):
                     continue
                 m = ucell + np.array([dx, dy, dz])
                 inr = np.all((m >= -KEY_LIM) & (m < KEY_LIM), axis=1)
-                mu = (np.where(inr[:, None], m, 0) + KEY_LIM).astype(np.uint64)
-                mk = (mu[:, 0] << np.uint64(2 * KEY_BITS)) | (mu[:, 1] << np.uint64(KEY_BITS)) | mu[:, 2]
+                mk = cell_keys(np.where(inr[:, None], m, 0))
                 pos = np.searchsorted(uniq, mk)
                 hit = inr & (pos < len(uniq))
                 hit[hit] = uniq[pos[hit]] == mk[hit]
@@ -81,7 +140,7 @@ def select(label, size, keep=0, min_size=0):
     label, size = np.asarray(label, np.int64), np.asarray(size, np.int64)
     n = len(label)
     roots = np.nonzero(label == np.arange(n))[0]
-    s = np.minimum(size[roots], 2 ** 31 - 1)
+    s = np.clip(size[roots], 0, 2 ** 31 - 1)                     # negative sizes rank (and sum) as 0
     order = np.lexsort((roots, -s))                              # size descending, then label ascending
     sizes = s[order]
     i = np.arange(len(order))

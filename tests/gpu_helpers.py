@@ -1,4 +1,6 @@
 """Helpers for the -m gpu parity tests (build product modules from golden fixtures)."""
+import math
+
 import numpy as np
 import torch
 
@@ -80,3 +82,37 @@ def oracle_local(lt, fields, ids, view, W, H, world2rf=None, blend=None, floater
                              c2w, np.asarray(world2rf, np.float32).reshape(n, 3),
                              np.asarray(blend, np.float32).reshape(1, n), exposure=expo,
                              floater_thresh=floater_thresh, with_margin=True)
+
+
+def components_scene(n_init_frames=2, grid=64):
+    """The bench's LocalTensorfs scene on the device, its init frames moved apart (the connected-components tests)."""
+    import bench
+    torch.manual_seed(0)
+    lt = bench._scene(L.LocalTensorfs, "cpu", grid, n_init_frames=n_init_frames, density_shift=2.0)
+    g = torch.Generator().manual_seed(3)
+    with torch.no_grad():
+        for i in range(n_init_frames):
+            lt.t_c2w[i].add_(0.3 * torch.randn(3, generator=g))
+    return lt.to("cuda")
+
+
+def components_boxes(rf, boxes, z_half):
+    """relu density S P(x, y) L(z) in the field's frame: P 1 inside the (x0, x1, y0, y1) rectangles, L 1 for |z| <=
+    z_half, ramps one grid cell wide; S puts alpha = 0.005 at P L = 1/2 (test_gpu_mesh's cylinder, as boxes)."""
+    G = rf.gridSize.tolist()[0]
+    cell = 4.0 / (G - 1)
+    c = torch.linspace(-2, 2, G, dtype=torch.float64)
+    yy, xx = torch.meshgrid(c, c, indexing="ij")
+    ramp = lambda d: (0.5 + d / cell).clamp(0, 1)
+    P = torch.zeros(G, G, dtype=torch.float64)
+    for x0, x1, y0, y1 in boxes:
+        P = torch.maximum(P, torch.minimum(ramp(torch.minimum(xx - x0, x1 - xx)), ramp(torch.minimum(yy - y0, y1 - yy))))
+    Lz = ramp(z_half - c.abs())
+    S = -math.log(1 - 0.005) / (float(rf.stepSize) * 0.5)
+    with torch.no_grad():
+        for i in range(3):
+            rf.density_plane[i].zero_()
+            rf.density_line[i].zero_()
+        rf.density_plane[0][0, 0] = P.float().cuda()
+        rf.density_line[0][0, 0, :, 0] = (S * Lz).float().cuda()
+    rf.fea2denseAct = "relu"

@@ -205,6 +205,18 @@ def test_voxel_extract_invalid():
     assert L.lrf_voxel_extract_scratch_bytes(6) == 0 and L.lrf_voxel_extract_scratch_bytes(2 ** 31) == 0
 
 
+def test_voxel_extract_refuses_scratch_smaller_than_its_buffers_without_a_device():
+    """A block smaller than the sort's key and slot buffers (two of 8 and two of 4 bytes per slot, each from a 256-byte
+    boundary) is refused before the sort-size query, which needs a device; alignment is checked first."""
+    L = _lib.lib()
+    buffers = 24 * 1024                                             # the table's 1024 slots
+    call = lambda s, nbytes: L.lrf_voxel_extract(C.byref(_table()), 1, FAKE, FAKE, FAKE, FAKE, s, nbytes, None)
+    for nbytes in (0, 256, buffers - 1):
+        _refused(call(FAKE, nbytes), b"scratch_bytes is smaller than lrf_voxel_extract_scratch_bytes(capacity)")
+    _refused(call(FAKE + 16, 0), b"256-byte aligned")
+    _refused(call(FAKE + 16, buffers - 1), b"256-byte aligned")
+
+
 def test_point_cloud64_agrees_with_ray_points():
     """The float64 reference on hand-built rays of a rotated, translated camera: the same rays kept and the same
     voxels as the float32 restatement, with no ray near a boundary (so none is ambiguous)."""

@@ -3,14 +3,13 @@ lrf_components_select and localrf_b200.export.keep_components) against the scipy
 tests/components_oracle.py bit for bit: labels, sizes, the ranking and selection, new_index and the compacted
 outputs, with canary words after every output buffer."""
 import ctypes as C
-import math
 
 import numpy as np
 import pytest
 import torch
 
 import components_oracle as co
-import localrf_b200 as L
+from gpu_helpers import components_boxes, components_scene
 from localrf_b200 import _lib
 from localrf_b200.export import keep_components, mesh, point_cloud, write_ply
 
@@ -246,42 +245,9 @@ def test_point_table_overflow_raises_and_names_capacity():
 
 
 # ---- through export ------------------------------------------------------------------------------------------------
-def _lt(n_init_frames=2, grid=64):
-    import bench
-    torch.manual_seed(0)
-    lt = bench._scene(L.LocalTensorfs, "cpu", grid, n_init_frames=n_init_frames, density_shift=2.0)
-    g = torch.Generator().manual_seed(3)
-    with torch.no_grad():
-        for i in range(n_init_frames):
-            lt.t_c2w[i].add_(0.3 * torch.randn(3, generator=g))
-    return lt.to("cuda")
-
-
-def _boxes(rf, boxes, z_half):
-    """relu density S P(x, y) L(z) in the field's frame: P 1 inside the (x0, x1, y0, y1) rectangles, L 1 for |z| <=
-    z_half, ramps one grid cell wide; S puts alpha = 0.005 at P L = 1/2 (test_gpu_mesh's cylinder, as boxes)."""
-    G = rf.gridSize.tolist()[0]
-    cell = 4.0 / (G - 1)
-    c = torch.linspace(-2, 2, G, dtype=torch.float64)
-    yy, xx = torch.meshgrid(c, c, indexing="ij")
-    ramp = lambda d: (0.5 + d / cell).clamp(0, 1)
-    P = torch.zeros(G, G, dtype=torch.float64)
-    for x0, x1, y0, y1 in boxes:
-        P = torch.maximum(P, torch.minimum(ramp(torch.minimum(xx - x0, x1 - xx)), ramp(torch.minimum(yy - y0, y1 - yy))))
-    Lz = ramp(z_half - c.abs())
-    S = -math.log(1 - 0.005) / (float(rf.stepSize) * 0.5)
-    with torch.no_grad():
-        for i in range(3):
-            rf.density_plane[i].zero_()
-            rf.density_line[i].zero_()
-        rf.density_plane[0][0, 0] = P.float().cuda()
-        rf.density_line[0][0, 0, :, 0] = (S * Lz).float().cuda()
-    rf.fea2denseAct = "relu"
-
-
 def test_mesh_floater_is_removed_whole(tmp_path):
-    lt = _lt(grid=128)
-    _boxes(lt.tensorfs[0], [(-0.6, 0.2, -0.5, 0.5), (0.5, 0.7, 0.3, 0.5)], 0.4)   # the scene, and a floater
+    lt = components_scene(grid=128)
+    components_boxes(lt.tensorfs[0], [(-0.6, 0.2, -0.5, 0.5), (0.5, 0.7, 0.3, 0.5)], 0.4)   # the scene, and a floater
     w = lt.world2rf[0].detach().cpu().double().numpy()
     m = mesh(lt, voxel_size=1 / 64, origin=tuple(float(-x) for x in w))
     before = {k: v.clone() for k, v in m.items()}
@@ -313,7 +279,7 @@ def test_mesh_floater_is_removed_whole(tmp_path):
 
 
 def test_point_cloud_components_equal_the_restatement():
-    lt = _lt(n_init_frames=3)
+    lt = components_scene(n_init_frames=3)
     vs = 1 / 128
     cloud = point_cloud(lt, 64, 48, voxel_size=vs, min_acc=0.05, capacity=1 << 16)
     xyz = cloud["xyz"].cpu().numpy()

@@ -233,6 +233,14 @@ def test_brick_table_and_output_refusals():
     _err(L.lrf_mesh_extract(C.byref(_table()), FAKE, FAKE, FAKE, FAKE + 8, 1 << 30, None), "256-byte")
     assert L.lrf_mesh_extract_scratch_bytes(3, 16) == 0 and L.lrf_mesh_extract_scratch_bytes(16, 0) == 0
     assert L.lrf_mesh_extract_scratch_bytes(16, 1 << 31) == 0
+    # a block smaller than its buffers (the cell sort's 24 bytes per slot, 4 per slot of the extract's own, the
+    # triangle sort's 24 per triangle, each array from a 256-byte boundary) is refused before the sort-size query,
+    # which needs a device; alignment is checked first
+    buffers = 24 * 1024 + 4 * 1024 + 24 * 1024
+    for nbytes in (0, 24 * 1024, buffers - 1):
+        _err(L.lrf_mesh_extract(C.byref(_table()), FAKE, FAKE, FAKE, FAKE, nbytes, None),
+             "scratch_bytes is smaller than lrf_mesh_extract_scratch_bytes(capacity, max_triangles)")
+    _err(L.lrf_mesh_extract(C.byref(_table()), FAKE, FAKE, FAKE, FAKE + 8, buffers - 1, None), "256-byte")
     _err(L.lrf_mesh_normals(C.byref(s), FAKE, -1, FAKE, FAKE, None), "n must")
     _err(L.lrf_mesh_normals(C.byref(s), None, 3, FAKE, FAKE, None), "NULL")
     bad = _valid_field()
