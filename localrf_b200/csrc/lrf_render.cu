@@ -595,24 +595,33 @@ render_kernel_t(const FieldDev F, const BatchDev B, const int nprod) {
       float sc[2][3];
       mlp_layers23(acc, tail, prep_a + (PE ? PE_B2HI : PREP_B2HI), prep_a + (PE ? PE_B2LO : PREP_B2LO), sc);
       // -- composite (tensorBase.py:632): w * rgb into the ray's fixed-point accumulators -------------
+      // The quad's 2 rows x 3 channels are spread over its four lanes (all four hold the same sums): lane q
+      // takes items q and q + 4 (row item / 3, channel item % 3).  Then one lane per row drops the row from
+      // its ray's pending count.
+      const unsigned char* mslot = smem + L.mslot + b * TM + 64 * h;
+      const float* mw = reinterpret_cast<const float*>(smem + L.mw) + b * TM + 64 * h;
+      const int slot0 = mslot[wg_row(0)], slot1 = mslot[wg_row(1)];
 #pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int row = 64 * h + wg_row(j);
-        const int my_slot = smem[L.mslot + b * TM + row];
-        if (q != 0 || my_slot == 0xFF) continue;
-        const float my_w = reinterpret_cast<const float*>(smem + L.mw)[b * TM + row];
+      for (int r = 0; r < 2; ++r) {
+        const int it = q + 4 * r, j = it >= 3 ? 1 : 0, c = it - 3 * j;
+        const int my_slot = j ? slot1 : slot0;
+        if (it >= 6 || my_slot == 0xFF) continue;
+        const float my_w = mw[wg_row(j)];
         Slot* sl = slots + my_slot;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          float v = sc[j][c];
-          if (PE) v += sl->vterm[c];
-          else v += W3_s[c * W3_LD + FC] * sl->vd[0] + W3_s[c * W3_LD + FC + 1] * sl->vd[1] +
-                    W3_s[c * W3_LD + FC + 2] * sl->vd[2];
-          v += b3_s[c];
-          v = __fdiv_rn(1.0f, 1.0f + expf(-v));
-          atomicAdd(&sl->rgb[c], __float2uint_rn(my_w * v * FIX_SCALE));
-        }
-        __threadfence_block();
+        float v = j ? (c == 0 ? sc[1][0] : c == 1 ? sc[1][1] : sc[1][2])
+                    : (c == 0 ? sc[0][0] : c == 1 ? sc[0][1] : sc[0][2]);
+        if (PE) v += sl->vterm[c];
+        else v += W3_s[c * W3_LD + FC] * sl->vd[0] + W3_s[c * W3_LD + FC + 1] * sl->vd[1] +
+                  W3_s[c * W3_LD + FC + 2] * sl->vd[2];
+        v += b3_s[c];
+        v = __fdiv_rn(1.0f, 1.0f + expf(-v));
+        atomicAdd(&sl->rgb[c], __float2uint_rn(my_w * v * FIX_SCALE));
+      }
+      __threadfence_block();
+      __syncwarp();                                     // the quad's channel adds precede its rows' pending drops
+      const int row_slot = q ? slot1 : slot0;
+      if (q < 2 && row_slot != 0xFF) {
+        Slot* sl = slots + row_slot;
         const int old = atomicSub(&sl->pending, 1);
         if (old == 1) { __threadfence_block(); finalize_slot(B, sl); }
       }
